@@ -1,8 +1,16 @@
 #!/usr/bin/env python
-"""bench.py — compression throughput of the zstd hot path on B200 (BASELINE.json metric).
+"""bench.py — compression throughput of the zstd hot path on H100 (BASELINE.json metric).
 
   python bench.py --gpus N --steps K --warmup W [--config C]            # our CUDA path
   python bench.py --impl reference --steps K --warmup W [--config C]    # reference libzstd on the host cores
+
+--dump-outputs DIR writes what the last timed step returned on rank 0 as .npy files, for comparing two builds output
+for output: frame_sizes.npy (float64, compressed bytes per frame of rank 0), with more than one GPU rank_sizes.npy
+(float64, the bytes each rank contributed to the gathered buffer), compressed.npy (float32: rank 0's compressed bytes, or
+with more than one GPU the gathered buffer; when that holds more than 4 Mi bytes, every byte at a multiple of the
+smallest power-of-two stride that keeps 4 Mi or fewer) and compressed_index.npy (float64, their positions).  The
+positions depend on the output size only through that stride, so two builds whose outputs differ by a few bytes are
+compared at the same positions.
 
 --config selects one of BASELINE.json's workloads (default 2, the one the metric is quoted on):
   2  datagen -g1GB -P50, level 1, one frame per GPU (weak scaling: every rank owns one 1 GiB shard, seed = rank)
@@ -16,13 +24,14 @@ With N > 1 the ranks' compressed buffers are gathered to rank 0 over NCCL inside
 compresses, the last one is waited for before the clock stops).
 """
 import argparse
+import atexit
 import ctypes
 import hashlib
 import json
 import os
 
 # the host path keeps ~10 streams busy (8 wave streams + upload + download): give every one its own hardware
-# queue, else a download can sit behind another wave's kernels (profiles/r1_e2e_timeline.md).  Must be set
+# queue, else a download can sit behind another wave's kernels.  Must be set
 # before the CUDA context exists; INTEGRATION.md tells embedders to do the same.
 os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")
 import subprocess
@@ -103,7 +112,7 @@ def peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "MEASURED_PEAKS.json (burst copy figure: kernels are timed alone)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "fallback: H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
 class ClockSampler:
@@ -117,6 +126,7 @@ class ClockSampler:
         try:
             self.proc = subprocess.Popen(["nvidia-smi", f"--query-gpu={self.Q}", "--format=csv,noheader,nounits", "-lms", "20", "-i", str(self.index)],
                                          stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
+            atexit.register(self.proc.terminate)               # never outlives the benchmark, whatever ends it
             threading.Thread(target=self._read, daemon=True).start()
         except Exception:
             self.proc = None
@@ -340,6 +350,25 @@ def run_reference(args):
 
 
 # ----------------------------------------------------------------------------------------------- our arm
+DUMP_SAMPLE = 4 << 20        # compressed bytes kept by --dump-outputs: 16 MB as float32 + 32 MB of float64 positions
+
+
+def dump_outputs(out_dir, frames, frame_sizes, rank_sizes=None):
+    """What the last timed step returned, as .npy files (module docstring)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    data = np.frombuffer(frames, dtype=np.uint8)
+    stride = 1
+    while data.size > DUMP_SAMPLE * stride:
+        stride *= 2
+    index = np.arange(0, data.size, stride)
+    np.save(os.path.join(out_dir, "frame_sizes.npy"), np.asarray(frame_sizes, dtype=np.float64))
+    if rank_sizes is not None:
+        np.save(os.path.join(out_dir, "rank_sizes.npy"), np.asarray(rank_sizes, dtype=np.float64))
+    np.save(os.path.join(out_dir, "compressed.npy"), data[index].astype(np.float32))
+    np.save(os.path.join(out_dir, "compressed_index.npy"), index.astype(np.float64))
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -434,10 +463,20 @@ def run_ours(args):
     gathered_bytes = bytes(last["gathered"].cpu().numpy()) if (world > 1 and rank == 0) else None
     gathered_sizes = last["sizes"]
     got_dev = bytes(d_dst[(args.steps - 1) & 1 if world > 1 else 0][:csize].cpu().numpy())
+    if args.dump_outputs and rank == 0:
+        if world > 1:
+            dump_outputs(args.dump_outputs, gathered_bytes, frame_sizes, gathered_sizes)
+        else:
+            dump_outputs(args.dump_outputs, got_dev, frame_sizes)
 
     # per-kernel CUDA-event times come from a serial-mode context (one wave, one stream): in the default
-    # mode waves on several streams overlap and a kernel's start->end no longer measures that kernel alone
-    kern = None
+    # mode waves on several streams overlap and a kernel's start->end no longer measures that kernel alone.  A serial call
+    # holds the workspace of its whole input at once (about 10 bytes per input byte): on an 80 GB card it covers the
+    # leading frames up to 2 GiB (config 3: 32 of the 128 frames)
+    kern, kframes, kbytes = None, 0, 0
+    while kframes < wl.nframes and (kframes == 0 or kbytes + wl.sizes[kframes] <= 2 * GiB):
+        kbytes += wl.sizes[kframes]
+        kframes += 1
     if rank == 0:
         os.environ["ZSTDB200_SERIAL"] = "1"
         sctx = zstd_b200.ZSTD_CCtx(device=local)
@@ -445,13 +484,14 @@ def run_ours(args):
         sstats = []
         for i in range(2 + 3):
             if cdict is not None:
-                r = L.ZSTDB200_compressFrames_usingCDict(sctx._h, d_dst[0].data_ptr(), cap, d_src.data_ptr(), wl.offs, wl.sizes, wl.nframes, cdict._h, csz, 1, None)
+                r = L.ZSTDB200_compressFrames_usingCDict(sctx._h, d_dst[0].data_ptr(), cap, d_src.data_ptr(), wl.offs, wl.sizes, kframes, cdict._h, csz, 1, None)
             else:
-                r = L.ZSTDB200_compressFrames(sctx._h, d_dst[0].data_ptr(), cap, d_src.data_ptr(), wl.offs, wl.sizes, wl.nframes, None, 0, csz, wl.level, 1, None)
-            assert not L.ZSTD_isError(r)
+                r = L.ZSTDB200_compressFrames(sctx._h, d_dst[0].data_ptr(), cap, d_src.data_ptr(), wl.offs, wl.sizes, kframes, None, 0, csz, wl.level, 1, None)
+            assert not L.ZSTD_isError(r), L.ZSTD_getErrorName(r)
             if i >= 2:
                 sstats.append(sctx.stats())
         kern = {k: sum(getattr(s, k) for s in sstats) / len(sstats) for k in ("kernel_ms", "cand_ms", "parse_ms", "literals_ms", "sequences_ms", "stitch_ms")}
+        kcsize = sum(csz[:kframes])
         sctx.close()
     torch.cuda.synchronize()
 
@@ -540,17 +580,7 @@ def run_ours(args):
     value = wl.total_input * args.steps / (ms / 1e3) / 1e9
     e2e = wl.total_input * args.steps / e2e_s / 1e9
     dom = max(("cand_ms", "parse_ms", "literals_ms", "sequences_ms", "stitch_ms"), key=lambda k: kern[k])
-    achieved = (size + csize) / (kern[dom] / 1e3) / 1e9
-    # DRAM bytes of that kernel per launch: from the committed ncu capture of this workload (not measured live)
-    traffic, traffic_src = None, None
-    try:
-        with open(os.path.join(ROOT, "profiles", "r2_traffic.json")) as f:
-            tj = json.load(f)
-        k = tj["kernels"][dom.replace("_ms", "")]
-        if args.config == 2 and args.scale == 1.0:
-            traffic, traffic_src = k["dram_read_bytes"] + k["dram_write_bytes"], "profiles/r2_traffic.json (ncu --set full, same workload)"
-    except Exception:
-        pass
+    achieved = (kbytes + kcsize) / (kern[dom] / 1e3) / 1e9
     # CPU baseline on this box: the reference on a bounded sample of the same workload (rank 0's share)
     cpu, ref_csize, ref_bytes = None, None, None
     if zref.have_ref() and not args.no_cpu:
@@ -565,13 +595,13 @@ def run_ours(args):
             "ms_per_step": round(ms / args.steps, 3), "higher_is_better": True, "scaling": wl.scaling, "vs_baseline": None,
             "dtype": "u8", "data": wl.data,
             "config": {"workload": wl.desc, "baseline_config": args.config, "level": wl.level,
-                       "l2": f"{size} input bytes per GPU per step > 126 MB L2 (no reuse between steps)" if size > 126 * MiB else "input smaller than L2",
+                       "l2": f"{size} input bytes per GPU per step > 50 MB L2 (no reuse between steps)" if size > 50 * MiB else "input smaller than L2",
                        "compressed_bytes_rank0": csize, "roundtrip_ok": ok_rt, "gathered_decodes_ok": gather_ok,
                        "size_delta_vs_ref": (round((ours_for_delta - ref_csize) / ref_csize, 5) if (ref_csize and ours_for_delta) else None)},
-            "kernel_ms": dict({k: round(v, 3) for k, v in kern.items()}, mode="serial (ZSTDB200_SERIAL=1): one wave on one stream, CUDA events around each kernel, rank 0's share"),
+            "kernel_ms": dict({k: round(v, 3) for k, v in kern.items()}, mode=f"serial (ZSTDB200_SERIAL=1): one wave on one stream, CUDA events around each kernel, the first {kframes} of rank 0's {wl.nframes} frames ({kbytes} bytes)"),
             "roofline": {"bound": "hbm", "kernel": dom.replace("_ms", ""), "achieved": round(achieved, 1), "peak": hbm, "unit": "GB/s",
-                         "frac": round(achieved / hbm, 4), "peak_source": peak_src, "traffic": traffic, "traffic_source": traffic_src,
-                         "algorithmic_bytes": size + csize, "read_only_frac": round(size / (kern[dom] / 1e3) / 1e9 / hbm, 4)},
+                         "frac": round(achieved / hbm, 4), "peak_source": peak_src,
+                         "algorithmic_bytes": kbytes + kcsize, "read_only_frac": round(kbytes / (kern[dom] / 1e3) / 1e9 / hbm, 4)},
             "cpu_baseline": cpu,
             "e2e": {"value": round(e2e, 3), "unit": "GB/s", "h2d_bytes_per_step": h2d_total, "d2h_bytes_per_step": d2h_total,
                     "api": "ZSTD_compressCCtx(host pinned src/dst)" if (wl.nframes == 1) else ("ZSTDB200_compressFrames_usingCDict" if cdict is not None else "ZSTDB200_compressFrames") + "(host pinned src/dst)"},
@@ -591,7 +621,10 @@ def main():
     ap.add_argument("--scale", type=float, default=1.0, help="shrink the workload (development only; 1.0 = the BASELINE size)")
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--no-decode", action="store_true", help="skip the GPU decompression round trip (configs 2 and 4)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step returned to DIR/*.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         run_reference(args)
     else:

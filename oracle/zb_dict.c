@@ -1,5 +1,5 @@
 /* zb_dict.c — oracle: loading a zstd-format dictionary's entropy tables (TEST INFRASTRUCTURE ONLY).
- * Restates ZSTD_loadCEntropy (/root/reference/lib/compress/zstd_compress.c:4987-5076): Huffman table
+ * Restates ZSTD_loadCEntropy (lib/compress/zstd_compress.c:4987-5076): Huffman table
  * (HUF_readCTable huf_compress.c:292-340, HUF_readStats common/entropy_common.c:236-330 incl. the FSE
  * decoding of the weights, common/fse_decompress.c), three FSE tables (FSE_readNCount
  * entropy_common.c:42-188, FSE_buildCTable), repeat modes (ZSTD_dictNCountRepeat :4973-4985) and the

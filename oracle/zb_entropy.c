@@ -1,6 +1,6 @@
 /* zb_entropy.c — oracle restatement of the reference entropy stage (TEST INFRASTRUCTURE ONLY).
  *
- * Every function names the reference lines it restates (paths relative to /root/reference/lib).
+ * Every function names the reference lines it restates (paths relative to the reference's lib/).
  * Output is meant to be byte-identical with the reference for the same (sequences, literals)
  * when the reference starts from a fresh entropy state (no repeat / treeless modes).
  */

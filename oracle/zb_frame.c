@@ -1,6 +1,6 @@
 /* zb_frame.c — oracle frame driver (TEST INFRASTRUCTURE ONLY): parameter derivation, frame header,
  * block loop and block headers, mirroring what ZSTD_compress / ZSTD_compress_usingDict do around
- * the hot path (/root/reference/lib/compress/zstd_compress.c:5398-5440, :4527-4623, :4626-4672).
+ * the hot path (lib/compress/zstd_compress.c:5398-5440, :4527-4623, :4626-4672).
  */
 #include <string.h>
 #include <stdlib.h>

@@ -2,7 +2,7 @@
  * (TEST INFRASTRUCTURE ONLY; the CUDA kernels in zstd_b200/csrc/zb_match.cu must reproduce it bit-for-bit).
  *
  * What it restates: the greedy single-probe LZ77 parse of ZSTD_compressBlock_fast
- * (/root/reference/lib/compress/zstd_fast.c:192-423) and ZSTD_compressBlock_doubleFast
+ * (lib/compress/zstd_fast.c:192-423) and ZSTD_compressBlock_doubleFast
  * (zstd_double_fast.c:105-323): multiplicative hash of `mls` bytes (zstd_compress_internal.h:821-861), one
  * candidate per bucket, 4-byte verification, repcode-1 probe, backward catch-up (:387-391), forward count
  * (:396), immediate repcode-2 loop (:410-420), step acceleration every 128 bytes without a match

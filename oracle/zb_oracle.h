@@ -4,7 +4,7 @@
  * Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline leg use it, and only as the
  * checker.  It is a plain-C restatement of
  *   (1) the reference's entropy stage (Huffman literals + FSE sequences), byte-exact with
- *       /root/reference/lib/compress/{huf_compress.c,fse_compress.c,zstd_compress_literals.c,
+ *       lib/compress/{huf_compress.c,fse_compress.c,zstd_compress_literals.c,
  *       zstd_compress_sequences.c,zstd_compress.c:2881-3035} given the same seqStore, and
  *   (2) the block-parallel "warp-batch" greedy match-finder the CUDA kernels implement (a
  *       deterministic data-parallel re-formulation of zstd_fast.c:192-423 /

@@ -1,8 +1,10 @@
 """Generates the committed golden fixtures from the compiled reference (run here, where
-/root/reference exists):  python tests/golden/make_golden.py
+the reference is built under oracle/_ref/):  ZSTD_REFERENCE=<reference tree> python tests/golden/make_golden.py
   entropy_vectors.json : (seed, draw) of randomised seqStores -> size + sha256 of the block body the
                          REFERENCE's ZSTD_entropyCompressSeqStore produces
   frames.json          : per input x level: reference compressed size, oracle size + sha256
+  cparams.json         : the reference's ZSTD_getCParams (simple API) per level x source size of
+                         tests/test_oracle_frames.py, and its ZSTD_compressBound per size
   inputs/              : the reference's own golden-compression inputs (tests/golden-compression/*) and
                          dictionaries, copied as test data
 """
@@ -17,11 +19,31 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(HERE))
 import zref  # noqa: E402
 from test_oracle_entropy import make_seqstore, run_both  # noqa: E402
+from test_oracle_frames import BOUND_SIZES, CPARAM_LEVELS, CPARAM_SIZES  # noqa: E402
 
-REF = "/root/reference/tests"
+REF = os.path.join(os.environ.get("ZSTD_REFERENCE", ""), "tests")
+
+
+def cparams():
+    import ctypes
+    R = zref.ref()
+    rows = {}
+    for level in CPARAM_LEVELS:
+        for size in CPARAM_SIZES:
+            out = (ctypes.c_uint * 7)()
+            R.ref_getCParams_simpleApi(level, size, 0, out)
+            rows[f"{level},{size}"] = list(out)
+    bounds = {str(n): R.ZSTD_compressBound(n) for n in BOUND_SIZES}
+    json.dump({"getCParams": rows, "compressBound": bounds}, open(os.path.join(HERE, "cparams.json"), "w"), indent=0)
 
 
 def main():
+    # everything is checked before the first fixture is written: a failed run must not leave them half regenerated
+    if not os.environ.get("ZSTD_REFERENCE") or not os.path.isdir(os.path.join(REF, "golden-compression")):
+        sys.exit("make_golden.py: set ZSTD_REFERENCE to the reference's source tree")
+    if not zref.have_ref():
+        sys.exit("make_golden.py: the compiled reference (oracle/_ref/libzstd_ref.so) is missing: run build() first")
+    cparams()
     vectors = []
     for seed in (11, 12, 13):
         rng = np.random.default_rng(seed)

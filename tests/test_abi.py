@@ -49,6 +49,26 @@ def test_helpers_match_reference_semantics():
             assert bool(L.ZSTD_isError(v)) == bool(R.ZSTD_isError(v))
 
 
+def test_xxh64_matches_the_specification():
+    """The host XXH64 of the content checksums (ZSTDB200_xxh64) against the test helpers' statement of the xxHash
+    specification, its published values, and the reference's ZSTD_XXH64 where that is built."""
+    L = zstd_b200.lib()
+    L.ZSTDB200_xxh64.restype = ctypes.c_ulonglong
+    L.ZSTDB200_xxh64.argtypes = [ctypes.c_char_p, ctypes.c_size_t]
+    assert zref.xxh64(b"") == 0xEF46DB3751D8E999 and zref.xxh64(b"abc") == 0x44BC2CF5AD770999
+    R = None
+    if zref.have_ref():
+        R = zref.ref()
+        R.ZSTD_XXH64.restype = ctypes.c_ulonglong
+        R.ZSTD_XXH64.argtypes = [ctypes.c_char_p, ctypes.c_size_t, ctypes.c_ulonglong]
+    for n in list(range(0, 70)) + [1000, 4096, 70_000, 300_001]:
+        data = zref.random_bytes(n, n)
+        want = zref.xxh64(data)
+        assert L.ZSTDB200_xxh64(data, n) == want, n
+        if R is not None:
+            assert R.ZSTD_XXH64(data, n, 0) == want, n
+
+
 def test_context_lifecycle_without_gpu():
     L = zstd_b200.lib()
     c = L.ZSTD_createCCtx()
@@ -93,10 +113,10 @@ def test_header_is_valid_c99_and_links(tmp_path):
     assert out.split()[0] == "10506" and "too small" in out
 
 
-REF_EXAMPLES = "/root/reference/examples"
+REF_EXAMPLES = os.path.join(zref.ROOT, "oracle", "_ref", "examples")      # objects compiled by `make -C oracle examples`
 
 
-@pytest.mark.skipif(not os.path.isdir(REF_EXAMPLES), reason="reference tree absent (GPU box)")
+@pytest.mark.skipif(not os.path.isdir(REF_EXAMPLES), reason="reference examples not built")
 @pytest.mark.parametrize("example", ["simple_compression.c", "multiple_simple_compression.c", "dictionary_compression.c"])
 def test_reference_examples_compile_and_link_unmodified(tmp_path, example):
     """The reference's own example programs (examples/simple_compression.c:28 ZSTD_compress, multiple_simple_compression.c:74
@@ -110,7 +130,7 @@ def test_reference_examples_compile_and_link_unmodified(tmp_path, example):
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     libdir = os.path.join(root, "zstd_b200")
     exe = tmp_path / "example"
-    cmd = [gcc, "-O1", "-I", "/root/reference/lib", "-I", REF_EXAMPLES, os.path.join(REF_EXAMPLES, example), "-o", str(exe),
+    cmd = [gcc, os.path.join(REF_EXAMPLES, example[:-2] + ".o"), "-o", str(exe),
            "-L", libdir, "-lzstd_b200", "-Wl,-rpath," + libdir, "-L/usr/local/cuda/lib64", "-Wl,-rpath,/usr/local/cuda/lib64"]
     subprocess.check_call(cmd)
     assert os.path.exists(exe)

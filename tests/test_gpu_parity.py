@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box: pytest -m gpu).  Every call goes through the C ABI of
+"""GPU parity tests (run on an H100: pytest -m gpu).  Every call goes through the C ABI of
 libzstd_b200.so.  The CUDA path must be bit-exact with the oracle, every frame must decode with the
 reference decoder (when its prebuilt .so travelled with the repo), sizes must stay within the two-sided bound of
 zref.size_delta_ok of the reference's (the north star's 0.5 % is met on part of the grid only: DESIGN.md section 5)."""
@@ -283,11 +283,14 @@ def test_cdict_errors():
 def _with_checksum(frame: bytes, src: bytes) -> bytes:
     """What a checksummed frame must be, given the same frame without checksum: Content_Checksum_flag set in the frame
     header descriptor and the low 32 bits of XXH64(content, 0) behind the last block (zstd_compress.c:4629, :5297-5303);
-    XXH64 taken from the compiled reference (ZSTD_XXH64, lib/common/xxhash.h)."""
-    R = zref.ref()
-    R.ZSTD_XXH64.restype = ctypes.c_ulonglong
-    R.ZSTD_XXH64.argtypes = [ctypes.c_char_p, ctypes.c_size_t, ctypes.c_ulonglong]
-    h = R.ZSTD_XXH64(src, len(src), 0) & 0xFFFFFFFF
+    XXH64 taken from the compiled reference (ZSTD_XXH64, lib/common/xxhash.h), else from the test helpers' own."""
+    if zref.have_ref():
+        R = zref.ref()
+        R.ZSTD_XXH64.restype = ctypes.c_ulonglong
+        R.ZSTD_XXH64.argtypes = [ctypes.c_char_p, ctypes.c_size_t, ctypes.c_ulonglong]
+        h = R.ZSTD_XXH64(src, len(src), 0) & 0xFFFFFFFF
+    else:
+        h = zref.xxh64(src) & 0xFFFFFFFF
     return frame[:4] + bytes([frame[4] | 4]) + frame[5:] + h.to_bytes(4, "little")
 
 

@@ -2,7 +2,7 @@
 same host+device functions the CUDA kernels call, block after block, and must reproduce the input of frames written by
 the reference encoder (every level, so Huffman treeless / FSE repeat modes, RLE tables, long offsets ...), by this repo's
 oracle, and of the reference's own golden decompression vectors (tests/golden/decompression*, copied from
-/root/reference/tests/golden-decompression*)."""
+the reference tree's tests/golden-decompression*)."""
 import ctypes
 import glob
 import os

@@ -1,7 +1,6 @@
 """Seeded differential fuzz of the oracle against the reference decoder (CPU): structured random inputs whose sizes
 cluster around the 16 KiB parse-segment and 128 KiB block boundaries, all level classes, with and without a zstd-format
-dictionary.  A longer run of the same generator (400 k cases) and its GPU twin (tests/fuzz_gpu.py) are recorded in
-profiles/r1_sanitizer.txt."""
+dictionary.  Its GPU twin is tests/fuzz_gpu.py."""
 import random
 
 import pytest

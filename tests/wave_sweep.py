@@ -33,7 +33,7 @@ def main():
     d_src = torch.frombuffer(bytearray(src), dtype=torch.uint8).cuda()
     base = one(d_src, G, level, {"ZSTDB200_SERIAL": "1"}, iters)
     print(f"serial: best {base[0]:.2f} ms  median {base[1]:.2f} ms  {G/base[0]/1e6:.1f} GB/s  size {base[2]}", flush=True)
-    for wb in (512, 1024, 2048):
+    for wb in (256, 512, 1024, 2048):
         for slots in (3, 4, 6, 8):
             r = one(d_src, G, level, {"ZSTDB200_WAVE_BLOCKS": str(wb), "ZSTDB200_WAVE_SLOTS": str(slots)}, iters)
             same = (r[2], r[3]) == (base[2], base[3])

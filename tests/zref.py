@@ -1,5 +1,5 @@
 """Test helpers: ctypes views of the oracle (oracle/libzb_oracle.so), of the compiled reference
-(oracle/_ref/libzstd_ref.so, present only where /root/reference was available at build time or
+(oracle/_ref/libzstd_ref.so, present only where the reference sources were available at build time or
 the prebuilt file travelled with the repo) and test-data generators.  TEST INFRASTRUCTURE ONLY."""
 import ctypes
 import hashlib
@@ -134,6 +134,48 @@ def have_datagen() -> bool:
 
 def sha(b: bytes) -> str:
     return hashlib.sha256(b).hexdigest()
+
+
+_P1, _P2, _P3, _P4, _P5 = 11400714785074694791, 14029467366897019727, 1609587929392839161, 9650029242287828579, 2870177450012600261
+_M64 = (1 << 64) - 1
+
+
+def _rotl64(x: int, r: int) -> int:
+    return ((x << r) | (x >> (64 - r))) & _M64
+
+
+def _xxh_round(acc: int, lane: int) -> int:
+    return (_rotl64((acc + lane * _P2) & _M64, 31) * _P1) & _M64
+
+
+def xxh64(data: bytes, seed: int = 0) -> int:
+    """XXH64 as the xxHash specification states it (the content checksum of a zstd frame is its low 32 bits); a
+    second implementation next to the product's, for the checksum tests where the compiled reference is absent."""
+    n, p = len(data), 0
+    if n >= 32:
+        v = [(seed + _P1 + _P2) & _M64, (seed + _P2) & _M64, seed & _M64, (seed - _P1) & _M64]
+        lanes = np.frombuffer(data, dtype="<u8", count=(n // 32) * 4).tolist()
+        for i in range(0, len(lanes), 4):
+            v = [_xxh_round(v[j], lanes[i + j]) for j in range(4)]
+        p = (n // 32) * 32
+        h = (_rotl64(v[0], 1) + _rotl64(v[1], 7) + _rotl64(v[2], 12) + _rotl64(v[3], 18)) & _M64
+        for x in v:
+            h = ((h ^ _xxh_round(0, x)) * _P1 + _P4) & _M64
+    else:
+        h = (seed + _P5) & _M64
+    h = (h + n) & _M64
+    while p + 8 <= n:
+        h = (_rotl64(h ^ _xxh_round(0, int.from_bytes(data[p:p + 8], "little")), 27) * _P1 + _P4) & _M64
+        p += 8
+    if p + 4 <= n:
+        h = (_rotl64(h ^ ((int.from_bytes(data[p:p + 4], "little") * _P1) & _M64), 23) * _P2 + _P3) & _M64
+        p += 4
+    while p < n:
+        h = (_rotl64(h ^ ((data[p] * _P5) & _M64), 11) * _P1) & _M64
+        p += 1
+    h = ((h ^ (h >> 33)) * _P2) & _M64
+    h = ((h ^ (h >> 29)) * _P3) & _M64
+    return h ^ (h >> 32)
 
 
 def random_bytes(n: int, seed: int = 0) -> bytes:

@@ -16,10 +16,10 @@ for spec in "$@"; do f=${spec%%:*}; fl=""; [[ "$spec" == *:* ]] && fl=${spec#*:}
 objs=""
 for f in zb_api zb_dict zb_match zb_literals zb_sequences zb_stitch zb_decode; do
   if [ -n "${flags[$f.cu]}" ]; then
-    nvcc -O3 -std=c++17 -lineinfo -gencode arch=compute_100a,code=sm_100a -Xcompiler -fPIC,-fvisibility=hidden -Xptxas -v ${flags[$f.cu]#x} -c $f.cu -o /tmp/zbv_$name/$f.o 2> /tmp/zbv_$name/$f.log
+    nvcc -O3 -std=c++17 -lineinfo -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fvisibility=hidden -Xptxas -v ${flags[$f.cu]#x} -c $f.cu -o /tmp/zbv_$name/$f.o 2> /tmp/zbv_$name/$f.log
     grep "spill" /tmp/zbv_$name/$f.log | grep -v " 0 bytes spill stores, 0 bytes spill loads" | head -4 || true
     objs="$objs /tmp/zbv_$name/$f.o"
   else objs="$objs $base/$f.o"; fi
 done
-nvcc -gencode arch=compute_100a,code=sm_100a -shared -o ../variants/libzstd_b200_$name.so $objs -lcudart
+nvcc -gencode arch=compute_90a,code=sm_90a -shared -o ../variants/libzstd_b200_$name.so $objs -lcudart
 echo built ../variants/libzstd_b200_$name.so

@@ -2,7 +2,7 @@
 order, with executed-instruction and stall-sample counts) with the line table of the same kernel in the cubin
 (`nvdisasm -g -c`).  Inlined device functions are attributed to the innermost line.
    python tools/ncu_lines.py <source.csv> <cubin> <mangled-name-substring> [min_pct]"""
-import csv, re, subprocess, sys, collections
+import csv, os, re, subprocess, sys, collections
 src_csv, cubin, kname = sys.argv[1:4]
 minpct = float(sys.argv[4]) if len(sys.argv) > 4 else 0.8
 rows = list(csv.reader(open(src_csv)))
@@ -31,7 +31,7 @@ for ln in sorted(ins, key=lambda k: (k[0], k[1]) if k else ('', 0)):
     if 100 * ins[ln] / ti < minpct and 100 * smp[ln] / max(ts, 1) < minpct: continue
     f, n = ln if ln else ('?', 0)
     if f not in srcs:
-        try: srcs[f] = open('/root/repo/zstd_b200/csrc/' + f).read().splitlines()
+        try: srcs[f] = open(os.path.join(os.path.dirname(os.path.abspath(__file__)), '..', 'zstd_b200', 'csrc', f)).read().splitlines()
         except Exception: srcs[f] = []
     text = srcs[f][n - 1].strip()[:110] if 0 < n <= len(srcs[f]) else ''
     print(f"{f}:{n:4d} {100*ins[ln]/ti:5.1f}% ins {100*smp[ln]/max(ts,1):5.1f}% smp | {text}")

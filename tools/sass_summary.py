@@ -1,5 +1,5 @@
 """Static SASS summary of the compression / decompression kernels of the current build (no GPU needed):
-   python tools/sass_summary.py > profiles/<tag>_sass_summary.md
+   python tools/sass_summary.py
 Per kernel: registers / shared memory / spills (ptxas), static instruction count and the opcode groups that matter for
 this path (global / shared loads and stores, shared atomics, shuffles, votes, barriers, integer multiply-adds, branches)."""
 import collections, os, re, subprocess, sys
@@ -27,7 +27,7 @@ def ptxas_info():
 
 def main():
     info = ptxas_info()
-    print("# Static SASS summary of the hot kernels (sm_100a, `cuobjdump -sass` of the in-tree objects; `tools/sass_summary.py`)\n")
+    print("# Static SASS summary of the hot kernels (sm_90a, `cuobjdump -sass` of the in-tree objects; `tools/sass_summary.py`)\n")
     print("Dynamic shared memory (the walk's table: 4 bytes per bucket, 48 KiB at level 1) is not in the ptxas figure.\n")
     print("| kernel | regs | static smem | spills | SASS instr | " + " | ".join(g for g, _ in GROUPS) + " |")
     print("|---|---|---|---|---|" + "---|" * len(GROUPS))
@@ -47,8 +47,8 @@ def main():
             short = subprocess.run(["c++filt", name], capture_output=True, text=True).stdout.split("(")[0].replace("void ", "").strip()
             print(f"| `{short}` | {r} | {sm} | {'yes: ' + sp if sp else '0'} | {len(lst)} | " + " | ".join(str(c) for c in cnt) + " |")
     print("\nNo tensor-core (`HMMA`/`UTC*MMA`), TMA (`UBLKCP`) or cluster instructions appear: the path is integer / byte work on")
-    print("shared-memory tables and L2-resident windows (DESIGN.md §5, §10); the Blackwell-specific part of the design is the sizing")
-    print("(148 SMs x 227 KiB of shared memory per SM decide the table sizes and CTAs per SM, 126 MB of L2 hold a wave's working set).")
+    print("shared-memory tables and L2-resident windows (DESIGN.md §5, §10); the GPU-specific part of the design is the sizing")
+    print("(up to 227 KB of shared memory per block decide the table sizes and CTAs per SM on the 132 SMs of an H100).")
 
 
 if __name__ == "__main__":

@@ -1,7 +1,7 @@
 /* zb_api.cu — host driver + C ABI of libzstd_b200.so.
  *
  * Mirrors what the reference does around the per-block hot path:
- *   ZSTD_compress / ZSTD_compressCCtx / ZSTD_compress_usingDict  (/root/reference/lib/compress/zstd_compress.c:5398-5440)
+ *   ZSTD_compress / ZSTD_compressCCtx / ZSTD_compress_usingDict  (lib/compress/zstd_compress.c:5398-5440)
  *   parameter derivation   ZSTD_getCParams_internal :7123-7146 + ZSTD_adjustCParams_internal :1465-1602 (compress/clevels.h:25-130)
  *   block planning         ZSTD_compress_frameChunk :4527-4623 (here: all blocks of a call at once)
  * and hands every block to the CUDA kernels (zb_match.cu, zb_literals.cu, zb_sequences.cu,
@@ -112,7 +112,7 @@ struct ZbDeviceGuard {
 
 #define ZB_WAVE_SLOTS_MAX 14u
 #define ZB_WAVE_SLOTS_DEFAULT 4u
-#define ZB_HOST_WAVE_SLOTS_DEFAULT 8u   /* measured best with 384-block waves (tests/e2e_sweep.py, profiles/r1_e2e_timeline.md) */
+#define ZB_HOST_WAVE_SLOTS_DEFAULT 8u   /* with 384-block waves; on the H100 no setting of tests/e2e_sweep.py was faster in every run: the upload bounds the call (DESIGN.md section 10) */
 #define ZB_HOST_WAVE_BLOCKS 384u     /* 48 MiB of input per wave */
 /* Digested dictionary (lib/zstd.h:979, zstd_compress.c:5477-5642): the content tail, its entropy tables and
  * the primed hash-table images live on the device across calls; any number of contexts may use it. */
@@ -200,7 +200,7 @@ extern "C" ZSTD_CCtx* ZSTD_createCCtx(void)
     if (c->bindDevice < 0) { int d = -1; if (cudaGetDevice(&d) == cudaSuccess) c->bindDevice = d; else cudaGetLastError(); }
     c->advLevel = 3;                                                         /* ZSTD_CLEVEL_DEFAULT */
     {   const char* s = getenv("ZSTDB200_SERIAL"); const char* w = getenv("ZSTDB200_WAVE_BLOCKS");
-        c->devWaveBlocks = (s && atoi(s)) ? 0u : (w ? (u32)atoi(w) : 1024u);     /* 128 MiB waves: tests/wave_sweep.py */
+        c->devWaveBlocks = (s && atoi(s)) ? 0u : (w ? (u32)atoi(w) : 1024u);     /* 128 MiB waves x 4 slots: among the best on the H100, tests/wave_sweep.py (DESIGN.md section 11) */
         const char* n = getenv("ZSTDB200_WAVE_SLOTS"); const char* h = getenv("ZSTDB200_HOST_WAVE_BLOCKS");
         c->waveSlots = n ? (u32)atoi(n) : ZB_WAVE_SLOTS_DEFAULT;
         c->hostWaveSlots = n ? (u32)atoi(n) : ZB_HOST_WAVE_SLOTS_DEFAULT;
@@ -633,7 +633,7 @@ struct ZbEventSet {
 
 /* XXH64 (lib/common/xxhash.h: XXH64_update / XXH64_digest, seed 0) of the frame's content: the frame checksum is
  * its low 32 bits (zstd_compress.c:5297-5303).  A serial recurrence over 32-byte stripes: it runs on the calling
- * host thread while the GPU works (about 10 GB/s — a checksummed frame is bound by this pass, not by the GPU). */
+ * host thread while the GPU works (a large checksummed frame can be bound by this pass rather than by the GPU). */
 static u64 zb_xxh64(const u8* p, size_t len)
 {
     u64 const P1 = 0x9E3779B185EBCA87ull, P2 = 0xC2B2AE3D27D4EB4Full, P3 = 0x165667B19E3779F9ull, P4 = 0x85EBCA77C2B2AE63ull, P5 = 0x27D4EB2F165667C5ull;
@@ -670,15 +670,14 @@ static size_t zb_compressFramesWaves(ZSTD_CCtx* c, u8* dst, size_t dstCapacity, 
     u32 const waveBlocks128 = deviceMemory ? c->devWaveBlocks : c->hostWaveBlocks;       /* wave size in 128 KiB blocks */
     u32 const ZB_WAVE_SLOTS = deviceMemory ? c->waveSlots : c->hostWaveSlots;
     /* streams are created on first use: every stream beyond the hardware queue count (8 by default) shares a
-     * queue with another one, and a download queued behind another wave's kernels stalls the whole pipeline
-     * (measured: 16 streams -> every download waited for the last upload; profiles/r1_e2e_timeline.md) */
+     * queue with another one, and a download queued behind another wave's kernels stalls the whole pipeline */
     auto getStream = [&](u32 i, cudaStream_t* out) -> size_t {
         if (!c->waveStream[i]) CK(cudaStreamCreateWithFlags(&c->waveStream[i], cudaStreamNonBlocking));
         *out = c->waveStream[i];
         return 0;
     };
     cudaStream_t sCopy, sD2H = (cudaStream_t)0;
-    if (deviceMemory) {                                           /* creation order as measured: wave streams first */
+    if (deviceMemory) {                                           /* wave streams first: they take the first hardware queues */
         cudaStream_t t;
         for (u32 i = 0; i < ZB_WAVE_SLOTS; i++) { size_t const e = getStream(i, &t); if (zb_isErr(e)) return e; }
     }
@@ -779,8 +778,8 @@ static size_t zb_compressFramesWaves(ZSTD_CCtx* c, u8* dst, size_t dstCapacity, 
         }
     }
     double const hostEnq = zb_now() - hostT0;
-    /* content checksums.  Host buffers: XXH64 on host threads while the GPU works (a serial recurrence per frame: ~10 GB/s
-     * per thread).  Device buffers: a warp per frame once the last wave is stitched. */
+    /* content checksums.  Host buffers: XXH64 on host threads while the GPU works (a serial recurrence per frame, one
+     * thread each).  Device buffers: a warp per frame once the last wave is stitched. */
     std::vector<u64> xxh;
     if (c->callChecksum && !err && !deviceMemory) {
         xxh.resize(nbFrames);

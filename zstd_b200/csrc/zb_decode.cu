@@ -1,7 +1,7 @@
 /* zb_decode.cu — GPU decompression of zstd frames (SURVEY.md 8f rank 2): the other half of the block pipeline.
  *
  * Replaces, with a block-parallel formulation, what the reference does serially per frame:
- *   ZSTD_decompress / ZSTD_decompressDCtx / ZSTD_decompressFrame  (/root/reference/lib/decompress/zstd_decompress.c:1011-1124)
+ *   ZSTD_decompress / ZSTD_decompressDCtx / ZSTD_decompressFrame  (lib/decompress/zstd_decompress.c:1011-1124)
  *   ZSTD_decodeLiteralsBlock, ZSTD_decodeSeqHeaders, ZSTD_decompressSequences_body, ZSTD_execSequence
  *                                                     (lib/decompress/zstd_decompress_block.c:343, :695, :1615, :1012)
  *   HUF_decompress4X1 / HUF_readDTableX1              (lib/decompress/huf_decompress.c:602, :383)
@@ -575,7 +575,7 @@ static size_t zbd_ctxInit(ZSTD_DCtx* d)
     DCK(cudaMalloc(&d->d_res, 16 * sizeof(u64)));
     DCK(cudaMallocHost(&d->h_res, 16 * sizeof(u64)));
     d->d_execErr = (u32*)(d->d_res + 9); d->d_ticket = (u32*)(d->d_res + 10);
-    if (cudaDeviceGetAttribute(&d->smCount, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || d->smCount <= 0) d->smCount = 148;
+    if (cudaDeviceGetAttribute(&d->smCount, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || d->smCount <= 0) d->smCount = 132;
     d->device = dev;
     return 0;
 }
@@ -705,9 +705,9 @@ static size_t zbd_decompressHost(ZSTD_DCtx* d, void* dst, size_t dstCapacity, co
 
 /* device buffers: the walk is a kernel (one thread follows the chain of block headers) */
 /* device buffers.  The headers have to be followed one after the other wherever they are read: one device thread pays a
- * memory round trip (~1 us) per header, the host ~0.1 us — so compressed inputs up to ZBD_HOSTWALK_MAX are copied to a
- * page-locked staging buffer (at PCIe speed) and walked there (a call of 131072 one-KiB frames: 207 -> ~30 ms); beyond
- * that the walk is a kernel (one thread follows the chain of block headers). */
+ * device-memory round trip per header, the host a cache access — so compressed inputs up to ZBD_HOSTWALK_MAX are copied
+ * to a page-locked staging buffer (at PCIe speed) and walked there; beyond that the walk is a kernel (one thread follows
+ * the chain of block headers). */
 static size_t zbd_decompressDevice(ZSTD_DCtx* d, void* d_dst, size_t dstCapacity, const void* d_src, size_t srcSize, cudaStream_t st)
 {
     if (srcSize <= d->hostWalkMax) {

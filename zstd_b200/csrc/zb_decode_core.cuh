@@ -1,5 +1,5 @@
 /* zb_decode_core.cuh — format-level pieces of the decompressor, written from the format specification
- * (/root/reference/doc/zstd_compression_format.md) as host+device functions: frame / block / section headers, the two
+ * (doc/zstd_compression_format.md) as host+device functions: frame / block / section headers, the two
  * bit readers, FSE table descriptions and decoding tables, Huffman tree descriptions and decoding tables, the sequence
  * bitstream.  The CUDA kernels of zb_decode.cu call them per warp / per lane; tests/host_decode.cpp compiles the same
  * functions for the CPU so that this logic is checked against the reference encoder's frames without a GPU (the

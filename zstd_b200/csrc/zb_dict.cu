@@ -1,6 +1,6 @@
 /* zb_dict.cu — host side: parsing a dictionary (no device code here).
  * Replaces ZSTD_compress_insertDictionary / ZSTD_loadZstdDictionary / ZSTD_loadCEntropy
- * (/root/reference/lib/compress/zstd_compress.c:5119-5156, :5087-5115, :4987-5076) for the simple API:
+ * (lib/compress/zstd_compress.c:5119-5156, :5087-5115, :4987-5076) for the simple API:
  *   < 8 bytes                -> ignored (:5132)
  *   no magic 0xEC30A437      -> raw content (:5143-5148)
  *   magic                    -> dictID, Huffman table (HUF_readCTable huf_compress.c:292, HUF_readStats

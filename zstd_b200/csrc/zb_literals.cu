@@ -1,6 +1,6 @@
 /* zb_literals.cu — K2: literals section of one block per CTA.
  *
- * Replaces ZSTD_compressLiterals (/root/reference/lib/compress/zstd_compress_literals.c:129-235)
+ * Replaces ZSTD_compressLiterals (lib/compress/zstd_compress_literals.c:129-235)
  * and HUF_compress_internal (huf_compress.c:1333-1430) for a fresh entropy state:
  *   1. 256-bin histogram: per-warp privatised bins in shared memory + merge (hist.c:66-133)
  *   2. raw / RLE / compressed decision with the reference's thresholds
@@ -18,7 +18,7 @@
 #define LIT_THREADS 128
 #endif
 #ifndef LIT_MIN_CTAS
-#define LIT_MIN_CTAS 12               /* 16 (32 registers) measured slower: 1.56 vs 1.40 ms */
+#define LIT_MIN_CTAS 12               /* 16 (32 registers) measured slower on the H100: literals 2.90 vs 2.68 ms per GiB of config 2 */
 #endif
 #define LIT_WARPS (LIT_THREADS / 32)
 #ifndef LIT_PACK2

@@ -1,7 +1,7 @@
 /* zb_match.cu — K1: LZ77 match-finder ("fast" and "doubleFast" strategies) = K1a candidate walk, K1b greedy parse, K1c merge.
  *
  * Replaces the CPU loops ZSTD_compressBlock_fast_noDict_generic / _extDict_generic
- * (/root/reference/lib/compress/zstd_fast.c:192-423, :709-960) and ZSTD_compressBlock_doubleFast_noDict_generic
+ * (lib/compress/zstd_fast.c:192-423, :709-960) and ZSTD_compressBlock_doubleFast_noDict_generic
  * (zstd_double_fast.c:105-323) with a data-parallel formulation:
  *   - K1a (one CTA per CHUNK of up to 4 blocks) keeps the chunk's hash table in shared memory — primed from
  *     the <=128 KiB in front of the chunk (zstd_fast.c:53-85 does this for dictionaries, zstdmt_compress.c:1182-1227 for
@@ -227,10 +227,10 @@ __device__ __forceinline__ bool zb_walk_batch(u32* __restrict__ table, u32 xa, c
 #define WALK_STEADY 1            /* development switch: 0 = every batch takes the general path */
 #endif
 #ifndef WALK_P_SMALL
-#define WALK_P_SMALL 8           /* positions per thread for tables <= 56 KiB: 128 threads per CTA (2.62 ms per GiB against 2.72 with 4; development knob: tools/build_variant.sh) */
+#define WALK_P_SMALL 8           /* positions per thread for tables <= 56 KiB: 128 threads per CTA (on the H100 the walk takes 3.05 ms per GiB of config 2 with 8 and 3.03 with 4: equal within run-to-run spread; development knob: tools/build_variant.sh) */
 #endif
 #ifndef WALK_P_MID
-#define WALK_P_MID 4             /* tables of 56 .. 113 KiB: two CTAs per SM (measured on config 4: 10.2 ms with 4 positions per thread, 11.2 with 2) */
+#define WALK_P_MID 4             /* tables of 56 .. 113 KiB: two CTAs per SM (walk on the H100, config 4: 8.22 ms with 4 positions per thread, 8.83 with 2) */
 #endif
 #ifndef WALK_MINB_SMALL
 #define WALK_MINB_SMALL 4        /* CTAs per SM the register allocation of that variant leaves room for */
@@ -382,7 +382,7 @@ zb_walk_kernel(const u8* __restrict__ src, const u8* __restrict__ dictEnd, const
 #define PARSE_WARPS 8            /* = ZB_PARSE_SEGS: the eight segments of a full block share a CTA */
 #endif
 #ifndef PARSE_MIN_CTAS
-#define PARSE_MIN_CTAS 6         /* 48 warps per SM at 40 registers (profiles/r1_history.md) */
+#define PARSE_MIN_CTAS 6         /* 48 warps per SM at 40 registers */
 #endif
 __device__ __forceinline__ u32 zb_dist_at(const u16* __restrict__ d16, const u32* __restrict__ far, u32 i)
 {
@@ -640,7 +640,7 @@ __device__ __forceinline__ u32 zb_rep_code(ZbRepHist& h, u32 off, u32 ll)
 
 #define MERGE_THREADS 256
 #ifndef MERGE_MIN_CTAS
-#define MERGE_MIN_CTAS 6           /* 40 registers (parse + merge 5.46 ms per GiB against 5.49 with 5 and 5.65 with 4) */
+#define MERGE_MIN_CTAS 6           /* 40 registers (parse + merge on the H100: 6.12 ms per GiB of config 2 against 6.22 with 5 and 6.41 with 4) */
 #endif
 #define MERGE_TILE 1024u                       /* sequences scanned and gathered per round */
 #define MERGE_PER (MERGE_TILE / MERGE_THREADS)  /* consecutive sequences of a tile owned by one thread */

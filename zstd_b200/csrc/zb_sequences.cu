@@ -1,7 +1,7 @@
 /* zb_sequences.cu — K3: sequences section of one block per CTA + final block-type decision.
  *
  * Replaces, for a fresh entropy state, ZSTD_buildSequencesStatistics
- * (/root/reference/lib/compress/zstd_compress.c:2755-2873), ZSTD_seqToCodes (:2686-2712),
+ * (lib/compress/zstd_compress.c:2755-2873), ZSTD_seqToCodes (:2686-2712),
  * ZSTD_selectEncodingType / ZSTD_buildCTable (zstd_compress_sequences.c:157-288),
  * ZSTD_encodeSequences_body (:291-382) and the block-level checks of
  * ZSTD_entropyCompressSeqStore (zstd_compress.c:2987-2993, :3025-3028) and

@@ -1,6 +1,6 @@
 /* zb_stitch.cu — K4: assemble frames from independently compressed blocks.
  *
- * The reference's block loop (ZSTD_compress_frameChunk, /root/reference/lib/compress/zstd_compress.c:4527-4623)
+ * The reference's block loop (ZSTD_compress_frameChunk, lib/compress/zstd_compress.c:4527-4623)
  * appends blocks one after the other; here all blocks of a call were compressed at once, so the
  * frame is assembled by (a) computing every block's output size (frame header for the first block
  * of a frame, :4626-4672; 3-byte block header, :4586-4590; payload), (b) an exclusive prefix sum,
@@ -187,7 +187,7 @@ extern "C" cudaError_t zb_launch_stitch(const u8* d_src, const ZbBlock* d_blocks
  * the reference computes it chunk by chunk on the host, zstd_compress.c:4544, :5297-5303).
  * XXH64 is four serial accumulator chains per input (acc = rotl(acc + x * P2, 31) * P1 over the 8-byte words of
  * every 32-byte stripe): nothing to split inside one frame, so one warp takes a frame — all lanes load 256 bytes,
- * lanes 0..3 run the chains — and the frames of a call are hashed side by side.  About 1 GB/s per frame. */
+ * lanes 0..3 run the chains — and the frames of a call are hashed side by side. */
 __device__ __forceinline__ u64 zbx_rotl(u64 x, int r) { return (x << r) | (x >> (64 - r)); }
 #define ZBX_P1 0x9E3779B185EBCA87ull
 #define ZBX_P2 0xC2B2AE3D27D4EB4Full
