@@ -440,6 +440,64 @@ def test_checksums_device_buffers_and_many_frames(ctx):
     c.close()
 
 
+def test_wave_executor_at_small_sizes():
+    """The executor's ways through a call, with 512 KiB waves taking turns on 2 workspace slots so that a few MiB make many
+    waves: device buffers in waves, host buffers in waves, one wave on one stream (ZSTDB200_SERIAL=1) and one wave on a
+    caller-supplied stream give the same bytes and sizes, equal to the oracle's frames.  One call has several frames with
+    content checksums, the other 24 frames against a dictionary (the table-image path)."""
+    import torch
+    knobs = ("ZSTDB200_WAVE_BLOCKS", "ZSTDB200_HOST_WAVE_BLOCKS", "ZSTDB200_WAVE_SLOTS", "ZSTDB200_SERIAL")
+    saved = {k: os.environ.get(k) for k in knobs}
+    try:
+        os.environ.update({"ZSTDB200_WAVE_BLOCKS": "4", "ZSTDB200_HOST_WAVE_BLOCKS": "4", "ZSTDB200_WAVE_SLOTS": "2"})
+        os.environ.pop("ZSTDB200_SERIAL", None)
+        waves = zstd_b200.ZSTD_CCtx()
+        os.environ["ZSTDB200_SERIAL"] = "1"
+        serial = zstd_b200.ZSTD_CCtx()
+    finally:
+        for k, v in saved.items():
+            if v is None:
+                os.environ.pop(k, None)
+            else:
+                os.environ[k] = v
+    d = zref.golden_input("zdict-16k-synthetic-seed77")
+    side = torch.cuda.Stream()
+    for sizes, dict_bytes, checksum in (([3 << 20, 1000, 0, 700_001, (1 << 20) + 5], None, True), ([150_000] * 16 + [1024] * 8, d, False)):
+        src = zref.synthetic(sum(sizes), 61, 0.5)
+        offs, o = [], 0
+        for n in sizes:
+            offs.append(o); o += n
+        cap = sum(zstd_b200.ZSTD_compressBound(n) + 32 for n in sizes)
+        d_src = torch.frombuffer(bytearray(src), dtype=torch.uint8).cuda()
+        sbuf = ctypes.create_string_buffer(src, len(src))
+        want = []
+        for off, n in zip(offs, sizes):
+            part = src[off:off + n]
+            f = zref.oracle_compress(part, 1) if dict_bytes is None else zref.oracle_compress_using_dict(part, dict_bytes, 1)
+            want.append(_with_checksum(f, part) if checksum else f)
+        for c in (waves, serial):
+            c.set_parameter("checksum_flag", int(checksum))
+
+        def run(c, device=True, stream=0):
+            if not device:
+                h_dst = ctypes.create_string_buffer(cap)
+                total, csz = c.compress_frames(ctypes.addressof(h_dst), cap, ctypes.addressof(sbuf), offs, sizes, level=1,
+                                               device_memory=False, dict_bytes=dict_bytes)
+                return h_dst.raw[:total], csz, c.stats()
+            d_dst = torch.zeros(cap, dtype=torch.uint8, device="cuda")
+            total, csz = c.compress_frames(d_dst.data_ptr(), cap, d_src.data_ptr(), offs, sizes, level=1, dict_bytes=dict_bytes, stream=stream)
+            return bytes(d_dst[:total].cpu().numpy()), csz, c.stats()
+
+        got = {"device waves": run(waves), "host waves": run(waves, device=False), "serial": run(serial),
+               "caller stream": run(waves, stream=side.cuda_stream)}
+        for name, (out, csz, st) in got.items():
+            assert csz == [len(f) for f in want], name
+            assert out == b"".join(want), name
+            assert (st.literals_ms > 0) == (name in ("serial", "caller stream")), name     # per-phase times: one-wave calls only
+    waves.close()
+    serial.close()
+
+
 def test_mixed_frame_lists(ctx):
     """Batch call over runs of equal single-block frames (the planner's template path), odd sizes, empty frames and a
     multi-block frame in between: every frame equals the single-call frame."""

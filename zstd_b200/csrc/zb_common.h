@@ -158,4 +158,26 @@ typedef struct {
     u32 state;         /* u16 per FSE stream per block inside the dist area (3 * state <= dist) */
 } ZbStrides;
 
+#ifdef __CUDACC__
+/* host helpers of the compression and decompression drivers (zb_api.cu, zb_decode.cu) */
+#include <cuda_runtime.h>
+#include <stdio.h>
+#include <stdlib.h>
+
+static inline bool zb_isErr(size_t c) { return c > ZB_ERR(ZB_error_maxCode); }
+
+/* a failed CUDA call returns an error code from the enclosing function; its sticky error is cleared, so that the caller's
+ * next cudaGetLastError() does not report it again */
+#define CK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { \
+    if (getenv("ZSTDB200_DEBUG")) fprintf(stderr, "zstd_b200: CUDA error %s at %s:%d\n", cudaGetErrorString(e_), __FILE__, __LINE__); \
+    cudaGetLastError(); return ZB_ERR(e_ == cudaErrorMemoryAllocation ? ZB_error_memory_allocation : ZB_error_GENERIC); } } while (0)
+
+/* restores the calling thread's current device when a call returns (a context works on the device it was created for) */
+struct ZbDeviceGuard {
+    int prev;
+    ZbDeviceGuard() : prev(-1) { if (cudaGetDevice(&prev) != cudaSuccess) { prev = -1; cudaGetLastError(); } }
+    ~ZbDeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
+};
+#endif
+
 #endif

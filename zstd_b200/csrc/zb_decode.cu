@@ -532,11 +532,6 @@ struct ZSTD_DCtx_s {
 };
 extern "C" int zb_boundDevice(void);                                 /* zb_api.cu: ZSTDB200_setDevice's value, or -1 */
 
-#define DCK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { \
-    if (getenv("ZSTDB200_DEBUG")) fprintf(stderr, "zstd_b200: CUDA error %s at %s:%d\n", cudaGetErrorString(e_), __FILE__, __LINE__); \
-    cudaGetLastError(); return ZB_ERR(e_ == cudaErrorMemoryAllocation ? ZB_error_memory_allocation : ZB_error_GENERIC); } } while (0)
-static inline bool zbd_isErr(size_t c) { return c > ZB_ERR(ZB_error_maxCode); }
-
 extern "C" ZSTD_DCtx* ZSTD_createDCtx(void)                          /* lib/zstd.h:289 */
 {
     ZSTD_DCtx* d = (ZSTD_DCtx*)calloc(1, sizeof(ZSTD_DCtx));
@@ -565,15 +560,15 @@ extern "C" size_t ZSTD_freeDCtx(ZSTD_DCtx* d)                        /* accepts 
 }
 static size_t zbd_ctxInit(ZSTD_DCtx* d)
 {
-    if (d->device >= 0) { DCK(cudaSetDevice(d->device)); return 0; }
+    if (d->device >= 0) { CK(cudaSetDevice(d->device)); return 0; }
     int n = 0;
     if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) { cudaGetLastError(); return ZB_ERR(ZB_error_GENERIC); }
     int dev = d->bindDevice < 0 ? 0 : d->bindDevice;
-    DCK(cudaSetDevice(dev));
-    DCK(cudaStreamCreateWithFlags(&d->stream, cudaStreamNonBlocking));
-    for (int i = 0; i < 7; i++) DCK(cudaEventCreate(&d->ev[i]));
-    DCK(cudaMalloc(&d->d_res, 16 * sizeof(u64)));
-    DCK(cudaMallocHost(&d->h_res, 16 * sizeof(u64)));
+    CK(cudaSetDevice(dev));
+    CK(cudaStreamCreateWithFlags(&d->stream, cudaStreamNonBlocking));
+    for (int i = 0; i < 7; i++) CK(cudaEventCreate(&d->ev[i]));
+    CK(cudaMalloc(&d->d_res, 16 * sizeof(u64)));
+    CK(cudaMallocHost(&d->h_res, 16 * sizeof(u64)));
     d->d_execErr = (u32*)(d->d_res + 9); d->d_ticket = (u32*)(d->d_res + 10);
     if (cudaDeviceGetAttribute(&d->smCount, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || d->smCount <= 0) d->smCount = 132;
     d->device = dev;
@@ -584,7 +579,7 @@ template <typename T> static size_t zbd_grow(T** p, size_t* cap, size_t need)
     if (need <= *cap) return 0;
     cudaFree(*p); *p = NULL; *cap = 0;
     size_t const n = need + need / 8 + 64;
-    DCK(cudaMalloc(p, n * sizeof(T)));
+    CK(cudaMalloc(p, n * sizeof(T)));
     *cap = n;
     return 0;
 }
@@ -592,38 +587,38 @@ template <typename T> static size_t zbd_grow(T** p, size_t* cap, size_t need)
 /* D1 .. D4 over descriptors that are already on the device; returns the output size */
 static size_t zbd_run(ZSTD_DCtx* d, u8* d_dst, size_t dstCapacity, const u8* d_src, u32 nb, u32 nf, u64 seqCount, cudaStream_t st)
 {
-    DCK(cudaMemsetAsync(d->d_execErr, 0, sizeof(u32), st));
-    DCK(cudaEventRecord(d->ev[1], st));
+    CK(cudaMemsetAsync(d->d_execErr, 0, sizeof(u32), st));
+    CK(cudaEventRecord(d->ev[1], st));
     u32 const grid = (nb + ZBD_WARPS - 1u) / ZBD_WARPS;
     zbd_literals_kernel<<<grid, 32 * ZBD_WARPS, 0, st>>>(d_src, d->d_blocks, nb, d->d_lits, d->d_bout, d->d_dict, d->di);
-    DCK(cudaEventRecord(d->ev[2], st));
+    CK(cudaEventRecord(d->ev[2], st));
     zbd_sequences_kernel<<<grid, 32 * ZBD_WARPS, 0, st>>>(d_src, d->d_blocks, nb, d->d_seqs, d->d_bout, d->d_dict, d->di);
-    DCK(cudaEventRecord(d->ev[3], st));
+    CK(cudaEventRecord(d->ev[3], st));
     zbd_scan_kernel<<<1, SCAN_THREADS, 0, st>>>(d->d_blocks, nb, d->d_frames, nf, d->d_bout, (u64)dstCapacity, d->d_res, d->di);
-    DCK(cudaMemcpyAsync(d->h_res, d->d_res, 2 * sizeof(u64), cudaMemcpyDeviceToHost, st));
-    DCK(cudaStreamSynchronize(st));                                  /* nothing is written to dst before the sizes are known to fit */
+    CK(cudaMemcpyAsync(d->h_res, d->d_res, 2 * sizeof(u64), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));                                  /* nothing is written to dst before the sizes are known to fit */
     if (d->h_res[0]) return ZB_ERR((u32)d->h_res[0]);
     size_t const total = (size_t)d->h_res[1];
-    DCK(cudaEventRecord(d->ev[4], st));
+    CK(cudaEventRecord(d->ev[4], st));
     u32 const dictContent = d->dictSize ? (u32)(d->dictSize - d->di.contentOff) : 0u;
     const u8* const d_dictContent = d->dictSize ? d->d_dict + d->di.contentOff : (const u8*)NULL;
-    {   size_t const r = zbd_grow(&d->d_tileFirst, &d->capTiles, (total >> ZBD_TILE_LOG) + 4); if (zbd_isErr(r)) return r; }
-    {   size_t const r = zbd_grow(&d->d_done, &d->capDone, (size_t)seqCount + 4); if (zbd_isErr(r)) return r; }
-    DCK(cudaMemsetAsync(d->d_tileFirst, 0xFF, ((total >> ZBD_TILE_LOG) + 4) * sizeof(u32), st));
-    DCK(cudaMemsetAsync(d->d_done, 0, (size_t)seqCount + 4, st));
+    {   size_t const r = zbd_grow(&d->d_tileFirst, &d->capTiles, (total >> ZBD_TILE_LOG) + 4); if (zb_isErr(r)) return r; }
+    {   size_t const r = zbd_grow(&d->d_done, &d->capDone, (size_t)seqCount + 4); if (zb_isErr(r)) return r; }
+    CK(cudaMemsetAsync(d->d_tileFirst, 0xFF, ((total >> ZBD_TILE_LOG) + 4) * sizeof(u32), st));
+    CK(cudaMemsetAsync(d->d_done, 0, (size_t)seqCount + 4, st));
     zbd_place_kernel<<<grid, 32 * ZBD_WARPS, 0, st>>>(d_src, d->d_blocks, nb, d->d_lits, d->d_seqs, d->d_matchPos, d->d_tileFirst, d->d_bout, d_dst,
                                                       d_dictContent, dictContent, d->d_execErr);
-    DCK(cudaEventRecord(d->ev[6], st));
+    CK(cudaEventRecord(d->ev[6], st));
     if (seqCount) {                                                  /* threads per frame by the matches a frame holds */
         u64 const perFrame = seqCount / (nf ? nf : 1u);
         if (perFrame >= 8192u)     zbd_matches_kernel<1024><<<nf, 1024, 0, st>>>(d->d_blocks, d->d_frames, d->d_seqs, d->d_matchPos, d->d_tileFirst, (u64)total, d_dst, d->d_done, d->d_execErr);
         else if (perFrame >= 256u) zbd_matches_kernel<128><<<nf, 128, 0, st>>>(d->d_blocks, d->d_frames, d->d_seqs, d->d_matchPos, d->d_tileFirst, (u64)total, d_dst, d->d_done, d->d_execErr);
         else                       zbd_matches_kernel<32><<<nf, 32, 0, st>>>(d->d_blocks, d->d_frames, d->d_seqs, d->d_matchPos, d->d_tileFirst, (u64)total, d_dst, d->d_done, d->d_execErr);
     }
-    DCK(cudaEventRecord(d->ev[5], st));
-    DCK(cudaMemcpyAsync(d->h_res + 2, d->d_execErr, sizeof(u32), cudaMemcpyDeviceToHost, st));
-    DCK(cudaStreamSynchronize(st));
-    DCK(cudaGetLastError());
+    CK(cudaEventRecord(d->ev[5], st));
+    CK(cudaMemcpyAsync(d->h_res + 2, d->d_execErr, sizeof(u32), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    CK(cudaGetLastError());
     if ((u32)d->h_res[2]) return ZB_ERR((u32)d->h_res[2]);
     {   float ms = 0;
         cudaEventElapsedTime(&ms, d->ev[1], d->ev[2]); d->stats.literals_ms = ms;
@@ -640,13 +635,13 @@ static size_t zbd_ensure(ZSTD_DCtx* d, u32 nb, u32 nf, u64 litBytes, u64 seqCoun
     if (nb > d->capBlocks) {
         cudaFree(d->d_blocks); cudaFree(d->d_bout); d->d_blocks = NULL; d->d_bout = NULL; d->capBlocks = 0;
         size_t const n = (size_t)nb + nb / 8 + 64;
-        DCK(cudaMalloc(&d->d_blocks, n * sizeof(ZbdBlock))); DCK(cudaMalloc(&d->d_bout, (n + 1) * sizeof(ZbdBlockOut)));
+        CK(cudaMalloc(&d->d_blocks, n * sizeof(ZbdBlock))); CK(cudaMalloc(&d->d_bout, (n + 1) * sizeof(ZbdBlockOut)));
         d->capBlocks = n;
     }
-    {   size_t const e = zbd_grow(&d->d_frames, &d->capFrames, (size_t)nf); if (zbd_isErr(e)) return e; }
-    {   size_t const e = zbd_grow(&d->d_lits, &d->capLits, (size_t)litBytes + 16); if (zbd_isErr(e)) return e; }
-    {   size_t const e = zbd_grow(&d->d_seqs, &d->capSeqs, (size_t)seqCount + 1); if (zbd_isErr(e)) return e; }
-    {   size_t const e = zbd_grow(&d->d_matchPos, &d->capMatchPos, (size_t)seqCount + 1); if (zbd_isErr(e)) return e; }
+    {   size_t const e = zbd_grow(&d->d_frames, &d->capFrames, (size_t)nf); if (zb_isErr(e)) return e; }
+    {   size_t const e = zbd_grow(&d->d_lits, &d->capLits, (size_t)litBytes + 16); if (zb_isErr(e)) return e; }
+    {   size_t const e = zbd_grow(&d->d_seqs, &d->capSeqs, (size_t)seqCount + 1); if (zb_isErr(e)) return e; }
+    {   size_t const e = zbd_grow(&d->d_matchPos, &d->capMatchPos, (size_t)seqCount + 1); if (zb_isErr(e)) return e; }
     return 0;
 }
 
@@ -666,19 +661,19 @@ static size_t zbd_decompressHost(ZSTD_DCtx* d, void* dst, size_t dstCapacity, co
     u64 known = 0; bool allKnown = true;
     for (u32 f = 0; f < nf; f++) { if (F[f].contentSize == ZBD_CONTENTSIZE_UNKNOWN) allKnown = false; else known += F[f].contentSize; }
     if (allKnown && known > dstCapacity) return ZB_ERR(ZB_error_dstSize_tooSmall);
-    {   size_t const r = zbd_grow(&d->d_in, &d->capIn, srcSize + 16); if (zbd_isErr(r)) return r; }
-    {   size_t const r = zbd_ensure(d, nb, nf, lit, seq); if (zbd_isErr(r)) return r; }
-    DCK(cudaEventRecord(d->ev[0], st));
-    DCK(cudaMemcpyAsync(d->d_in, in, srcSize, cudaMemcpyHostToDevice, st));
+    {   size_t const r = zbd_grow(&d->d_in, &d->capIn, srcSize + 16); if (zb_isErr(r)) return r; }
+    {   size_t const r = zbd_ensure(d, nb, nf, lit, seq); if (zb_isErr(r)) return r; }
+    CK(cudaEventRecord(d->ev[0], st));
+    CK(cudaMemcpyAsync(d->d_in, in, srcSize, cudaMemcpyHostToDevice, st));
     /* the output can not be larger than the blocks' maximum sizes */
     size_t const outNeed = allKnown ? (size_t)known : (dstCapacity < (size_t)nb * ZB_BLOCK_MAX ? dstCapacity : (size_t)nb * ZB_BLOCK_MAX);
-    {   size_t const r = zbd_grow(&d->d_out, &d->capOut, outNeed + 16); if (zbd_isErr(r)) return r; }
-    DCK(cudaMemcpyAsync(d->d_blocks, B.data(), (size_t)nb * sizeof(ZbdBlock), cudaMemcpyHostToDevice, st));
-    DCK(cudaMemcpyAsync(d->d_frames, F.data(), (size_t)nf * sizeof(ZbdFrame), cudaMemcpyHostToDevice, st));
+    {   size_t const r = zbd_grow(&d->d_out, &d->capOut, outNeed + 16); if (zb_isErr(r)) return r; }
+    CK(cudaMemcpyAsync(d->d_blocks, B.data(), (size_t)nb * sizeof(ZbdBlock), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d->d_frames, F.data(), (size_t)nf * sizeof(ZbdFrame), cudaMemcpyHostToDevice, st));
     size_t const total = zbd_run(d, d->d_out, outNeed, d->d_in, nb, nf, seq, st);
-    if (zbd_isErr(total)) return total;
+    if (zb_isErr(total)) return total;
     if (total > dstCapacity) return ZB_ERR(ZB_error_dstSize_tooSmall);
-    if (total) DCK(cudaMemcpy(dst, d->d_out, total, cudaMemcpyDeviceToHost));
+    if (total) CK(cudaMemcpy(dst, d->d_out, total, cudaMemcpyDeviceToHost));
     /* frame checksums (format: "Content_Checksum"): XXH64 of the regenerated content, low 32 bits */
     {   size_t off = 0;
         for (u32 f = 0; f < nf; f++) {
@@ -687,9 +682,9 @@ static size_t zbd_decompressHost(ZSTD_DCtx* d, void* dst, size_t dstCapacity, co
             else { /* sizes of frames without the field: from the scan */
                 std::vector<ZbdBlockOut> tmp(2);
                 u32 const last = F[f].firstBlock + F[f].nbBlocks;
-                DCK(cudaMemcpy(&tmp[0], d->d_bout + F[f].firstBlock, sizeof(ZbdBlockOut), cudaMemcpyDeviceToHost));
+                CK(cudaMemcpy(&tmp[0], d->d_bout + F[f].firstBlock, sizeof(ZbdBlockOut), cudaMemcpyDeviceToHost));
                 u64 end = total;
-                if (last < nb) { DCK(cudaMemcpy(&tmp[1], d->d_bout + last, sizeof(ZbdBlockOut), cudaMemcpyDeviceToHost)); end = tmp[1].dstOff; }
+                if (last < nb) { CK(cudaMemcpy(&tmp[1], d->d_bout + last, sizeof(ZbdBlockOut), cudaMemcpyDeviceToHost)); end = tmp[1].dstOff; }
                 size = end - tmp[0].dstOff;
             }
             if (F[f].hasChecksum) {
@@ -714,11 +709,11 @@ static size_t zbd_decompressDevice(ZSTD_DCtx* d, void* d_dst, size_t dstCapacity
         if (srcSize > d->capStage) {
             cudaFreeHost(d->h_stage); d->h_stage = NULL; d->capStage = 0;
             size_t const n = srcSize + srcSize / 4 + 4096;
-            DCK(cudaMallocHost(&d->h_stage, n));
+            CK(cudaMallocHost(&d->h_stage, n));
             d->capStage = n;
         }
-        DCK(cudaMemcpyAsync(d->h_stage, d_src, srcSize, cudaMemcpyDeviceToHost, st));
-        DCK(cudaStreamSynchronize(st));
+        CK(cudaMemcpyAsync(d->h_stage, d_src, srcSize, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
         const u8* const in = d->h_stage;
         u32 nb = 0, nf = 0; u64 lit = 0, seq = 0;
         u32 e = zbd_walk(in, srcSize, NULL, 0, NULL, 0, &nb, &nf, &lit, &seq, d->di.entropy != 0, d->di.dictID);
@@ -727,18 +722,18 @@ static size_t zbd_decompressDevice(ZSTD_DCtx* d, void* d_dst, size_t dstCapacity
         std::vector<ZbdBlock> B(nb); std::vector<ZbdFrame> F(nf ? nf : 1);
         e = zbd_walk(in, srcSize, B.data(), nb, F.data(), nf, &nb, &nf, &lit, &seq, d->di.entropy != 0, d->di.dictID);
         if (e) return ZB_ERR(e);
-        {   size_t const r = zbd_ensure(d, nb, nf, lit, seq); if (zbd_isErr(r)) return r; }
-        DCK(cudaMemcpyAsync(d->d_blocks, B.data(), (size_t)nb * sizeof(ZbdBlock), cudaMemcpyHostToDevice, st));
-        DCK(cudaMemcpyAsync(d->d_frames, F.data(), (size_t)nf * sizeof(ZbdFrame), cudaMemcpyHostToDevice, st));
-        DCK(cudaStreamSynchronize(st));                               /* B and F are pageable and go out of scope */
+        {   size_t const r = zbd_ensure(d, nb, nf, lit, seq); if (zb_isErr(r)) return r; }
+        CK(cudaMemcpyAsync(d->d_blocks, B.data(), (size_t)nb * sizeof(ZbdBlock), cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(d->d_frames, F.data(), (size_t)nf * sizeof(ZbdFrame), cudaMemcpyHostToDevice, st));
+        CK(cudaStreamSynchronize(st));                               /* B and F are pageable and go out of scope */
         return zbd_run(d, (u8*)d_dst, dstCapacity, (const u8*)d_src, nb, nf, seq, st);
     }
     u32 capB = (u32)(srcSize / 4096u) + 1024u, capF = 1024u;
     for (int attempt = 0; attempt < 2; attempt++) {
-        {   size_t const r = zbd_ensure(d, capB, capF, 0, 0); if (zbd_isErr(r)) return r; }
+        {   size_t const r = zbd_ensure(d, capB, capF, 0, 0); if (zb_isErr(r)) return r; }
         zbd_walk_kernel<<<1, 32, 0, st>>>((const u8*)d_src, (u64)srcSize, d->d_blocks, (u32)d->capBlocks, d->d_frames, (u32)d->capFrames, d->d_res, d->di.entropy, d->di.dictID);
-        DCK(cudaMemcpyAsync(d->h_res, d->d_res, 5 * sizeof(u64), cudaMemcpyDeviceToHost, st));
-        DCK(cudaStreamSynchronize(st));
+        CK(cudaMemcpyAsync(d->h_res, d->d_res, 5 * sizeof(u64), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
         if (d->h_res[0]) return ZB_ERR((u32)d->h_res[0]);
         if (d->h_res[1] <= d->capBlocks && d->h_res[2] <= d->capFrames) break;
         capB = (u32)d->h_res[1]; capF = (u32)d->h_res[2];
@@ -746,11 +741,9 @@ static size_t zbd_decompressDevice(ZSTD_DCtx* d, void* d_dst, size_t dstCapacity
     }
     u32 const nb = (u32)d->h_res[1], nf = (u32)d->h_res[2];
     if (nb == 0) return 0;
-    {   size_t const r = zbd_ensure(d, nb, nf, d->h_res[3], d->h_res[4]); if (zbd_isErr(r)) return r; }
+    {   size_t const r = zbd_ensure(d, nb, nf, d->h_res[3], d->h_res[4]); if (zb_isErr(r)) return r; }
     return zbd_run(d, (u8*)d_dst, dstCapacity, (const u8*)d_src, nb, nf, d->h_res[4], st);
 }
-
-struct ZbdDeviceGuard { int prev; ZbdDeviceGuard() : prev(-1) { if (cudaGetDevice(&prev) != cudaSuccess) { prev = -1; cudaGetLastError(); } } ~ZbdDeviceGuard() { if (prev >= 0) cudaSetDevice(prev); } };
 
 /* the call's dictionary: parsed on the host (zbd_parseDict), uploaded whole; NULL / 0 = none.  A dictionary without the
  * magic number — or shorter than 8 bytes — is raw content (zstd_decompress.c:1541-1560). */
@@ -760,9 +753,9 @@ static size_t zbd_setDict(ZSTD_DCtx* d, const void* dict, size_t dictSize, cudaS
     if (!dict || dictSize == 0) return 0;
     u32 const e = zbd_parseDict(&d->di, (const u8*)dict, dictSize);
     if (e) return ZB_ERR(e);
-    {   size_t const r = zbd_grow(&d->d_dict, &d->capDict, dictSize + 16); if (zbd_isErr(r)) return r; }
-    DCK(cudaMemcpyAsync(d->d_dict, dict, dictSize, cudaMemcpyHostToDevice, st));
-    DCK(cudaStreamSynchronize(st));                                    /* the caller's dictionary buffer is pageable memory that may change after the call */
+    {   size_t const r = zbd_grow(&d->d_dict, &d->capDict, dictSize + 16); if (zb_isErr(r)) return r; }
+    CK(cudaMemcpyAsync(d->d_dict, dict, dictSize, cudaMemcpyHostToDevice, st));
+    CK(cudaStreamSynchronize(st));                                    /* the caller's dictionary buffer is pageable memory that may change after the call */
     d->dictSize = dictSize;
     return 0;
 }
@@ -774,10 +767,10 @@ extern "C" size_t ZSTD_decompress_usingDict(ZSTD_DCtx* d, void* dst, size_t dstC
     if (srcSize == 0) return 0;                                       /* zstd_decompress.c:1093 : an empty input is an empty output */
     if (!src) return ZB_ERR(ZB_error_srcSize_wrong);
     if (dstCapacity && !dst) return ZB_ERR(ZB_error_dstBuffer_null);
-    ZbdDeviceGuard guard;
-    {   size_t const e = zbd_ctxInit(d); if (zbd_isErr(e)) return e; }
+    ZbDeviceGuard guard;
+    {   size_t const e = zbd_ctxInit(d); if (zb_isErr(e)) return e; }
     memset(&d->stats, 0, sizeof(d->stats));
-    {   size_t const e = zbd_setDict(d, dict, dictSize, d->stream); if (zbd_isErr(e)) return e; }
+    {   size_t const e = zbd_setDict(d, dict, dictSize, d->stream); if (zb_isErr(e)) return e; }
     return zbd_decompressHost(d, dst, dstCapacity, src, srcSize);
 }
 extern "C" size_t ZSTD_decompressDCtx(ZSTD_DCtx* d, void* dst, size_t dstCapacity, const void* src, size_t srcSize)      /* lib/zstd.h:299 */
@@ -799,11 +792,11 @@ extern "C" size_t ZSTDB200_decompressDevice_usingDict(ZSTD_DCtx* d, void* d_dst,
 {
     if (!d) return ZB_ERR(ZB_error_GENERIC);
     if (srcSize == 0) return 0;
-    ZbdDeviceGuard guard;
-    {   size_t const e = zbd_ctxInit(d); if (zbd_isErr(e)) return e; }
+    ZbDeviceGuard guard;
+    {   size_t const e = zbd_ctxInit(d); if (zb_isErr(e)) return e; }
     memset(&d->stats, 0, sizeof(d->stats));
     cudaStream_t const st = stream ? (cudaStream_t)stream : d->stream;
-    {   size_t const e = zbd_setDict(d, dict, dictSize, st); if (zbd_isErr(e)) return e; }
+    {   size_t const e = zbd_setDict(d, dict, dictSize, st); if (zb_isErr(e)) return e; }
     return zbd_decompressDevice(d, d_dst, dstCapacity, d_src, srcSize, st);
 }
 extern "C" size_t ZSTDB200_decompressDevice(ZSTD_DCtx* d, void* d_dst, size_t dstCapacity, const void* d_src, size_t srcSize, void* stream)
