@@ -103,7 +103,7 @@ extern "C" size_t zbh_decompress_usingDict(void* dstv, size_t cap, const void* s
             if (b.type == ZB_BT_RLE) { if (out + b.rawSize > cap) return ERR(70); memset(dst + out, in[b.srcOff], b.rawSize); out += b.rawSize; continue; }
             BlockOut o;
             if (decodeLiterals(o, in, B, bi)) return ERR(ZBD_CORRUPT);
-            if (decodeSeqs(o, in, B, bi)) return ERR(ZBD_CORRUPT);
+            {   u32 const se = decodeSeqs(o, in, B, bi); if (se) return ERR(se); }          /* 20, or 16 for an offset beyond 28 bits */
             if (o.sumLL > b.litRegen) return ERR(ZBD_CORRUPT);
             size_t const regen = (size_t)b.litRegen + o.sumML;
             if (regen > ZB_BLOCK_MAX) return ERR(ZBD_CORRUPT);

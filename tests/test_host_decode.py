@@ -2,7 +2,8 @@
 same host+device functions the CUDA kernels call, block after block, and must reproduce the input of frames written by
 the reference encoder (every level, so Huffman treeless / FSE repeat modes, RLE tables, long offsets ...), by this repo's
 oracle, and of the reference's own golden decompression vectors (tests/golden/decompression*, copied from
-the reference tree's tests/golden-decompression*)."""
+the reference tree's tests/golden-decompression*).  Frames of chosen sequences and of the reference encoder's advanced
+parameters come from tests/seqgen.py."""
 import ctypes
 import glob
 import os
@@ -10,6 +11,7 @@ import subprocess
 
 import pytest
 
+import seqgen
 import zref
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -28,9 +30,14 @@ def H():
     return h
 
 
-def dec(H, frame, cap):
+def dec(H, frame, cap, d=None):
     out = ctypes.create_string_buffer(cap + 16)
-    r = H.zbh_decompress(out, cap, frame, len(frame))
+    if d is None:
+        r = H.zbh_decompress(out, cap, frame, len(frame))
+    else:
+        H.zbh_decompress_usingDict.restype = ctypes.c_size_t
+        H.zbh_decompress_usingDict.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_char_p, ctypes.c_size_t, ctypes.c_char_p, ctypes.c_size_t]
+        r = H.zbh_decompress_usingDict(out, cap, frame, len(frame), d, len(d))
     if r > (1 << 63):
         return ("ERR", (1 << 64) - r)
     return out.raw[:r]
@@ -155,3 +162,34 @@ def test_corrupted_frames_differential(H):
             assert ref is not None and ours == ref
             both += 1
     assert both > 100
+
+
+@needs_ref
+@pytest.mark.parametrize("name", sorted(seqgen.DICTATED))
+def test_dictated_sequences(H, name):
+    """frames of chosen sequences (tests/seqgen.py): every copy offset, length and alignment, every repcode form,
+    dependency chains, block and count extremes, a 1 KiB window, several frames in one call, matches that straddle the
+    dictionary's end.  The reference decoder must agree with the plain LZ77 execution, and so must the harness."""
+    frame, src, d = seqgen.DICTATED[name]()
+    assert seqgen.ref_decompress(frame, len(src), d) == src
+    assert dec(H, frame, len(src), d) == src
+
+
+@needs_ref
+@pytest.mark.parametrize("name", sorted(seqgen.ADVANCED))
+def test_advanced_parameter_frames(H, name):
+    """frames of the reference encoder's advanced parameters: no content size, streamed, checksums, hundreds of small
+    blocks, 1 KiB blocks and windows, raw or Huffman literals forced, level 22, long-distance matches of ~120 MiB"""
+    frame, src = seqgen.ADVANCED[name]()
+    assert seqgen.ref_decompress(frame, len(src)) == src
+    assert dec(H, frame, len(src)) == src
+
+
+@needs_ref
+@pytest.mark.parametrize("name", sorted(seqgen.REFUSED))
+def test_offsets_beyond_28_bits_refused(H, name):
+    """a window descriptor of 2^28, and a Single_Segment frame (it states no window) whose offsets need 29 bits: both
+    frameParameter_windowTooLarge (16), where the reference decoder takes them"""
+    frame, src = seqgen.REFUSED[name]()
+    assert seqgen.ref_decompress(frame, len(src)) == src
+    assert dec(H, frame, len(src)) == ("ERR", 16)

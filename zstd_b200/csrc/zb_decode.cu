@@ -7,6 +7,9 @@
  *   HUF_decompress4X1 / HUF_readDTableX1              (lib/decompress/huf_decompress.c:602, :383)
  * Any frame the format allows is accepted (this library's own and the reference encoder's, every level), window
  * sizes up to 128 MiB, raw-content and zstd-format dictionaries (ZSTD_decompress_usingDict, zstd_decompress.c:1133).
+ * Offsets are kept in 28 bits: a frame whose offsets need more than 27 bits gets frameParameter_windowTooLarge (16)
+ * whatever its header says (a window descriptor above 2^27 from the walk; a Single_Segment frame, which states no window,
+ * from the first such offset code).
  * The format-level functions are in zb_decode_core.cuh.
  *
  *   D0  walker    frames and blocks of the input: block headers, section headers, which earlier block a treeless /
@@ -201,6 +204,8 @@ zbd_scan_kernel(const ZbdBlock* __restrict__ blocks, u32 nbBlocks, const ZbdFram
         __syncthreads();
     }
     u64 const total = carry;
+    u32 const blockErr = firstErr;                                   /* a block that failed has no size: no content-size check over it hides its code */
+    __syncthreads();
     /* per frame: content size, start offset, repcode histories */
     for (u32 f = warp; f < nbFrames; f += SCAN_THREADS / 32u) {
         ZbdFrame const fr = frames[f];
@@ -221,7 +226,7 @@ zbd_scan_kernel(const ZbdBlock* __restrict__ blocks, u32 nbBlocks, const ZbdFram
             }
             if (k < fr.nbBlocks) { ZbdBlockOut& o = bout[fr.firstBlock + k]; o.start = mine; o.frameOff = fOff; }
         }
-        if (lane == 0 && fr.contentSize != ZBD_CONTENTSIZE_UNKNOWN) {
+        if (lane == 0 && !blockErr && fr.contentSize != ZBD_CONTENTSIZE_UNKNOWN) {
             u64 const end = (fr.firstBlock + fr.nbBlocks < nbBlocks) ? bout[fr.firstBlock + fr.nbBlocks].dstOff : total;
             if (end - fOff != fr.contentSize) atomicMax(&firstErr, ZBD_CORRUPT);
         }

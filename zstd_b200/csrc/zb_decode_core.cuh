@@ -521,7 +521,7 @@ ZBD_HD u64 zbd_packSeq(u32 offBase, u32 ll, u32 ml) { return (u64)offBase | ((u6
 /* ---- the sequence bitstream (format: "Sequences_Section", "Sequence Execution" reads these in order) ----
  * tables: LL / OF / ML decoding tables with their accuracy logs (0 for an RLE table).  Writes nbSeq packed sequences;
  * *sumLL / *sumML their totals; *transfer the repcode history at the block's end as a function of its start.
- * Returns 0 or ZBD_CORRUPT. */
+ * Returns 0, ZBD_CORRUPT, or 16 (frameParameter_windowTooLarge) for an offset code above 27. */
 ZBD_HDN u32 zbd_decodeSequences(u64* seqs, u32 nbSeq, const u8* p, u32 size, const u32* llT, u32 llLog, const u32* ofT, u32 ofLog,
                                 const u32* mlT, u32 mlLog, u32* sumLL, u32* sumML, ZbdRep* transfer)
 {
@@ -534,7 +534,7 @@ ZBD_HDN u32 zbd_decodeSequences(u64* seqs, u32 nbSeq, const u8* p, u32 size, con
         u32 const el = llT[sl], eo = ofT[so], em = mlT[sm];
         u32 const lc = ZBD_FSE_SYM(el), oc = ZBD_FSE_SYM(eo), mc = ZBD_FSE_SYM(em);
         if (oc > ZBD_OF_MAXSYM || lc > ZBD_LL_MAXSYM || mc > ZBD_ML_MAXSYM) return ZBD_CORRUPT;
-        if (oc > 27u) return ZBD_CORRUPT;                        /* offsets beyond 2^27: window sizes this decoder does not take */
+        if (oc > 27u) return 16u;                                 /* an offset of 2^28 or more: a window this decoder does not take, whatever the header says (frameParameter_windowTooLarge) */
         u32 const offBase = (1u << oc) + zbd_back_read(&bs, oc);
         u32 const ml = zbd_mlBase(mc) + zbd_back_read(&bs, zbd_mlBits(mc));
         u32 const ll = zbd_llBase(lc) + zbd_back_read(&bs, zbd_llBits(lc));
@@ -576,7 +576,7 @@ ZBD_HDN u32 zbd_walk(const u8* src, u64 size, ZbdBlock* blocks, u32 capB, ZbdFra
             pos += 8u + fh.contentSize;
             continue;
         }
-        if (fh.windowLog > 27u) return 16u;                       /* offsets are kept in 28 bits (a Single_Segment frame of any size is fine: offset codes above 27 are refused where they appear) */
+        if (fh.windowLog > 27u) return 16u;                       /* offsets are kept in 28 bits.  A Single_Segment frame states no window: any content size passes here, and an offset that needs more than 27 bits gets the same 16 from zbd_decodeSequences */
         ZbdFrame fr; memset(&fr, 0, sizeof(fr));
         fr.srcOff = pos; fr.contentSize = fh.contentSize; fr.windowSize = fh.windowSize; fr.firstBlock = nb;
         fr.hasChecksum = fh.hasChecksum; fr.dictID = fh.dictID;
