@@ -1,8 +1,8 @@
 """Test helpers for frames with chosen contents: a plain LZ77 executor (the reference answer), the reference encoder's
 sequence API (ZSTD_compressSequences, lib/zstd.h:1642) and advanced-parameter API (ZSTD_CCtx_setParameter,
 ZSTD_compress2, ZSTD_compressStream2), and a parser of frame and block headers that lets a test assert the frame has the
-shape it was built for.  Everything but execute() and frame_layout() needs oracle/_ref/libzstd_ref.so.  TEST
-INFRASTRUCTURE ONLY."""
+shape it was built for.  execute(), serial_codes(), frame_layout(), block_layout() and single_block_frame() work
+without the reference; everything else needs oracle/_ref/libzstd_ref.so.  TEST INFRASTRUCTURE ONLY."""
 import ctypes
 
 import numpy as np
@@ -58,15 +58,22 @@ def _check(R, r):
     return r
 
 
-def execute(blocks, rng, dict_content=b"", alphabet=256):
+def execute(blocks, rng, dict_content=b"", alphabet=256, literals=None):
     """The input a list of blocks describes.  blocks: [(sequences, trailing_literals)], a sequence is (litLength, offset,
-    matchLength).  Literal bytes are drawn from rng (numpy Generator) among the first `alphabet` byte values; a match
-    copies byte after byte, so it may overlap itself, and an offset beyond the output so far reads from the end of
-    dict_content."""
+    matchLength).  Literal bytes are taken in order from `literals` when it is given, else drawn from rng (numpy
+    Generator) among the first `alphabet` byte values; a match copies byte after byte, so it may overlap itself, and an
+    offset beyond the output so far reads from the end of dict_content."""
     h = bytearray(dict_content)
+    taken = 0
 
     def lits(n):
-        h.extend(rng.integers(0, alphabet, n, dtype="u1").tobytes())
+        nonlocal taken
+        if literals is None:
+            h.extend(rng.integers(0, alphabet, n, dtype="u1").tobytes())
+        else:
+            assert taken + n <= len(literals), (taken, n, len(literals))
+            h.extend(literals[taken:taken + n])
+            taken += n
     for seqs, trailing in blocks:
         for ll, off, ml in seqs:
             lits(ll)
@@ -78,7 +85,34 @@ def execute(blocks, rng, dict_content=b"", alphabet=256):
                 s += n
                 ml -= n
         lits(trailing)
+    assert literals is None or taken == len(literals), (taken, len(literals))
     return bytes(h[len(dict_content):])
+
+
+def serial_codes(offs, lls, hist):
+    """offBase of every sequence (1..3: a repeat offset, else offset + 3) and the repeat offsets after the last one, from
+    the real offsets and literal lengths and the history `hist` (r1, r2, r3) in front of them: ZSTD_updateRep + the offBase
+    choice of ZSTD_storeSeq, one sequence after the other (what zb_rep_code() of zb_match.cu computes)."""
+    r1, r2, r3 = hist
+    out = []
+    for off, ll in zip(offs, lls):
+        off = int(off)
+        if ll > 0:
+            if off == r1:
+                out.append(1); continue
+            if off == r2:
+                out.append(2); r1, r2 = off, r1; continue
+            if off == r3:
+                out.append(3); r1, r2, r3 = off, r1, r2; continue
+        else:
+            if off == r2:
+                out.append(1); r1, r2 = off, r1; continue
+            if off == r3:
+                out.append(2); r1, r2, r3 = off, r1, r2; continue
+            if r1 > 1 and off == r1 - 1:
+                out.append(3); r1, r2, r3 = off, r1, r2; continue
+        out.append(off + 3); r1, r2, r3 = off, r1, r2
+    return out, (r1, r2, r3)
 
 
 def dict_content(d):
@@ -198,6 +232,45 @@ def frame_layout(buf):
         f["size"] = pos - start
         frames.append(f)
     return frames
+
+
+def block_layout(body):
+    """The headers of a compressed block's body (format: "Literals_Section_Header", "Huffman_Tree_Description",
+    "Sequences_Section_Header"): lit_type (0 raw, 1 RLE, 2 compressed, 3 treeless), lit_size, lit_header (bytes),
+    streams (1 or 4, None unless Huffman), huf_desc ("fse", "direct", or None where the block carries no tree),
+    nb_seq, nb_seq_bytes, and modes = (LL, OF, ML) (0 predefined, 1 RLE, 2 compressed, 3 repeat; None without
+    sequences)."""
+    lt, sf = body[0] & 3, (body[0] >> 2) & 3
+    out = {"lit_type": lt, "streams": None, "huf_desc": None}
+    if lt < 2:
+        hs = (1, 2, 1, 3)[sf]
+        out["lit_size"] = int.from_bytes(body[:hs], "little") >> (3 if hs == 1 else 4)
+        s = hs + (out["lit_size"] if lt == 0 else 1)
+    else:
+        hs = (3, 3, 4, 5)[sf]
+        v = int.from_bytes(body[:hs], "little") >> 4
+        bits = (10, 10, 14, 18)[sf]
+        out["lit_size"], out["streams"] = v & ((1 << bits) - 1), 1 if sf == 0 else 4
+        if lt == 2:
+            out["huf_desc"] = "fse" if body[hs] < 128 else "direct"
+        s = hs + (v >> bits)
+    out["lit_header"] = hs
+    c = body[s]
+    out["nb_seq"] = c if c < 128 else (((c - 128) << 8) + body[s + 1] if c < 255 else body[s + 1] + (body[s + 2] << 8) + 0x7F00)
+    out["nb_seq_bytes"] = 1 if c < 128 else (2 if c < 255 else 3)
+    m = body[s + out["nb_seq_bytes"]] if out["nb_seq"] else None
+    out["modes"] = (m >> 6, (m >> 4) & 3, (m >> 2) & 3) if out["nb_seq"] else None
+    return out
+
+
+def single_block_frame(btype, body, size):
+    """A Single_Segment frame whose only block is `body` (type btype: the byte of an RLE block, the input of a raw one),
+    of `size` bytes of content; it states no dictionary ID, so the decoder takes the dictionary it is given."""
+    fcs = 0 if size < 256 else (1 if size < 65536 + 256 else 2)
+    hdr = (0xFD2FB528).to_bytes(4, "little") + bytes([0x20 | (fcs << 6)])
+    hdr += size.to_bytes(1, "little") if fcs == 0 else ((size - 256).to_bytes(2, "little") if fcs == 1 else size.to_bytes(4, "little"))
+    bh = 1 | (btype << 1) | ((size if btype == BT_RLE else len(body)) << 3)
+    return hdr + bh.to_bytes(3, "little") + body
 
 
 # ---------------------------------------------------------------------------------------------------- the cases

@@ -10,31 +10,9 @@
 import numpy as np
 import pytest
 
+from seqgen import serial_codes
+
 TILE = 1024
-
-
-def serial_codes(offs, lls, hist):
-    """zb_rep_code() of zb_match.cu == ZSTD_updateRep + the offBase choice of ZSTD_storeSeq, one sequence after the other."""
-    r1, r2, r3 = hist
-    out = []
-    for off, ll in zip(offs, lls):
-        off = int(off)
-        if ll > 0:
-            if off == r1:
-                out.append(1); continue
-            if off == r2:
-                out.append(2); r1, r2 = off, r1; continue
-            if off == r3:
-                out.append(3); r1, r2, r3 = off, r1, r2; continue
-        else:
-            if off == r2:
-                out.append(1); r1, r2 = off, r1; continue
-            if off == r3:
-                out.append(2); r1, r2, r3 = off, r1, r2; continue
-            if r1 > 1 and off == r1 - 1:
-                out.append(3); r1, r2, r3 = off, r1, r2; continue
-        out.append(off + 3); r1, r2, r3 = off, r1, r2
-    return out, (r1, r2, r3)
 
 
 def last_flag_before(flags):

@@ -317,12 +317,6 @@ static size_t zb_ensureDesc(ZSTD_CCtx* c, size_t nbBlocks, size_t nbFrames, size
     }
     return 0;
 }
-static ZbStrides zb_strides(u32 maxBlock)
-{
-    u32 const M = ((maxBlock < 64u ? 64u : maxBlock) + 63u) & ~63u;
-    ZbStrides sd; sd.dist = M; sd.seq = M / 4u + 8u; sd.lit = M + 256u; sd.body = M + 1024u; sd.state = M / 4u;
-    return sd;
-}
 /* workspace for nbSlotBlocks blocks laid out with the strides `sd` (capacities are kept in bytes) */
 static size_t zb_ensureHeavy(ZSTD_CCtx* c, size_t nbSlotBlocks, const ZbStrides& sd, bool needDist2)
 {

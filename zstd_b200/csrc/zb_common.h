@@ -159,6 +159,23 @@ typedef struct {
 } ZbStrides;
 
 #ifdef __CUDACC__
+#define ZB_HD __host__ __device__
+#else
+#define ZB_HD
+#endif
+static inline ZB_HD ZbStrides zb_strides(u32 maxBlock)
+{
+    u32 const M = ((maxBlock < 64u ? 64u : maxBlock) + 63u) & ~63u;
+    ZbStrides sd; sd.dist = M; sd.seq = M / 4u + 8u; sd.lit = M + 256u; sd.body = M + 1024u; sd.state = M / 4u;
+    return sd;
+}
+/* a final sequence as the sequences kernel reads it: offBase (24 bits), literal length (18 bits), match length (>= 4) */
+static inline ZB_HD u64 zb_pack_seq(u32 offBase, u32 litLen, u32 matchLen)
+{
+    return (u64)offBase | ((u64)litLen << 24) | ((u64)matchLen << 42);
+}
+
+#ifdef __CUDACC__
 /* host helpers of the compression and decompression drivers (zb_api.cu, zb_decode.cu) */
 #include <cuda_runtime.h>
 #include <stdio.h>

@@ -68,11 +68,6 @@ __device__ __forceinline__ u64 zb_pack_raw(u32 off, u32 mlen, u32 msRel) { retur
 #define ZB_RAW_OFF(r)  ((u32)(r) & 0xFFFFFFu)
 #define ZB_RAW_MLEN(r) ((u32)((r) >> 24) & 0x3FFFFu)
 #define ZB_RAW_MS(r)   ((u32)((r) >> 42))
-/* final sequence, read by the sequences kernel */
-__device__ __forceinline__ u64 zb_pack_seq(u32 offBase, u32 litLen, u32 matchLen)
-{
-    return (u64)offBase | ((u64)litLen << 24) | ((u64)matchLen << 42);
-}
 
 /* ------------------------------------------------------------------------------------------------
  * K1a — candidate walk (parse-independent).  One CTA per chunk, table in shared memory.
