@@ -71,6 +71,7 @@ static size_t fse_decodeWeights(u8* out, size_t maxOut, const u8* src, size_t sr
         bitpos = (long)(n - 1) * 8 + (long)hb32(bs[n - 1]);          /* bits below the end mark */
 #define RD(k) ({ u32 v_ = 0; for (u32 i_ = 0; i_ < (k); i_++) { long const bp_ = bitpos - (long)(k) + (long)i_; if (bp_ >= 0) v_ |= (u32)((bs[bp_ >> 3] >> (bp_ & 7)) & 1) << i_; } bitpos -= (long)(k); v_; })
         s1 = RD(tableLog); s2 = RD(tableLog);
+        if (bitpos < 0) return 0;                                         /* shorter than its two initial states (fse_decompress.c:193) */
         while (1) {
             if (op + 2 > maxOut) return 0;
             out[op++] = dt[s1].sym; s1 = dt[s1].newState + RD(dt[s1].nbBits);

@@ -3,9 +3,14 @@ Frames must decode with the reference's ZSTD_decompress_usingDict and stay withi
 reference's size for raw-content and zstd-format dictionaries; the dictionary entropy stage (treeless
 literals, set_repeat tables, start repcodes) is pinned byte-for-byte against ZSTD_loadCEntropy +
 ZSTD_entropyCompressSeqStore of the compiled reference."""
+import ctypes
+import random
+
 import pytest
 
 import zref
+import zstd_b200
+from test_host_decode import H, dec  # noqa: F401  (H: the CPU decode harness fixture)
 
 needs_ref = pytest.mark.skipif(not zref.have_ref(), reason="oracle/_ref/libzstd_ref.so not built")
 REC = 1024
@@ -137,3 +142,120 @@ def test_size_parity_with_reference_cdict(level):
         tot_o += len(f)
     tot_r = sum(len(f) for f in ref_frames)
     assert abs(tot_o - tot_r) / tot_r <= 0.01, (tot_o, tot_r)
+
+
+def _huf_desc_len(d):
+    """bytes of the Huffman tree description at d[8:] (format: "Huffman Tree Description")"""
+    hb = d[8]
+    return 1 + (hb - 127 + 1) // 2 if hb >= 128 else 1 + hb
+
+
+def _oracle_load(d):
+    """zbo_loadDictEntropy: the content offset, or an error code (> 2^63)"""
+    O = zref.oracle()
+    O.zbo_loadDictEntropy.restype = ctypes.c_size_t
+    O.zbo_loadDictEntropy.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t]
+    return O.zbo_loadDictEntropy(ctypes.create_string_buffer(16384), d, len(d))
+
+
+def _cdict_decisions(dicts):
+    """(product, oracle, reference) for every dictionary: accepted (True) or refused by the product's ZSTD_createCDict, the
+    oracle's zbo_loadDictEntropy and the reference's ZSTD_createCDict"""
+    L, R = zstd_b200.lib(), zref.ref()
+    L.ZSTD_freeCDict.argtypes = [ctypes.c_void_p]
+    R.ZSTD_createCDict.restype = ctypes.c_void_p
+    R.ZSTD_createCDict.argtypes = [ctypes.c_char_p, ctypes.c_size_t, ctypes.c_int]
+    R.ZSTD_freeCDict.argtypes = [ctypes.c_void_p]
+    out = []
+    for d in dicts:
+        ours = L.ZSTD_createCDict(d, len(d), 1)
+        L.ZSTD_freeCDict(ours)
+        ref = R.ZSTD_createCDict(d, len(d), 1)
+        R.ZSTD_freeCDict(ref)
+        out.append((bool(ours), _oracle_load(d) < (1 << 63), bool(ref)))
+    return out
+
+
+def _mutants(d, n, seed):
+    """n byte flips, bit flips and truncations across the entropy header (everything in front of the content) of d"""
+    end = _oracle_load(d)
+    assert 8 < end < len(d)
+    rng = random.Random(seed)
+    out = []
+    for _ in range(n):
+        b = bytearray(d)
+        kind = rng.random()
+        if kind < 0.15:
+            out.append(bytes(b[:rng.randrange(8, end + 16)]))
+            continue
+        for _ in range(2 if kind > 0.85 else 1):
+            p = rng.randrange(8, end)
+            b[p] ^= (1 << rng.randrange(8)) if kind < 0.4 else rng.randrange(1, 256)
+        out.append(bytes(b))
+    return out
+
+
+def corrupted_dictionaries():
+    """the seeded corpus: 2500 mutants of each of the three golden zstd-format dictionaries and of a trained one"""
+    train = zref.train_dict(zref.synthetic(1024 * 2000, 11), 1024, 2000, 8 << 10)
+    dicts = [zref.golden_input(n) for n in ("zdict-16k-synthetic-seed77", "http-dict-missing-symbols", "zero-weight-dict")] + [train]
+    return [_mutants(d, 2500, k) for k, d in enumerate(dicts)]
+
+
+@needs_ref
+def test_corrupted_dictionaries_refused_as_the_reference_refuses():
+    """the product's ZSTD_createCDict (which reads the format with the decoder's code, zb_decode_core.cuh) and the oracle
+    refuse exactly the zstd-format dictionaries the reference's ZSTD_createCDict refuses"""
+    for k, corpus in enumerate(corrupted_dictionaries()):
+        got = _cdict_decisions(corpus)
+        differ = [(i, g) for i, g in enumerate(got) if len(set(g)) > 1]
+        assert not differ, (k, len(differ), [(corpus[i][:40].hex(), g) for i, g in differ[:5]])
+        accepted = sum(g[0] for g in got)
+        assert 100 < accepted < len(corpus) - 100, (k, accepted)
+
+
+def _fse_description(norm, table_log):
+    """FSE table description of normalised counts, written by the reference's FSE_writeNCount"""
+    R = zref.ref()
+    R.FSE_writeNCount.restype = ctypes.c_size_t
+    R.FSE_writeNCount.argtypes = [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_uint, ctypes.c_uint]
+    n = (ctypes.c_short * len(norm))(*norm)
+    buf = ctypes.create_string_buffer(512)
+    r = R.FSE_writeNCount(buf, 512, n, len(norm) - 1, table_log)
+    assert not R.ZSTD_isError(r)
+    return buf.raw[:r]
+
+
+def _weights4(weights):
+    """Huffman tree description with 4-bit weights"""
+    w = list(weights) + [0]
+    return bytes([127 + len(weights)]) + bytes(w[i] << 4 | w[i + 1] for i in range(0, len(weights), 2))
+
+
+def _weightsFse(last_symbol, stream):
+    """Huffman tree description with FSE-compressed weights: 32 states, symbol 1 in all but the top one, which belongs to
+    last_symbol.  State 0 is the only one that reads a bit, so the stream of bytes 00 04 (initial states 0 and 0, then that
+    bit) decodes to the weights 1, 1 (and the implied last weight 2)."""
+    norm = [0, 31] + [0] * (last_symbol - 2) + [-1]
+    nc = _fse_description(norm, 5)
+    return bytes([len(nc) + len(stream)]) + nc + stream
+
+
+@needs_ref
+@pytest.mark.parametrize("row", [1, 2, 3, 4])
+def test_rules_where_compressor_and_decoder_differ(H, row):  # noqa: F811
+    """one hand-built dictionary per rule where the compressor's and the decoder's readers of a dictionary's Huffman tree
+    description differ (both read it with zbd_readHufWeights, with their own limits); the tables behind it are those of a
+    golden dictionary.  Accepted by the compressor, the oracle and the reference alike:
+      1: weights and table log of 12 (HUF_TABLELOG_MAX); the decoder's tables stop at 11: it refuses.
+      2: the weights' FSE description gives a probability to symbol 13, which no decoded weight uses.  The reference reads
+         these descriptions over 256 symbols, the decoder over 13: it refuses.
+    Refused by the compressor, the oracle and the reference alike:
+      3: a weight bitstream shorter than its two initial states (fse_decompress.c:193); the decoder refuses it too.
+      4: no weight of 1 (HUF_readStats: rank[1] >= 2); the decoder does not check, and accepts."""
+    g = zref.golden_input("zdict-16k-synthetic-seed77")
+    huf = {1: _weights4(range(12, 0, -1)), 2: _weightsFse(13, b"\x00\x04"), 3: _weightsFse(2, b"\x01"), 4: _weights4([2, 2, 2])}[row]
+    d = g[:8] + huf + g[8 + _huf_desc_len(g):]
+    [(ours, oracle, ref)] = _cdict_decisions([d])
+    assert ours == oracle == ref == (row in (1, 2))
+    assert dec(H, zref.ref_compress(b"", 1), 0, d) == (b"" if row == 4 else ("ERR", 30))

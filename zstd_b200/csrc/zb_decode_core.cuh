@@ -13,7 +13,7 @@
 
 #ifdef __CUDACC__
 #define ZBD_HD __host__ __device__ __forceinline__
-#define ZBD_HDN __host__ __device__
+#define ZBD_HDN static __host__ __device__        /* internal linkage: more than one .cu file includes this header */
 #else
 #define ZBD_HD static inline
 #define ZBD_HDN static
@@ -27,6 +27,7 @@
 #define ZBD_MAGIC 0xFD2FB528u
 #define ZBD_MAGIC_SKIPPABLE 0x184D2A50u   /* .. 0x184D2A5F */
 #define ZBD_HUF_LOG_MAX 11u
+#define ZBD_HUF_WEIGHT_MAXSYM 12u       /* largest symbol the FSE description of Huffman weights may hold */
 #define ZBD_LL_LOG_MAX 9u
 #define ZBD_OF_LOG_MAX 8u
 #define ZBD_ML_LOG_MAX 9u
@@ -373,9 +374,12 @@ ZBD_HD short zbd_defaultNorm(u32 stream, u32 s)
 }
 
 /* ---- Huffman tree description (format: "Huffman Tree Description") ----
- * weights[0 .. *nbSym) receive every symbol's weight incl. the implied last one; fseTable / norm / next are scratch
- * (64 u32, 16 short, 16 u16).  Returns the bytes of the description (> 0), or 0 on corruption. */
-ZBD_HDN u32 zbd_readHufWeights(u8* weights, u32* nbSymPtr, u32* logPtr, const u8* p, u32 avail, u32* fseTable, short* norm, u16* next)
+ * weights[0 .. *nbSym) receive every symbol's weight incl. the implied last one.  fseTable / norm / next are scratch (64
+ * u32, fseMaxSym + 1 short and u16).  maxLog: the largest weight and table log taken; fseMaxSym: the largest symbol the
+ * weights' FSE description may hold.  The defaults are the decoder's; the compressor reads dictionaries with the
+ * reference's limits (zb_dict.cu).  Returns the bytes of the description (> 0), or 0 on corruption. */
+ZBD_HDN u32 zbd_readHufWeights(u8* weights, u32* nbSymPtr, u32* logPtr, const u8* p, u32 avail, u32* fseTable, short* norm, u16* next,
+                               u32 maxLog = ZBD_HUF_LOG_MAX, u32 fseMaxSym = ZBD_HUF_WEIGHT_MAXSYM)
 {
     if (avail < 1) return 0;
     u32 const hb = p[0];
@@ -389,7 +393,7 @@ ZBD_HDN u32 zbd_readHufWeights(u8* weights, u32* nbSymPtr, u32* logPtr, const u8
         used = 1u + hb;
         if (hb == 0 || used > avail) return 0;
         u32 maxSym = 0, log = 0;
-        u32 const nc = zbd_readNCount(norm, &maxSym, &log, 12u, 6u, p + 1, hb);
+        u32 const nc = zbd_readNCount(norm, &maxSym, &log, fseMaxSym, 6u, p + 1, hb);
         if (nc == 0 || nc >= hb) return 0;
         zbd_buildFseTable(fseTable, norm, maxSym, log, next);
         ZbdBack bs;
@@ -409,10 +413,10 @@ ZBD_HDN u32 zbd_readHufWeights(u8* weights, u32* nbSymPtr, u32* logPtr, const u8
     }
     /* the last weight completes the sum of 2^(w-1) to a power of two */
     u32 total = 0;
-    for (u32 i = 0; i < n; i++) { if (weights[i] > ZBD_HUF_LOG_MAX) return 0; total += weights[i] ? (1u << (weights[i] - 1u)) : 0u; }
+    for (u32 i = 0; i < n; i++) { if (weights[i] > maxLog) return 0; total += weights[i] ? (1u << (weights[i] - 1u)) : 0u; }
     if (total == 0) return 0;
     u32 const log = zbd_hb(total) + 1u;
-    if (log > ZBD_HUF_LOG_MAX) return 0;
+    if (log > maxLog) return 0;
     u32 const rest = (1u << log) - total;
     if (rest & (rest - 1u)) return 0;                             /* not a power of two */
     weights[n++] = (u8)(zbd_hb(rest) + 1u);
@@ -645,15 +649,18 @@ typedef struct {
     u32 pad;
 } ZbdDictInfo;
 #define ZBD_MAGIC_DICT 0xEC30A437u
-/* returns 0, or 30 (dictionary_corrupted) */
-ZBD_HDN u32 zbd_parseDict(ZbdDictInfo* di, const u8* dict, u64 size)
+/* hufMaxLog / hufFseMaxSym (<= 255): the limits of the Huffman tree description, as zbd_readHufWeights takes them (the
+ * defaults are the decoder's).
+ * Returns 0, or 30 (dictionary_corrupted). */
+ZBD_HDN u32 zbd_parseDict(ZbdDictInfo* di, const u8* dict, u64 size, u32 hufMaxLog = ZBD_HUF_LOG_MAX, u32 hufFseMaxSym = ZBD_HUF_WEIGHT_MAXSYM)
 {
     memset(di, 0, sizeof(*di));
     if (size < 8 || zbd_le(dict, 4) != ZBD_MAGIC_DICT) return ZBD_OK;          /* raw content */
     di->entropy = 1; di->dictID = zbd_le(dict + 4, 4);
     u32 p = 8;
-    {   u8 weights[256]; u32 nbSym, log; u32 fse[64]; short norm[16]; u16 next[16];
-        u32 const used = zbd_readHufWeights(weights, &nbSym, &log, dict + p, (u32)(size - p > 0xFFFFu ? 0xFFFFu : size - p), fse, norm, next);
+    {   u8 weights[256]; u32 nbSym, log; u32 fse[64]; short norm[256]; u16 next[256];
+        u32 const used = zbd_readHufWeights(weights, &nbSym, &log, dict + p, (u32)(size - p > 0xFFFFu ? 0xFFFFu : size - p), fse, norm, next,
+                                            hufMaxLog, hufFseMaxSym);
         if (!used) return 30u;
         di->hufOff = p; di->hufLen = used; p += used; }
     u32 const order[3] = { 1u, 2u, 0u };                                        /* the file holds OF, ML, LL */
