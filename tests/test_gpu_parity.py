@@ -266,6 +266,94 @@ def test_many_records_with_cdict(ctx):
     cd.close()
 
 
+def _batch(c, src, sizes, level=1, dict_bytes=None, cdict=None):
+    """one batch call over host buffers, with a raw dictionary, a CDict or neither: the list of frames"""
+    offs = [sum(sizes[:i]) for i in range(len(sizes))]
+    cap = sum(zstd_b200.ZSTD_compressBound(n) + 32 for n in sizes)
+    dst = ctypes.create_string_buffer(cap)
+    sbuf = ctypes.create_string_buffer(src, max(len(src), 1))
+    if cdict is None:
+        total, csz = c.compress_frames(ctypes.addressof(dst), cap, ctypes.addressof(sbuf), offs, sizes, level=level,
+                                       device_memory=False, dict_bytes=dict_bytes)
+    else:
+        total, csz = c.compress_frames_using_cdict(ctypes.addressof(dst), cap, ctypes.addressof(sbuf), offs, sizes, cdict, device_memory=False)
+    assert sum(csz) == total
+    return [dst.raw[sum(csz[:i]):sum(csz[:i + 1])] for i in range(len(sizes))]
+
+
+def _check_frames(frames, src, sizes, dict_bytes, level=1):
+    """every frame equals the oracle's and, where the reference is built, decodes with the reference decoder"""
+    pos = 0
+    for i, (frame, n) in enumerate(zip(frames, sizes)):
+        part = src[pos:pos + n]
+        pos += n
+        if dict_bytes is None:
+            assert frame == zref.oracle_compress(part, level), i
+            decode_ok(frame, part)
+        else:
+            assert frame == zref.oracle_compress_using_dict(part, dict_bytes, level), i
+            if zref.have_ref():
+                assert zref.ref_decompress_using_dict(frame, dict_bytes, n) == part, i
+
+
+def test_raw_dictionaries_switch_on_one_context():
+    """Batch calls of 16 frames on one context, each against another dictionary of the same size (two raw ones, then a
+    zstd-format one): nothing of a call's dictionary (content tail, entropy tables, table images) carries over into the next
+    call, also when the caller rewrites one buffer in place between the calls"""
+    n = 16 << 10
+    dicts = [zref.synthetic(n, 501, 0.5), zref.synthetic(n, 502, 0.5), zref.golden_input("zdict-16k-synthetic-seed77")]
+    assert all(len(d) == n for d in dicts)
+    # every frame holds pieces of all three dictionaries' content
+    src = b"".join(dicts[0][k * 900:k * 900 + 340] + dicts[1][k * 900:k * 900 + 340] + dicts[2][n - (k + 1) * 900:][:344] for k in range(16))
+    sizes = [1024] * 16
+    c = zstd_b200.ZSTD_CCtx()
+    for d in dicts:
+        _check_frames(_batch(c, src, sizes, dict_bytes=d), src, sizes, d)
+    buf = bytearray(n)
+    for d in dicts + dicts[:1]:
+        buf[:] = d
+        _check_frames(_batch(c, src, sizes, dict_bytes=buf), src, sizes, d)
+    c.close()
+
+
+def test_dictionary_parameter_groups_beyond_image_slots():
+    """A batch call whose frames fall into six parameter groups (window logs 14 to 19 with the 16 KiB dictionary at level
+    1), twice over: more groups than a dictionary has table-image slots.  The groups without an image walk the dictionary per
+    frame; the raw dictionary and the CDict give the same bytes, equal to the oracle's."""
+    d = zref.golden_input("zdict-16k-synthetic-seed77")
+    sizes = [0, 1000, 20_000, 60_000, 150_000, 400_000] * 2
+    src = b"".join((d[-2000:] + zref.synthetic(n, 80 + i, 0.5))[:n] for i, n in enumerate(sizes))
+    c = zstd_b200.ZSTD_CCtx()
+    raw = _batch(c, src, sizes, dict_bytes=d)
+    _check_frames(raw, src, sizes, d)
+    cd = zstd_b200.ZSTD_CDict(d, 1)
+    for _ in range(2):                                      # the second call finds the images the first one built
+        assert _batch(c, src, sizes, cdict=cd) == raw
+    cd.close()
+    c.close()
+
+
+def test_cdict_raw_dictionary_and_no_dictionary_in_turn():
+    """A CDict call, a raw-dictionary call and a call without a dictionary, in turn on one context, as batches of 9 frames
+    and as single frames: each equals the oracle's frames, so no call sees the dictionary of the call before"""
+    d_cd = zref.golden_input("zdict-16k-synthetic-seed77")
+    d_raw = zref.synthetic(16 << 10, 503, 0.5)
+    sizes = [1024] * 8 + [5000]
+    src = b"".join((d_cd[-(k + 1) * 1500:][:600] + d_raw[k * 1500:k * 1500 + 600] + zref.synthetic(n, 90 + k, 0.5))[:n] for k, n in enumerate(sizes))
+    c = zstd_b200.ZSTD_CCtx()
+    cd = zstd_b200.ZSTD_CDict(d_cd, 1)
+    for _ in range(2):
+        _check_frames(_batch(c, src, sizes, cdict=cd), src, sizes, d_cd)
+        _check_frames(_batch(c, src, sizes, dict_bytes=d_raw), src, sizes, d_raw)
+        _check_frames(_batch(c, src, sizes), src, sizes, None)
+        part = src[:sizes[0]]
+        assert c.compress_using_cdict(part, cd) == zref.oracle_compress_using_dict(part, d_cd, 1)
+        assert c.compress_using_dict(part, d_raw, 1) == zref.oracle_compress_using_dict(part, d_raw, 1)
+        assert c.compress(part, 1) == zref.oracle_compress(part, 1)
+    cd.close()
+    c.close()
+
+
 def test_cdict_errors():
     bad = bytearray(zref.golden_input("zdict-16k-synthetic-seed77")); bad[12:40] = b"\xff" * 28      # entropy tables destroyed
     with pytest.raises(zstd_b200.ZstdError):
