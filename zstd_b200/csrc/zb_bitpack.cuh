@@ -31,27 +31,6 @@ __device__ __forceinline__ void zbd_pw_add(ZbdParW* w, u32 value, u32 nbBits)
         w->nacc -= 32u;
     }
 }
-/* the same in two halves for short fields (Huffman codes, <= 12 bits): zbd_pw_put only accumulates, zbd_pw_flush — due at
- * least once per two fields: fewer than 32 bits stay behind a flush, 32 + 2 * 12 < 64 — emits a word when one is full.
- * Written without branches: lanes of a warp fill their words at different moments, a branch would make every lane's
- * iteration pay for the emit path. */
-__device__ __forceinline__ void zbd_pw_put(ZbdParW* w, u32 value, u32 nbBits)
-{
-    w->acc |= (u64)value << w->nacc;
-    w->nacc += nbBits;
-}
-__device__ __forceinline__ void zbd_pw_flush(ZbdParW* w)
-{
-    bool const full = w->nacc >= 32u;
-    u32 const lo = (u32)w->acc;
-    u32* const wp = w->words + w->widx;
-    if (full && w->first == 0u) *wp = lo;
-    if (full && w->first != 0u) atomicOr(wp, lo);
-    w->first = full ? 0u : w->first;
-    w->widx += full ? 1u : 0u;
-    w->acc = full ? (w->acc >> 32) : w->acc;
-    w->nacc -= full ? 32u : 0u;
-}
 __device__ __forceinline__ void zbd_pw_finish(ZbdParW* w)
 {
     u32 const lo = (u32)w->acc;

@@ -2,55 +2,53 @@
  *
  * Replaces ZSTD_compressLiterals (lib/compress/zstd_compress_literals.c:129-235)
  * and HUF_compress_internal (huf_compress.c:1333-1430) for a fresh entropy state:
- *   1. 256-bin histogram: per-warp privatised bins in shared memory + merge (hist.c:66-133)
+ *   1. 256-bin histogram: warp w counts the bytes of Huffman stream w into its own shared-memory bins, count[] is the sum
+ *      of the four (hist.c:66-133)
  *   2. raw / RLE / compressed decision with the reference's thresholds
  *   3. Huffman table + tree description: the whole CTA (zb_entropy.cuh)
- *   4. 1 or 4 streams (huf_compress.c:1056-1118, :1168-1215): every thread owns a contiguous run of
- *      symbols, a suffix sum over per-thread bit counts gives its bit offset (streams grow from the
- *      LAST symbol), then bits are packed straight into the output words (edge words by atomicOr).
+ *   4. 1 or 4 streams (huf_compress.c:1056-1118, :1168-1215): a stream's size is its histogram dotted with the code
+ *      lengths, so every size and offset is known before any packing; then warp s encodes stream s in one pass
+ *      (zb_huf_stream).
  * Output: body[0 .. litSecSize) of the block's staging area; meta.litSecSize.
  */
 #include "zb_entropy.cuh"
 #include "zb_kernels.h"
-#include "zb_bitpack.cuh"
 
-#ifndef LIT_THREADS
-#define LIT_THREADS 128
-#endif
+#define LIT_THREADS 128               /* one warp per Huffman stream */
 #ifndef LIT_MIN_CTAS
-#define LIT_MIN_CTAS 12               /* 16 (32 registers) measured slower on the H100: literals 2.90 vs 2.68 ms per GiB of config 2 */
+#define LIT_MIN_CTAS 12               /* 40 registers.  H100, literals per GiB of config 2: 8 CTAs (56 registers) 1.35-1.37 ms,
+                                       * 10 (48) 1.39-1.40, 12 1.39-1.41, and the same wave totals; on config 5 (1 KiB blocks)
+                                       * 8 took 6.52 ms against 6.36.  16 would spill at 32 registers. */
 #endif
 #define LIT_WARPS (LIT_THREADS / 32)
-#ifndef LIT_PACK2
-#define LIT_PACK2 1                   /* the stream packer looks for a full word once per two codes, without a branch */
-#endif
-#ifndef LIT_AHEAD
-#define LIT_AHEAD 2                   /* 16-byte vectors of a thread's run requested ahead of the one in use */
-#endif
+#define LIT_WIN 256u                  /* words of a warp's encoding window: a tile adds at most 512 codes x 12 bits = 192 words */
 
-/* block-wide histogram of src[0..n) into count[256]; returns nothing, count valid after the call */
-__device__ void zb_hist256(const u8* __restrict__ src, u32 n, u32 (*whist)[256], u32* count)   /* whist: LIT_WARPS private histograms */
+/* histogram of src[0..n) into count[256]; warp w counts the bytes [w * seg, (w + 1) * seg), seg = ceil(n / 4), into
+ * whist[w]: over a literal buffer of four Huffman streams, whist[w] is stream w's histogram.  16-byte aligned vector
+ * loads, bytes outside the warp's range masked. */
+__device__ void zb_hist256(const u8* __restrict__ src, u32 n, u32 (*whist)[256], u32* count)
 {
-    u32 const tid = threadIdx.x, warp = tid >> 5;
+    u32 const tid = threadIdx.x, warp = tid >> 5, lane = tid & 31u;
     for (u32 i = tid; i < LIT_WARPS * 256; i += LIT_THREADS) (&whist[0][0])[i] = 0;
     __syncthreads();
-    u32 const head = (u32)((16u - ((uintptr_t)src & 15u)) & 15u);       /* bytes before 16-byte alignment */
-    u32 const headN = head < n ? head : n;
-    if (tid < headN) atomicAdd(&whist[warp][src[tid]], 1u);
-    u32 const nvec = (n - headN) / 16u;
-    const uint4* v4 = reinterpret_cast<const uint4*>(src + headN);
-    for (u32 i = tid; i < nvec; i += LIT_THREADS) {
-        uint4 const q = __ldg(v4 + i);
-        u32 w[4] = { q.x, q.y, q.z, q.w };
+    u32 const head = (u32)((uintptr_t)src & 15u);                      /* src[i] is byte i + head of the vectors */
+    const uint4* const v4 = reinterpret_cast<const uint4*>(src - head);
+    u32 const seg = (n + 3u) / 4u;
+    u32 const beg = min(warp * seg, n) + head, end = min((warp + 1u) * seg, n) + head;
+    if (beg < end) {
+        u32 const vLo = beg >> 4, nVec = ((end - 1u) >> 4) - vLo + 1u;
+        uint4 nx = lane < nVec ? __ldg(v4 + vLo + lane) : make_uint4(0, 0, 0, 0);
+        for (u32 i = lane; i < nVec; i += 32u) {
+            uint4 const q = nx;
+            if (i + 32u < nVec) nx = __ldg(v4 + vLo + i + 32u);
+            u32 const p0 = (vLo + i) << 4;
+            u32 const kLo = beg > p0 ? beg - p0 : 0u, kHi = min(end - p0, 16u);     /* bytes [kLo, kHi) are the warp's */
+            u32 const w[4] = { q.x, q.y, q.z, q.w };
 #pragma unroll
-        for (int k = 0; k < 4; k++) {
-            atomicAdd(&whist[warp][w[k] & 0xFF], 1u);
-            atomicAdd(&whist[warp][(w[k] >> 8) & 0xFF], 1u);
-            atomicAdd(&whist[warp][(w[k] >> 16) & 0xFF], 1u);
-            atomicAdd(&whist[warp][w[k] >> 24], 1u);
+            for (u32 k = 0; k < 16u; k++)
+                if (k >= kLo && k < kHi) atomicAdd(&whist[warp][(w[k >> 2] >> (8u * (k & 3u))) & 0xFFu], 1u);
         }
     }
-    for (u32 i = headN + nvec * 16u + tid; i < n; i += LIT_THREADS) atomicAdd(&whist[warp][src[i]], 1u);
     __syncthreads();
     for (u32 sym = tid; sym < 256u; sym += LIT_THREADS) {
         u32 s = 0;
@@ -82,56 +80,91 @@ __device__ void zb_hist_stats(const u32* count, u32* red, u32* largestOut, u32* 
     __syncthreads();
 }
 
-
-/* Visit the symbols of lit[beg, end) from the LAST to the first (the order the Huffman stream is
- * written in, huf_compress.c:1056-1118) with 16-byte aligned vector loads: a thread's run is
- * contiguous, so byte loads would cost one request per symbol. */
-struct ZbNoop { __device__ __forceinline__ void operator()() const {} };
-template <typename F, typename G = ZbNoop>
-__device__ __forceinline__ void zb_for_each_symbol_rev(const u8* __restrict__ lit, u32 beg, u32 end, F f, G every2 = G())
+/* One Huffman stream, lit[beg, end) (lit 16-byte aligned, beg < end), by one warp: the symbols from the LAST to the first
+ * (huf_compress.c:1056-1118), then the end mark (:973-982).  The stream's first bit is bit `bitPos` of `ow`.
+ * Tiles of 32 lanes x 16 bytes, lane 0 on the highest vector, so that bit offsets grow with the lane; bytes of a vector
+ * outside the stream are zero-length codes.  A warp scan over the lanes' bit counts places every lane's codes.  A lane ORs
+ * them into the warp's window `win` (LIT_WIN words, zero on entry, word k of `ow` at win[k % LIT_WIN]): its first and its
+ * last word may hold a neighbour's bits (shared atomicOr), the words between are its own (plain stores).  The warp then
+ * stores the tile's completed words coalesced.  Only the stream's first and last word can share bytes with the headers or
+ * a neighbouring stream: those two are ORed into global words the caller zeroed. */
+__device__ __forceinline__ void zb_huf_stream(const u8* __restrict__ lit, u32 beg, u32 end, const u32* enc, u32* win, u32* ow,
+                                              u32 bitPos, u32 lane)
 {
-    /* every2() runs after at most two symbols (the packer's flush point) */
-    u32 const aBeg = (beg + 15u) & ~15u, aEnd = end & ~15u;
-    if (aBeg >= aEnd) { for (u32 i = end; i-- > beg; ) { f(lit[i]); every2(); } return; }
-    for (u32 i = end; i-- > aEnd; ) { f(lit[i]); every2(); }
-    const uint4* v4 = reinterpret_cast<const uint4*>(lit);
-    /* a thread's run is walked one 16-byte vector at a time, each needing the one before it consumed: the next LIT_AHEAD
-     * vectors are requested before the current one is used */
-    u32 k = aEnd / 16u;
-    u32 const kLo = aBeg / 16u;
-    uint4 nx[LIT_AHEAD];
-#pragma unroll
-    for (u32 a = 0; a < LIT_AHEAD; a++) nx[a] = (k >= kLo + a + 1u) ? __ldg(v4 + (k - a - 1u)) : make_uint4(0, 0, 0, 0);
-    while (k > kLo) {
-        k--;
-        uint4 const q = nx[0];
-#pragma unroll
-        for (u32 a = 0; a + 1u < LIT_AHEAD; a++) nx[a] = nx[a + 1u];
-        if (k >= kLo + LIT_AHEAD) nx[LIT_AHEAD - 1u] = __ldg(v4 + (k - LIT_AHEAD));
+    const uint4* const v4 = reinterpret_cast<const uint4*>(lit);
+    uint4 const zero = make_uint4(0, 0, 0, 0);
+    u32 const vHi = (end - 1u) >> 4, nVec = vHi - (beg >> 4) + 1u;
+    u32 const firstW = bitPos >> 5;
+    /* two more tiles' vectors in flight behind the one in use */
+    uint4 q1 = lane < nVec ? __ldg(v4 + vHi - lane) : zero;
+    uint4 q2 = lane + 32u < nVec ? __ldg(v4 + vHi - lane - 32u) : zero;
+    for (u32 t = 0; t < nVec; t += 32u) {
+        uint4 const q = q1;
+        q1 = q2;
+        q2 = t + 64u + lane < nVec ? __ldg(v4 + vHi - (t + 64u + lane)) : zero;
+        u32 kLo = 0, kHi = 0;                                            /* bytes [kLo, kHi) of the vector are the stream's */
+        if (t + lane < nVec) { u32 const p0 = (vHi - t - lane) << 4; kLo = beg > p0 ? beg - p0 : 0u; kHi = min(end - p0, 16u); }
         u32 const w[4] = { q.x, q.y, q.z, q.w };
+        u32 nb = 0;
 #pragma unroll
-        for (int t = 3; t >= 0; t--) { f((u8)(w[t] >> 24)); f((u8)(w[t] >> 16)); every2(); f((u8)(w[t] >> 8)); f((u8)w[t]); every2(); }
+        for (u32 k = 0; k < 16u; k++) {
+            u32 const e = enc[(w[k >> 2] >> (8u * (k & 3u))) & 0xFFu];
+            nb += (k >= kLo && k < kHi) ? e >> 16 : 0u;
+        }
+        u32 incl = nb;
+#pragma unroll
+        for (u32 o = 1; o < 32u; o <<= 1) { u32 const x = __shfl_up_sync(ZB_FULL, incl, o); if (lane >= o) incl += x; }
+        u32 const tileBits = __shfl_sync(ZB_FULL, incl, 31);
+        {   /* the codes, last byte first; a full word is looked for once per two codes (fewer than 32 bits stay behind,
+             * 32 + 2 * 12 < 64) and emitted without a branch: lanes fill their words at different moments */
+            u32 const p = bitPos + incl - nb;
+            u32 widx = p >> 5, nacc = p & 31u, first = 1;
+            u64 acc = 0;
+#pragma unroll
+            for (int k = 15; k >= 0; k--) {
+                u32 const e = ((u32)k >= kLo && (u32)k < kHi) ? enc[(w[k >> 2] >> (8u * (k & 3u))) & 0xFFu] : 0u;
+                acc |= (u64)(e & 0xFFFFu) << nacc;
+                nacc += e >> 16;
+                if (k & 1) continue;
+                bool const full = nacc >= 32u;
+                u32* const wp = win + widx % LIT_WIN;
+                if (full && first == 0u) *wp = (u32)acc;
+                if (full && first != 0u) atomicOr(wp, (u32)acc);
+                first = full ? 0u : first;
+                widx += full ? 1u : 0u;
+                acc = full ? (acc >> 32) : acc;
+                nacc -= full ? 32u : 0u;
+            }
+            if (nacc != 0u && (u32)acc != 0u) atomicOr(win + widx % LIT_WIN, (u32)acc);
+        }
+        __syncwarp();
+        u32 const wEnd = (bitPos + tileBits) >> 5;                       /* words below this one are complete */
+        for (u32 k = (bitPos >> 5) + lane; k < wEnd; k += 32u) {
+            u32 const v = win[k % LIT_WIN];
+            win[k % LIT_WIN] = 0u;
+            if (k == firstW) atomicOr(ow + k, v); else ow[k] = v;
+        }
+        __syncwarp();
+        bitPos += tileBits;
     }
-    for (u32 i = aBeg; i-- > beg; ) { f(lit[i]); every2(); }
+    if (lane == 0) atomicOr(ow + (bitPos >> 5), win[(bitPos >> 5) % LIT_WIN] | (1u << (bitPos & 31u)));  /* end mark: the last word */
 }
 
 __global__ void __launch_bounds__(LIT_THREADS, LIT_MIN_CTAS)
 zb_literals_kernel(const ZbBlock* __restrict__ blocks, ZbParams prm, ZbStrides sd, const ZbDictEntropy* __restrict__ de,
                    const u8* __restrict__ lits, u8* __restrict__ body, ZbBlockMeta* __restrict__ meta)
 {
-    /* the per-warp histograms are dead once count[] is merged, the Huffman workspace only lives after that: one area */
-    __shared__ __align__(16) u8 scratch[sizeof(ZbdHufWksp) > sizeof(u32) * LIT_WARPS * 256 ? sizeof(ZbdHufWksp) : sizeof(u32) * LIT_WARPS * 256];
-    u32 (* const whist)[256] = reinterpret_cast<u32 (*)[256]>(scratch);
-    ZbdHufWksp& wk = *reinterpret_cast<ZbdHufWksp*>(scratch);
+    /* the per-warp (per-stream) histograms live until the stream sizes are known, then hold the encoding windows */
+    __shared__ __align__(16) u32 whist[LIT_WARPS][256];
+    __shared__ ZbdHufWksp wk;
     __shared__ u32 count[256];
     __shared__ u32 enc[256];
     __shared__ __align__(16) u8 hdr[288];                         /* the FSE form of the tree description is written before it is known to be short */
     __shared__ u32 red[16];
-    __shared__ u32 chunkBits[LIT_THREADS];
     __shared__ u32 sh_largest, sh_maxSym, sh_mode, sh_hSize, sh_usePrev;
-    __shared__ u32 sh_streamSize[4];
+    __shared__ u32 sh_bits[LIT_WARPS];
 
-    u32 const tid = threadIdx.x;
+    u32 const tid = threadIdx.x, warp = tid >> 5, lane = tid & 31u;
     u32 const b = blockIdx.x;
     ZbBlockMeta const m = meta[b];
     if (m.forceRaw) return;
@@ -166,8 +199,9 @@ zb_literals_kernel(const ZbBlock* __restrict__ blocks, ZbParams prm, ZbStrides s
             if (l1 + l2 <= ((2u * 4096u) >> 7) + 4u) mode = MODE_RAW;
         }
     }
+    /* the stream histograms are taken in the treeless case too: they give the stream sizes */
+    if (mode == MODE_HUF) zb_hist256(lit, n, whist, count);
     if (mode == MODE_HUF && !usePrev) {
-        zb_hist256(lit, n, whist, count);
         zb_hist_stats(count, red, &sh_largest, &sh_maxSym);
         u32 const largest = sh_largest;
         if (largest == n) mode = MODE_RLE;
@@ -209,30 +243,24 @@ zb_literals_kernel(const ZbBlock* __restrict__ blocks, ZbParams prm, ZbStrides s
         __syncthreads();
     }
 
-    /* ---------------- stream geometry + bit counts ---------------- */
+    /* ---------------- stream sizes: each warp's histogram against the code lengths ---------------- */
     u32 const hType = usePrev ? 3u : 2u;              /* set_repeat (treeless) : set_compressed */
-    u32 const T = LIT_THREADS / nbStreams;           /* threads per stream */
-    u32 const s = tid / T, j = tid % T;
     u32 const seg = (n + 3u) / 4u;                   /* huf_compress.c:1172 */
-    u32 const sBeg = (nbStreams == 1u) ? 0u : s * seg;
-    u32 const sEnd = (nbStreams == 1u) ? n : ((s == 3u) ? n : (s + 1u) * seg);
-    u32 const sLen = sEnd - sBeg;
-    u32 const cs = (sLen + T - 1u) / T;
-    u32 const cBeg = sBeg + min(j * cs, sLen);
-    u32 const cEnd = sBeg + min((j + 1u) * cs, sLen);
-    u32 hSize = 0, total = 0, bitOff = 0;
+    u32 streamSize[4] = { 0u, 0u, 0u, 0u };
+    u32 hSize = 0, total = 0;
     if (mode == MODE_HUF) {
         hSize = sh_hSize;
         u32 bits = 0;
-        zb_for_each_symbol_rev(lit, cBeg, cEnd, [&](u8 sym) { bits += enc[sym] >> 16; });
-        chunkBits[tid] = bits;
+        for (u32 sym = lane; sym < 256u; sym += 32u) bits += whist[warp][sym] * (enc[sym] >> 16);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) bits += __shfl_xor_sync(ZB_FULL, bits, o);
+        if (lane == 0) sh_bits[warp] = bits;
         __syncthreads();
-        /* suffix sum inside the stream: symbols AFTER mine are written before mine */
-        for (u32 k = j + 1u; k < T; k++) bitOff += chunkBits[s * T + k];
-        if (j == 0) sh_streamSize[s] = (bitOff + bits + 1u + 7u) >> 3;     /* + end mark, huf_compress.c:973-982 */
-        __syncthreads();
+        if (nbStreams == 4u) for (u32 k = 0; k < 4u; k++) streamSize[k] = (sh_bits[k] + 1u + 7u) >> 3;   /* + end mark, huf_compress.c:973-982 */
+        else streamSize[0] = (sh_bits[0] + sh_bits[1] + sh_bits[2] + sh_bits[3] + 1u + 7u) >> 3;
         u32 cSize = 0; bool tooBig = false;
-        for (u32 k = 0; k < nbStreams; k++) { cSize += sh_streamSize[k]; tooBig |= (sh_streamSize[k] > 65535u); }
+#pragma unroll
+        for (u32 k = 0; k < 4u; k++) { cSize += streamSize[k]; tooBig |= (streamSize[k] > 65535u); }
         if (nbStreams == 4u) cSize += 6u;
         total = hSize + cSize;
         if (nbStreams == 4u && tooBig) mode = MODE_RAW;                       /* huf_compress.c:1185 */
@@ -269,11 +297,14 @@ zb_literals_kernel(const ZbBlock* __restrict__ blocks, ZbParams prm, ZbStrides s
         return;
     }
 
-    /* compressed: zero the words we are going to OR into, then headers, then the packed streams */
-    {   u32 const endByte = lhSize + total;
-        uint4* o4 = reinterpret_cast<uint4*>(out);
-        for (u32 i = tid; i < (endByte + 15u) / 16u; i += LIT_THREADS) o4[i] = make_uint4(0, 0, 0, 0);
-    }
+    /* compressed.  Stream k occupies bytes [sOff, sOff + streamSize[k]); its first and last word are zeroed here, the
+     * headers are written behind a barrier (their bytes may share the first stream's first word), then the streams. */
+    u32 sOff = lhSize + hSize + (nbStreams == 4u ? 6u : 0u), sSize = 0;
+#pragma unroll
+    for (u32 k = 0; k < 4u; k++) { sOff += k < warp ? streamSize[k] : 0u; sSize = k == warp ? streamSize[k] : sSize; }
+    u32* const ow = reinterpret_cast<u32*>(out);
+    for (u32 i = tid; i < LIT_WARPS * 256u; i += LIT_THREADS) (&whist[0][0])[i] = 0u;         /* the windows */
+    if (warp < nbStreams && lane == 0) { ow[sOff >> 2] = 0u; ow[(sOff + sSize - 1u) >> 2] = 0u; }
     __syncthreads();
     if (tid == 0) {                                                           /* zstd_compress_literals.c:209-232 */
         u32 const cLitSize = total;
@@ -286,23 +317,15 @@ zb_literals_kernel(const ZbBlock* __restrict__ blocks, ZbParams prm, ZbStrides s
                            out[4] = (u8)(cLitSize >> 10); }
         if (nbStreams == 4u) {
             u8* jt = out + lhSize + hSize;
-            for (int k = 0; k < 3; k++) { jt[2 * k] = (u8)sh_streamSize[k]; jt[2 * k + 1] = (u8)(sh_streamSize[k] >> 8); }
+            for (int k = 0; k < 3; k++) { jt[2 * k] = (u8)streamSize[k]; jt[2 * k + 1] = (u8)(streamSize[k] >> 8); }
         }
         meta[b].litSecSize = lhSize + total;
     }
     for (u32 i = tid; i < hSize; i += LIT_THREADS) out[lhSize + i] = hdr[i];
     __syncthreads();          /* byte stores above share words with the streams' first bits: order them before the ORs */
-    {
-        u32 sOff = lhSize + hSize + (nbStreams == 4u ? 6u : 0u);
-        for (u32 k = 0; k < s; k++) sOff += sh_streamSize[k];
-        ZbdParW pw; zbd_pw_init(&pw, reinterpret_cast<u32*>(out), (u64)sOff * 8u + bitOff);
-#if LIT_PACK2
-        zb_for_each_symbol_rev(lit, cBeg, cEnd, [&](u8 sym) { u32 const e = enc[sym]; zbd_pw_put(&pw, e & 0xFFFFu, e >> 16); }, [&]() { zbd_pw_flush(&pw); });
-#else
-        zb_for_each_symbol_rev(lit, cBeg, cEnd, [&](u8 sym) { u32 const e = enc[sym]; zbd_pw_add(&pw, e & 0xFFFFu, e >> 16); });
-#endif
-        if (j == 0) zbd_pw_add(&pw, 1u, 1u);
-        zbd_pw_finish(&pw);
+    if (warp < nbStreams) {
+        u32 const beg = nbStreams == 1u ? 0u : min(warp * seg, n), end = nbStreams == 1u ? n : min((warp + 1u) * seg, n);
+        zb_huf_stream(lit, beg, end, enc, whist[warp], ow, sOff * 8u, lane);
     }
 }
 
