@@ -74,7 +74,8 @@ typedef enum {
     ZSTD_c_minMatch = 105, ZSTD_c_targetLength = 106, ZSTD_c_strategy = 107,
     ZSTD_c_enableLongDistanceMatching = 160,
     ZSTD_c_contentSizeFlag = 200, ZSTD_c_checksumFlag = 201, ZSTD_c_dictIDFlag = 202,
-    ZSTD_c_nbWorkers = 400, ZSTD_c_jobSize = 401, ZSTD_c_overlapLog = 402
+    ZSTD_c_nbWorkers = 400, ZSTD_c_jobSize = 401, ZSTD_c_overlapLog = 402,
+    ZSTD_c_blockDelimiters = 1008, ZSTD_c_validateSequences = 1009     /* lib/zstd.h:2123-2149, see ZSTD_compressSequences */
 } ZSTD_cParameter;
 typedef enum { ZSTD_reset_session_only = 1, ZSTD_reset_parameters = 2, ZSTD_reset_session_and_parameters = 3 } ZSTD_ResetDirective;
 ZSTDB200_API size_t ZSTD_CCtx_setParameter(ZSTD_CCtx* cctx, ZSTD_cParameter param, int value);
@@ -105,6 +106,36 @@ ZSTDB200_API size_t ZSTD_flushStream(ZSTD_CStream* zcs, ZSTD_outBuffer* output);
 ZSTDB200_API size_t ZSTD_endStream(ZSTD_CStream* zcs, ZSTD_outBuffer* output);
 ZSTDB200_API size_t ZSTD_CStreamInSize(void);
 ZSTDB200_API size_t ZSTD_CStreamOutSize(void);
+
+/* lib/zstd.h:1291-1322, 1555-1644 — compression of sequences the caller found (an external or GPU match finder, a format
+ * transcoder): zstd does the entropy stage and the framing only.  `rep` is ignored, as in the reference.
+ * ZSTD_c_blockDelimiters (0 or 1, sticky, reset by ZSTD_reset_parameters):
+ *   ZSTD_sf_explicitBlockDelimiters: a sequence with offset == 0 && matchLength == 0 ends a block, its litLength being the
+ *     block's trailing literals.  A block larger than min(128 KiB, window), sequences that run past srcSize or that stop
+ *     before srcSize is covered (no final delimiter) are invalid; an empty block produces no block, delimiters behind
+ *     the last byte are ignored.
+ *   ZSTD_sf_noBlockDelimiters: blocks of min(128 KiB, window) bytes, as ZSTD_compress2 cuts a frame; bytes beyond the sum of
+ *     the sequences are literals.  A sequence that crosses a block edge is split there: its literals go to the block they
+ *     fall in; a part of its match that is at least 3 bytes long stays a match (the part behind the edge with
+ *     litLength 0 and the same offset), a shorter part becomes literals.  The reference's splitter may cut other
+ *     blocks; both give valid frames.
+ * A sequence is invalid when offset == 0 (and it is not a delimiter), matchLength < 3, or offset > (pos > window ? window :
+ * pos + dictionary content size) with pos its end (zstd_compress.c:6531), or offset > 2^24 - 4.  Matches of 3 bytes are
+ * accepted whatever ZSTD_c_minMatch says (the reference rejects them unless minMatch is 3; minMatch is default-only here).
+ * Invalid sequences return ZSTD_error_externalSequences_invalid (107).  Validation always runs (on the GPU: it costs a few
+ * compares in a pass that reads every sequence, and the kernels rely on the lengths it checks), so ZSTD_c_validateSequences
+ * (0 or 1) is accepted and has no effect.
+ * Repcodes: the history is {1,4,8} (or the dictionary's) at the frame's first block and unknown at every other block; inside
+ * a block it runs as the reference runs it.  Feeding back the sequences of one of this library's frames, with its level,
+ * dictionary and block boundaries, gives that frame again byte for byte.
+ * Level, checksum flag, dictID flag and the dictionary (ZSTD_CCtx_loadDictionary / ZSTD_CCtx_refCDict) apply as for
+ * ZSTD_compress2, window and strategy come from the level and srcSize.  The call writes one frame. */
+typedef struct { unsigned int offset, litLength, matchLength, rep; } ZSTD_Sequence;
+typedef enum { ZSTD_sf_noBlockDelimiters = 0, ZSTD_sf_explicitBlockDelimiters = 1 } ZSTD_sequenceFormat_e;
+ZSTDB200_API size_t ZSTD_sequenceBound(size_t srcSize);                                       /* zstd_compress.c:3456 */
+ZSTDB200_API size_t ZSTD_mergeBlockDelimiters(ZSTD_Sequence* sequences, size_t seqsSize);   /* zstd_compress.c:3497, host code */
+ZSTDB200_API size_t ZSTD_compressSequences(ZSTD_CCtx* cctx, void* dst, size_t dstSize, const ZSTD_Sequence* inSeqs, size_t inSeqsSize,
+                                           const void* src, size_t srcSize);
 
 /* lib/zstd.h:236,242-246,114-120 ; lib/zstd_errors.h:106 */
 ZSTDB200_API size_t      ZSTD_compressBound(size_t srcSize);
@@ -175,6 +206,14 @@ ZSTDB200_API void ZSTDB200_getLastDStats(const ZSTD_DCtx* dctx, ZSTDB200_dstats*
  * several waves on several streams.  d_src needs no padding: no byte outside [d_src, d_src + srcSize) is read. */
 ZSTDB200_API size_t ZSTDB200_compressDevice(ZSTD_CCtx* cctx, void* d_dst, size_t dstCapacity,
                                             const void* d_src, size_t srcSize, int compressionLevel, void* stream);
+
+/* ZSTD_compressSequences with sequences, input and output in device memory (a match finder on the GPU hands its sequences
+ * over without a round trip through the host).  d_seqs: nbSeqs ZSTD_Sequence.  `stream`: as for ZSTDB200_compressDevice.
+ * Inputs of more than 1024 blocks run in waves of blocks on the one stream.  ZSTDB200_getLastStats: match_ms is the time of
+ * the sequence import (partition, validation, conversion). */
+ZSTDB200_API size_t ZSTDB200_compressSequencesDevice(ZSTD_CCtx* cctx, void* d_dst, size_t dstCapacity,
+                                                     const ZSTD_Sequence* d_seqs, size_t nbSeqs,
+                                                     const void* d_src, size_t srcSize, void* stream);
 
 /* One frame compressed by several GPUs (the reference's counterpart: the jobs of ZSTDMT, zstdmt_compress.c:1168-1227 —
  * every job reads an overlap of the input in front of it, only the first writes the frame header, only the last the end

@@ -109,6 +109,14 @@ def lib() -> ctypes.CDLL:
     L.ZSTD_compress2.argtypes = [_vp, _vp, _sz, _vp, _sz]
     L.ZSTD_compressStream2.restype = _sz
     L.ZSTD_compressStream2.argtypes = [_vp, _vp, _vp, ctypes.c_int]
+    L.ZSTD_compressSequences.restype = _sz
+    L.ZSTD_compressSequences.argtypes = [_vp, _vp, _sz, _vp, _sz, _vp, _sz]
+    L.ZSTDB200_compressSequencesDevice.restype = _sz
+    L.ZSTDB200_compressSequencesDevice.argtypes = [_vp, _vp, _sz, _vp, _sz, _vp, _sz, _vp]
+    L.ZSTD_sequenceBound.restype = _sz
+    L.ZSTD_sequenceBound.argtypes = [_sz]
+    L.ZSTD_mergeBlockDelimiters.restype = _sz
+    L.ZSTD_mergeBlockDelimiters.argtypes = [_vp, _sz]
     L.ZSTDB200_compressFrames_usingCDict.restype = _sz
     L.ZSTDB200_compressFrames_usingCDict.argtypes = [_vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, ctypes.c_int, _vp]
     if hasattr(L, "ZSTD_createDCtx"):
@@ -289,10 +297,48 @@ class ZSTD_CCtx:
                                                            1 if device_memory else 0, stream))
         return r, list(csz)
 
+    # -- sequence API (lib/zstd.h:1555-1644) --
+    def compress_sequences(self, seqs, src, dst_capacity: Optional[int] = None) -> bytes:
+        """ZSTD_compressSequences: one frame from the caller's sequences (host buffers).  seqs: an (n, 4) uint32 array of
+        (offset, litLength, matchLength, rep) or a list of (offset, litLength, matchLength) tuples.  The block format is
+        the sticky ZSTD_c_blockDelimiters (set_parameter(1008, 0 or 1)); level, checksum and dictionary apply as for
+        compress2."""
+        arr = _sequences(seqs)
+        p, n, keep = _buf(src)
+        cap = ZSTD_compressBound(n) + 8 if dst_capacity is None else dst_capacity
+        dst = ctypes.create_string_buffer(max(cap, 1))
+        r = _check(lib().ZSTD_compressSequences(self._h, dst, cap, arr.ctypes.data if len(arr) else None, len(arr), p, n))
+        return dst.raw[:r]
+
+    def compress_sequences_device(self, d_dst: int, dst_capacity: int, d_seqs: int, nb_seqs: int, d_src: int, src_size: int,
+                                  stream: int = 0) -> int:
+        """ZSTDB200_compressSequencesDevice: sequences (nb_seqs x 16 bytes), input and output in device memory (ints, e.g.
+        torch.Tensor.data_ptr()).  Returns the compressed size."""
+        return _check(lib().ZSTDB200_compressSequencesDevice(self._h, d_dst, dst_capacity, d_seqs, nb_seqs, d_src, src_size, stream))
+
     def stats(self) -> Stats:
         s = Stats()
         lib().ZSTDB200_getLastStats(self._h, ctypes.byref(s))
         return s
+
+
+def _sequences(seqs):
+    """an (n, 4) uint32 array (offset, litLength, matchLength, rep) from such an array or from (offset, litLength,
+    matchLength) tuples"""
+    import numpy as np
+    a = np.asarray(seqs, dtype=np.uint32)
+    if a.size == 0:
+        return np.zeros((0, 4), dtype=np.uint32)
+    if a.ndim != 2 or a.shape[1] not in (3, 4):
+        raise ValueError("sequences: an (n, 4) array or (offset, litLength, matchLength) tuples")
+    if a.shape[1] == 3:
+        a = np.concatenate([a, np.zeros((len(a), 1), dtype=np.uint32)], axis=1)
+    return np.ascontiguousarray(a)
+
+
+def sequence_bound(src_size: int) -> int:
+    """ZSTD_sequenceBound: the most sequences (delimiters included) a frame of src_size bytes can need."""
+    return int(lib().ZSTD_sequenceBound(src_size))
 
 
 class ZSTD_DCtx:

@@ -162,6 +162,10 @@ struct ZSTD_CCtx_s {
     u8* stIn; size_t stInSize, stInCap;
     u8* stOut; size_t stOutSize, stOutPos, stOutCap;
     int stFrames;                  /* frames produced in the current session */
+    /* sequence calls (ZSTD_compressSequences): sticky ZSTD_c_blockDelimiters, staging of host sequences, import scratch */
+    int advDelims;
+    u8* d_seqIn; size_t d_seqInCap;
+    void* d_seqTile; size_t d_seqTileCap; void* d_seqBlk; size_t d_seqBlkCap; u64* d_seqCtrl;
 };
 
 static double zb_now(void) { struct timespec ts; clock_gettime(CLOCK_MONOTONIC, &ts); return (double)ts.tv_sec + 1e-9 * (double)ts.tv_nsec; }
@@ -276,6 +280,7 @@ extern "C" size_t ZSTD_freeCCtx(ZSTD_CCtx* c)
         zb_freeWorkspace(c);
         zb_freeWaveEvents(c);
         cudaFree(c->d_in); cudaFree(c->d_out);
+        cudaFree(c->d_seqIn); cudaFree(c->d_seqTile); cudaFree(c->d_seqBlk); cudaFree(c->d_seqCtrl);
         for (u32 s = 0; s <= ZB_WAVE_SLOTS_MAX; s++) if (c->waveStream[s]) cudaStreamDestroy(c->waveStream[s]);
         cudaEventDestroy(c->evStart); cudaEventDestroy(c->evK0); cudaEventDestroy(c->evK1);
         cudaEventDestroy(c->evK2); cudaEventDestroy(c->evK3); cudaEventDestroy(c->evMid);
@@ -316,13 +321,14 @@ static size_t zb_ensureDesc(ZSTD_CCtx* c, size_t nbBlocks, size_t nbFrames, size
     return 0;
 }
 /* workspace for nbSlotBlocks blocks laid out with the strides `sd` (capacities are kept in bytes) */
-static size_t zb_ensureHeavy(ZSTD_CCtx* c, size_t nbSlotBlocks, const ZbStrides& sd, bool needDist2)
+/* (sequence calls, needMatch = false: no candidate or segment arrays beyond the dist area that K3 uses) */
+static size_t zb_ensureHeavy(ZSTD_CCtx* c, size_t nbSlotBlocks, const ZbStrides& sd, bool needDist2, bool needMatch = true)
 {
     size_t const nb = nbSlotBlocks;
     size_t const need[9] = { nb * sizeof(ZbBlockMeta), nb * sd.seq * sizeof(u64), nb * (size_t)sd.lit, nb * (size_t)sd.body,
                              nb * (size_t)sd.dist * sizeof(u16), needDist2 ? nb * (size_t)sd.dist * sizeof(u16) : 0,
-                             nb * ((sd.dist + ZB_PARSE_SEG - 1u) / ZB_PARSE_SEG) * sizeof(ZbSegMeta),
-                             nb * (size_t)sd.dist * sizeof(u32), needDist2 ? nb * (size_t)sd.dist * sizeof(u32) : 0 };
+                             needMatch ? nb * ((sd.dist + ZB_PARSE_SEG - 1u) / ZB_PARSE_SEG) * sizeof(ZbSegMeta) : 0,
+                             needMatch ? nb * (size_t)sd.dist * sizeof(u32) : 0, needDist2 ? nb * (size_t)sd.dist * sizeof(u32) : 0 };
     void** const ptr[9] = { (void**)&c->d_meta, (void**)&c->d_seqs, (void**)&c->d_lits, (void**)&c->d_body, (void**)&c->d_dist, (void**)&c->d_dist2,
                             (void**)&c->d_segmeta, (void**)&c->d_far, (void**)&c->d_far2 };
     for (int i = 0; i < 9; i++) {
@@ -1014,6 +1020,9 @@ extern "C" size_t ZSTD_CCtx_setParameter(ZSTD_CCtx* c, ZSTD_cParameter paramE, i
     case 201: c->advChecksum = value != 0; return 0;                                         /* ZSTD_c_checksumFlag */
     case 202: c->advNoDictID = value == 0; return 0;                                         /* ZSTD_c_dictIDFlag */
     case 400: case 401: case 402: return 0;                                                  /* nbWorkers, jobSize, overlapLog */
+    case 1008: if (value != 0 && value != 1) return ZB_ERR(ZB_error_parameter_unsupported);  /* ZSTD_c_blockDelimiters */
+        c->advDelims = value; return 0;
+    case 1009: return (value == 0 || value == 1) ? 0 : ZB_ERR(ZB_error_parameter_unsupported);   /* ZSTD_c_validateSequences: validation always runs */
     case 101: case 102: case 103: case 104: case 105: case 106: case 107:                    /* windowLog .. strategy: default only */
     case 160: case 161: case 162: case 163: case 164:                                        /* long distance matching: off only */
         return value == 0 ? 0 : ZB_ERR(ZB_error_parameter_unsupported);
@@ -1028,7 +1037,7 @@ extern "C" size_t ZSTD_CCtx_reset(ZSTD_CCtx* c, ZSTD_ResetDirective reset)      
     if (!c) return ZB_ERR(ZB_error_GENERIC);
     if (reset == 1 || reset == 3) { c->stInSize = 0; c->stOutSize = 0; c->stOutPos = 0; c->stFrames = 0; }   /* an unfinished stream is dropped */
     if (reset == 2 || reset == 3) {
-        c->advLevel = 3; c->advChecksum = 0; c->advNoDictID = 0;
+        c->advLevel = 3; c->advChecksum = 0; c->advNoDictID = 0; c->advDelims = 0;
         ZSTD_freeCDict(c->advLocalDict); c->advLocalDict = NULL; c->advRefCDict = NULL;
     }
     return 0;
@@ -1057,6 +1066,179 @@ extern "C" size_t ZSTD_compress2(ZSTD_CCtx* c, void* dst, size_t dstCapacity, co
     const ZSTD_CDict* const cd = c->advRefCDict ? c->advRefCDict : c->advLocalDict;
     int const level = c->advRefCDict ? c->advRefCDict->level : c->advLevel;                  /* a referenced CDict brings its own level (:5836) */
     return zb_compressOne(c, dst, dstCapacity, src, srcSize, cd, level, c->advChecksum != 0, c->advNoDictID != 0);
+}
+
+/* ------------------------------------------------------------------ sequence calls (lib/zstd.h:1555-1644)
+ * K1s (zb_seqimport.cu) takes the place of K1: the sequences are partitioned and validated on the device, every block's
+ * share is clipped to it and coded; K2 / K3 / K4 run unchanged.  One stream; more than devWaveBlocks blocks run in waves
+ * over the block table, in order, through one workspace slot. */
+extern "C" size_t ZSTD_sequenceBound(size_t srcSize)                                    /* zstd_compress.c:3456-3460 */
+{
+    return (srcSize / 3) + 1 + (srcSize / 1024) + 1;                                     /* ZSTD_MINMATCH_MIN, ZSTD_BLOCKSIZE_MAX_MIN */
+}
+
+extern "C" size_t ZSTD_mergeBlockDelimiters(ZSTD_Sequence* seqs, size_t n)               /* zstd_compress.c:3497-3511 */
+{
+    size_t out = 0;
+    for (size_t in = 0; in < n; in++) {
+        if (seqs[in].offset == 0 && seqs[in].matchLength == 0) { if (in != n - 1) seqs[in + 1].litLength += seqs[in].litLength; }
+        else seqs[out++] = seqs[in];
+    }
+    return out;
+}
+
+template <typename T> static size_t zb_grow(T** p, size_t* cap, size_t bytes)
+{
+    if (bytes <= *cap) return 0;
+    cudaFree(*p); *p = NULL; *cap = 0;
+    CK(cudaMalloc((void**)p, bytes));
+    *cap = bytes;
+    return 0;
+}
+#define TRY(x) do { size_t const e_ = (x); if (zb_isErr(e_)) return e_; } while (0)
+
+static size_t zb_compressSeqs(ZSTD_CCtx* c, void* dst, size_t dstCapacity, const ZSTD_Sequence* seqs, size_t n,
+                              const void* src, size_t srcSize, bool deviceMemory, cudaStream_t userStream)
+{
+    if (!c) return ZB_ERR(ZB_error_GENERIC);
+    if (dstCapacity && !dst) return ZB_ERR(ZB_error_dstBuffer_null);
+    if (n && !seqs) return ZB_ERR(ZB_error_externalSequences_invalid);
+    if (n > 0xFFFFFFF0u) return ZB_ERR(ZB_error_srcSize_wrong);
+    ZbDeviceGuard guard;
+    TRY(zb_ctxInit(c));
+    memset(&c->stats, 0, sizeof(c->stats));
+    const ZSTD_CDict* const cdArg = c->advRefCDict ? c->advRefCDict : c->advLocalDict;
+    int const level = c->advRefCDict ? c->advRefCDict->level : c->advLevel;
+    ZSTD_CDict* const cd = (cdArg && cdArg->size >= 8) ? const_cast<ZSTD_CDict*>(cdArg) : NULL;
+    if (g_strictLevels && level > 4) return ZB_ERR(ZB_error_parameter_unsupported);
+    bool const expl = c->advDelims != 0;
+    cudaStream_t const st = (deviceMemory && userStream) ? userStream : c->stream;
+    if (cd) TRY(zb_residentDict(cd, c->device, true, st));
+    const ZbDictEntropy* const de = (cd && cd->entropy.present) ? &cd->entropy : NULL;
+    ZbCParams const cp = zb_getCParams(level, srcSize, cd ? cd->size : 0);
+    ZbParams prm = zb_makeParams(cp);
+    if (de) { prm.codeRep[0] = de->rep[0]; prm.codeRep[1] = de->rep[1]; prm.codeRep[2] = de->rep[2]; }
+    u32 const blockMax = (1u << cp.windowLog) < ZB_BLOCK_MAX ? (1u << cp.windowLog) : ZB_BLOCK_MAX;      /* zstd_compress.c:2124 */
+    u32 const dictFlag = (cd && cd->tail) ? ZB_FLAG_DICT : 0u;
+    /* inputs on the device: the sequences need 16-byte alignment for the tile loads */
+    const u8* d_src = (const u8*)src; const void* d_seqs = seqs;
+    size_t const seqBytes = n * sizeof(ZSTD_Sequence);
+    if (!deviceMemory) {
+        TRY(zb_grow(&c->d_in, &c->d_inCap, srcSize + 16));
+        if (srcSize) CK(cudaMemcpyAsync(c->d_in, src, srcSize, cudaMemcpyHostToDevice, st));
+        d_src = c->d_in;
+    }
+    if (n && (!deviceMemory || ((uintptr_t)seqs & 15u))) {
+        TRY(zb_grow(&c->d_seqIn, &c->d_seqInCap, seqBytes));
+        CK(cudaMemcpyAsync(c->d_seqIn, seqs, seqBytes, deviceMemory ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
+        d_seqs = c->d_seqIn;
+    }
+    if (!c->d_seqCtrl) CK(cudaMalloc(&c->d_seqCtrl, 4 * sizeof(u64)));
+    u64 ctrl[4] = { 0, 0, ~0ull, 0 };
+    CK(cudaMemcpyAsync(c->d_seqCtrl, ctrl, sizeof(ctrl), cudaMemcpyHostToDevice, st));
+    CK(cudaStreamSynchronize(st));                                 /* the pageable sources above are staged */
+    CK(cudaEventRecord(c->evK0, st));
+    /* K1s-a */
+    u32 const nbTiles = (u32)((n + 1023) / 1024);
+    TRY(zb_grow(&c->d_seqTile, &c->d_seqTileCap, (size_t)nbTiles * 12 + 16));
+    u64* const d_tileLen = (u64*)c->d_seqTile; u32* const d_tileEnds = (u32*)(d_tileLen + nbTiles);
+    CK(zb_launch_seq_partition(d_seqs, (u32)n, expl, d_tileLen, d_tileEnds, c->d_seqCtrl, st));
+    u32 nbBlocks;
+    if (srcSize == 0) nbBlocks = 1;                                /* the frame's one empty block */
+    else if (!expl) nbBlocks = (u32)((srcSize + blockMax - 1) / blockMax);
+    else {
+        CK(cudaMemcpyAsync(ctrl, c->d_seqCtrl, 2 * sizeof(u64), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        if (ctrl[0] > srcSize || ctrl[1] == 0) return ZB_ERR(ZB_error_externalSequences_invalid);
+        nbBlocks = (u32)ctrl[1];
+    }
+    TRY(zb_ensureDesc(c, nbBlocks, 1, 1, 0));
+    size_t const blkBytes = (size_t)nbBlocks * 24 + 16;              /* blockFirstPos / blockEnd (u64), blockFirst / blockSeq (u32) */
+    TRY(zb_grow(&c->d_seqBlk, &c->d_seqBlkCap, blkBytes));
+    u64* const d_firstPos = (u64*)c->d_seqBlk; u64* const d_blockEnd = d_firstPos + nbBlocks;
+    u32* const d_first = (u32*)(d_blockEnd + nbBlocks); u32* const d_blockSeq = d_first + nbBlocks;
+    if (!expl || srcSize == 0) {                                    /* the planner's geometry */
+        if (!c->plan) { c->plan = new (std::nothrow) ZbPlan(); if (!c->plan) return ZB_ERR(ZB_error_memory_allocation); }
+        ZbVec<ZbBlock>& B = c->plan->blocks;
+        B.clear(); B.reserve(nbBlocks);
+        for (u32 k = 0; k < nbBlocks; k++) {
+            ZbBlock b; memset(&b, 0, sizeof(b));
+            b.srcOff = (u64)k * blockMax; b.size = (u32)(srcSize - b.srcOff < blockMax ? srcSize - b.srcOff : blockMax);
+            b.flags = (k == 0 ? ZB_FLAG_FIRST | dictFlag : 0u) | (k + 1 == nbBlocks ? ZB_FLAG_LAST : 0u);
+            B.push_back(b);
+        }
+        CK(cudaMemcpyAsync(c->d_blocks, B.data(), nbBlocks * sizeof(ZbBlock), cudaMemcpyHostToDevice, st));
+        CK(cudaMemsetAsync(d_first, 0xFF, nbBlocks * sizeof(u32), st));
+    }
+    u64 const dictContent = cd ? cd->size - cd->contentOff : 0;
+    CK(zb_launch_seq_place(d_seqs, (u32)n, expl, d_tileLen, d_tileEnds, srcSize, 1ull << cp.windowLog, dictContent, blockMax,
+                           nbBlocks, d_blockEnd, d_blockSeq, d_first, d_firstPos, c->d_seqCtrl, st));
+    if (expl && srcSize) CK(zb_launch_seq_blocks(d_blockEnd, d_blockSeq, nbBlocks, blockMax, dictFlag, c->d_blocks, d_first, d_firstPos, c->d_seqCtrl, st));
+    CK(cudaMemcpyAsync(ctrl, c->d_seqCtrl, sizeof(ctrl), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (ctrl[2] != ~0ull || ctrl[0] > srcSize || (expl && srcSize && ctrl[3] != srcSize)) return ZB_ERR(ZB_error_externalSequences_invalid);
+    ZbFrame fr; memset(&fr, 0, sizeof(fr));
+    fr.srcSize = srcSize; fr.nbBlocks = nbBlocks; fr.windowLog = cp.windowLog;
+    fr.dictID = (c->advNoDictID || !de) ? 0u : de->dictID; fr.checksum = c->advChecksum != 0;
+    CK(cudaMemcpyAsync(c->d_frames, &fr, sizeof(fr), cudaMemcpyHostToDevice, st));
+    /* K1s-b, K2, K3, K4 in waves through one workspace slot */
+    ZbStrides const sd = zb_seq_strides(blockMax);
+    u32 const waveBlocks = (c->devWaveBlocks && nbBlocks > c->devWaveBlocks) ? c->devWaveBlocks : nbBlocks;
+    u32 const nbWaves = (nbBlocks + waveBlocks - 1) / waveBlocks;
+    TRY(zb_ensureDesc(c, nbBlocks, 1, nbWaves, 0));
+    TRY(zb_ensureHeavy(c, waveBlocks, sd, false, false));
+    u8* d_out = (u8*)dst; size_t outCap = dstCapacity;
+    if (!deviceMemory) {
+        size_t const bound = srcSize + 3 * (size_t)nbBlocks + 64;      /* every block at most raw: 3 header bytes each, blocks may be tiny */
+        outCap = dstCapacity < bound ? dstCapacity : bound;
+        TRY(zb_grow(&c->d_out, &c->d_outCap, outCap + 16));
+        d_out = c->d_out;
+    }
+    bool const timed = nbWaves == 1;
+    unsigned launches = 2 + (n ? 2u : 0u) + (expl && srcSize ? 1u : 0u);
+    for (u32 w = 0; w < nbWaves; w++) {
+        u32 const b0 = w * waveBlocks, nb = (b0 + waveBlocks <= nbBlocks) ? waveBlocks : nbBlocks - b0;
+        CK(zb_launch_seq_convert(d_src, c->d_blocks + b0, nb, d_first + b0, d_firstPos + b0, d_seqs, (u32)n, &prm, &sd, c->d_seqs, c->d_lits, c->d_meta, st));
+        if (w == 0) CK(cudaEventRecord(c->evK1, st));
+        CK(zb_launch_literals(c->d_blocks + b0, nb, &prm, &sd, de ? cd->d_de : NULL, c->d_lits, c->d_body, c->d_meta, st));
+        if (timed) CK(cudaEventRecord(c->evK2, st));
+        CK(zb_launch_sequences(d_src, c->d_blocks + b0, nb, &prm, &sd, de ? cd->d_de : NULL, c->d_seqs, c->d_dist, c->d_body, c->d_meta, st));
+        if (timed) CK(cudaEventRecord(c->evK3, st));
+        CK(zb_launch_stitch(d_src, c->d_blocks + b0, nb, c->d_frames, c->d_body, sd.body, c->d_meta, c->d_outOffsets + b0,
+                            w > 0 ? c->d_totals + (w - 1) : NULL, c->d_totals + w, d_out, outCap, st));
+        launches += 5;
+    }
+    if (c->advChecksum) { CK(zb_launch_checksums(d_src, c->d_frames, 1, c->d_outOffsets, d_out, outCap, st)); launches++; }
+    CK(cudaEventRecord(c->evKEnd, st));
+    u64 total = 0;
+    CK(cudaMemcpyAsync(&total, c->d_totals + nbWaves - 1, sizeof(u64), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (!deviceMemory && total <= dstCapacity) CK(cudaMemcpy(dst, d_out, total, cudaMemcpyDeviceToHost));
+    float ms = 0;
+    cudaEventElapsedTime(&ms, c->evK0, c->evKEnd); c->stats.kernel_ms = ms; c->stats.total_ms = ms;
+    cudaEventElapsedTime(&ms, c->evK0, c->evK1); c->stats.match_ms = ms;     /* the first wave's import */
+    if (timed) {
+        cudaEventElapsedTime(&ms, c->evK1, c->evK2); c->stats.literals_ms = ms;
+        cudaEventElapsedTime(&ms, c->evK2, c->evK3); c->stats.sequences_ms = ms;
+        cudaEventElapsedTime(&ms, c->evK3, c->evKEnd); c->stats.stitch_ms = ms;
+    }
+    c->stats.launches = launches; c->stats.nbBlocks = nbBlocks;
+    if (!deviceMemory) { c->stats.h2d_bytes = srcSize + seqBytes; c->stats.d2h_bytes = total <= dstCapacity ? (size_t)total : 0; }
+    if (total > dstCapacity) return ZB_ERR(ZB_error_dstSize_tooSmall);
+    return (size_t)total;
+}
+#undef TRY
+
+extern "C" size_t ZSTD_compressSequences(ZSTD_CCtx* c, void* dst, size_t dstCapacity, const ZSTD_Sequence* seqs, size_t n,
+                                         const void* src, size_t srcSize)                       /* zstd_compress.c:6858 */
+{
+    return zb_compressSeqs(c, dst, dstCapacity, seqs, n, src, srcSize, false, NULL);
+}
+
+extern "C" size_t ZSTDB200_compressSequencesDevice(ZSTD_CCtx* c, void* d_dst, size_t dstCapacity, const ZSTD_Sequence* d_seqs, size_t n,
+                                                   const void* d_src, size_t srcSize, void* stream)
+{
+    return zb_compressSeqs(c, d_dst, dstCapacity, d_seqs, n, d_src, srcSize, true, (cudaStream_t)stream);
 }
 
 /* Streaming (lib/zstd.h:681-862).  The unit of GPU work is a whole frame, so the stream front end collects input on the
@@ -1213,6 +1395,7 @@ extern "C" const char* ZSTD_getErrorName(size_t code)                           
     case 74: return "Operation on NULL destination buffer";
     case 80: return "Operation made no progress over multiple calls, due to output buffer being full";
     case 82: return "Operation made no progress over multiple calls, due to input being empty";
+    case 107: return "External sequences are not valid";
     default: return "Unspecified error code";
     }
 }

@@ -59,6 +59,7 @@ typedef uint64_t u64;
 #define ZB_error_dstSize_tooSmall 70
 #define ZB_error_srcSize_wrong 72
 #define ZB_error_dstBuffer_null 74
+#define ZB_error_externalSequences_invalid 107
 #define ZB_error_maxCode 120
 
 typedef struct {
@@ -169,6 +170,16 @@ static inline ZB_HD ZbStrides zb_strides(u32 maxBlock)
     ZbStrides sd; sd.dist = M; sd.seq = M / 4u + 8u; sd.lit = M + 256u; sd.body = M + 1024u; sd.state = M / 4u;
     return sd;
 }
+/* Sequence calls (ZSTD_compressSequences): matches of 3 bytes allow M / 3 sequences per block, so the seq slots hold
+ * M / 3 + 8 and the FSE state records (3 x state u16 inside the dist area) ceil(M / 3), rounded up to 16 bytes. */
+static inline ZB_HD ZbStrides zb_seq_strides(u32 maxBlock)
+{
+    ZbStrides sd = zb_strides(maxBlock);
+    u32 const M = sd.dist;
+    sd.seq = M / 3u + 8u; sd.state = ((M + 2u) / 3u + 7u) & ~7u; sd.dist = 3u * sd.state;
+    return sd;
+}
+#define ZB_SEQ_OFF_MAX ((1u << 24) - 4u)   /* largest offset of a sequence call: offBase = offset + 3 has 24 bits in a packed sequence */
 /* a final sequence as the sequences kernel reads it: offBase (24 bits), literal length (18 bits), match length (>= 4) */
 static inline ZB_HD u64 zb_pack_seq(u32 offBase, u32 litLen, u32 matchLen)
 {

@@ -23,6 +23,23 @@ cudaError_t zb_launch_match(const u8* d_src, const u8* d_dictEnd, const u32* d_i
                             u16* d_dist, u32* d_far, u16* d_dist2, u32* d_far2, u64* d_seqs, u8* d_lits, ZbBlockMeta* d_meta, ZbSegMeta* d_segmeta,
                             cudaEvent_t evMid, cudaStream_t stream);
 
+/* K1s: caller-supplied sequences (ZSTD_Sequence[n], 16-byte aligned, device memory) in place of K1 (zb_seqimport.cu).
+ * partition: per-tile sums (d_tileLen / d_tileEnds: one per 1024 sequences), scanned; d_ctrl[0] = sum of the lengths,
+ * d_ctrl[1] = delimiters that close a non-empty block (expl != 0).  place: validation (d_ctrl[2] = first invalid index,
+ * to be preset to ~0) and the block starts: explicit delimiters -> d_blockEnd / d_blockSeq per closing delimiter, else
+ * d_blockFirst / d_blockFirstPos of the nbBlocks blocks of blockMax bytes (preset d_blockFirst to ~0).  blocks (explicit
+ * only): the ZbBlock table, d_blockFirst / d_blockFirstPos, d_ctrl[3] = end of the last block.  convert (K1s-b): the
+ * blocks' triples, literals and meta into the workspace rows [0, nbBlocks) with strides sd (zb_seq_strides). */
+cudaError_t zb_launch_seq_partition(const void* d_seqs, u32 n, int expl, u64* d_tileLen, u32* d_tileEnds, u64* d_ctrl, cudaStream_t stream);
+cudaError_t zb_launch_seq_place(const void* d_seqs, u32 n, int expl, const u64* d_tileLen, const u32* d_tileEnds,
+                                u64 srcSize, u64 window, u64 dictContent, u32 blockMax, u32 nbBlocks,
+                                u64* d_blockEnd, u32* d_blockSeq, u32* d_blockFirst, u64* d_blockFirstPos, u64* d_ctrl, cudaStream_t stream);
+cudaError_t zb_launch_seq_blocks(const u64* d_blockEnd, const u32* d_blockSeq, u32 nbBlocks, u32 blockMax, u32 dictFlag,
+                                 ZbBlock* d_blocks, u32* d_blockFirst, u64* d_blockFirstPos, u64* d_ctrl, cudaStream_t stream);
+cudaError_t zb_launch_seq_convert(const u8* d_src, const ZbBlock* d_blocks, u32 nbBlocks, const u32* d_blockFirst, const u64* d_blockFirstPos,
+                                  const void* d_seqs, u32 n, const ZbParams* prm, const ZbStrides* sd,
+                                  u64* d_seqOut, u8* d_lits, ZbBlockMeta* d_meta, cudaStream_t stream);
+
 /* host: the format's predefined FSE tables (zb_dict.cu), and their upload to the current device (zb_sequences.cu) */
 void zb_buildDefaultTables(ZbdFseCTable* out3);
 cudaError_t zb_upload_default_tables(const ZbdFseCTable* host3, cudaStream_t stream);
