@@ -18,6 +18,10 @@ struct BlockOut { std::vector<u8> lits; std::vector<u64> seqs; u32 sumLL, sumML;
 /* dependency statistics of the last call (development: how parallel is the match stage of a frame?) */
 extern "C" { unsigned long long zbh_nbMatches, zbh_maxDepth, zbh_nearDeps, zbh_anyDeps, zbh_tileDepth; }
 static std::vector<unsigned> g_tDepth;
+/* which check refused the last call, where the reference decoder's one-shot call may accept: 1 = the end of a Huffman
+ * stream of the literals (the reference accepts some streams that read past their start), 2 = a compressed block that
+ * regenerates more than Block_Maximum_Size (the reference's one-shot call accepts up to ~32 bytes more) */
+extern "C" { unsigned zbh_refusedBy; }
 
 static std::vector<unsigned long long> g_mStart, g_mEnd; static std::vector<unsigned> g_mDepth;
 static const u8* g_dict = NULL;            /* the call's dictionary (single-threaded test code) */
@@ -51,11 +55,14 @@ static u32 decodeLiterals(BlockOut& o, const u8* in, const std::vector<ZbdBlock>
     if (desc > b.litComp) return ZBD_CORRUPT;
     const u8* s = c + b.litHdr + desc;
     u32 const total = b.litComp - desc;
-    if (b.litStreams == 1) return zbd_hufDecodeStream(o.lits.data(), b.litRegen, s, total, table.data(), log);
+    if (b.litStreams == 1) {
+        if (zbd_hufDecodeStream(o.lits.data(), b.litRegen, s, total, table.data(), log)) { zbh_refusedBy = 1; return ZBD_CORRUPT; }
+        return ZBD_OK;
+    }
     u32 off[4], size[4], count[4];
     if (zbd_litStreams(off, size, count, s, total, b.litRegen)) return ZBD_CORRUPT;
     for (u32 k = 0; k < 4; k++)
-        if (zbd_hufDecodeStream(o.lits.data() + k * count[0], count[k], s + off[k], size[k], table.data(), log)) return ZBD_CORRUPT;
+        if (zbd_hufDecodeStream(o.lits.data() + k * count[0], count[k], s + off[k], size[k], table.data(), log)) { zbh_refusedBy = 1; return ZBD_CORRUPT; }
     return ZBD_OK;
 }
 
@@ -80,7 +87,7 @@ extern "C" size_t zbh_decompress_usingDict(void* dstv, size_t cap, const void* s
 {
     const u8* const in = (const u8*)srcv;
     u8* const dst = (u8*)dstv;
-    g_dict = (const u8*)dictv; memset(&g_di, 0, sizeof(g_di));
+    g_dict = (const u8*)dictv; memset(&g_di, 0, sizeof(g_di)); zbh_refusedBy = 0;
     if (g_dict && dictSize) { u32 const de = zbd_parseDict(&g_di, g_dict, dictSize); if (de) return ERR(de); }
     const u8* const content = g_dict ? g_dict + g_di.contentOff : NULL;
     size_t const contentSize = g_dict ? dictSize - g_di.contentOff : 0;
@@ -106,7 +113,7 @@ extern "C" size_t zbh_decompress_usingDict(void* dstv, size_t cap, const void* s
             {   u32 const se = decodeSeqs(o, in, B, bi); if (se) return ERR(se); }          /* 20, or 16 for an offset beyond 28 bits */
             if (o.sumLL > b.litRegen) return ERR(ZBD_CORRUPT);
             size_t const regen = (size_t)b.litRegen + o.sumML;
-            if (regen > ZB_BLOCK_MAX) return ERR(ZBD_CORRUPT);
+            if (regen > b.blockMax) { zbh_refusedBy = 2; return ERR(ZBD_CORRUPT); }
             if (out + regen > cap) return ERR(70);
             /* the history at the block's end, first as the transfer function says, then by executing: both must agree */
             ZbdRep predicted; for (int k = 0; k < 3; k++) predicted.r[k] = zbd_rep_resolve(o.transfer.r[k], &rep);
@@ -150,3 +157,29 @@ extern "C" size_t zbh_decompress_usingDict(void* dstv, size_t cap, const void* s
     return out;
 }
 extern "C" size_t zbh_decompress(void* dst, size_t cap, const void* src, size_t size) { return zbh_decompress_usingDict(dst, cap, src, size, NULL, 0); }
+
+#ifdef ZBH_CORPUS_MAIN
+/* A program over a corpus of inputs, for runs under sanitizers (tests/test_decode_invalid.py): stdin holds records
+ * u64 cap, u64 dictSize, dict, u64 size, src (little-endian); stdout gets one line per record: the return value, the
+ * sum of out[i] * (i + 1) mod 2^64 over the output, and whether the 16 bytes behind dst[cap) kept their value. */
+#include <stdio.h>
+static bool readAll(void* p, size_t n) { return fread(p, 1, n, stdin) == n; }
+int main()
+{
+    unsigned long long cap, dn, sn;
+    while (readAll(&cap, 8)) {
+        std::vector<u8> d, s, out(cap + 16, 0xA5);
+        if (!readAll(&dn, 8)) return 2;
+        d.resize(dn); if (dn && !readAll(d.data(), dn)) return 2;
+        if (!readAll(&sn, 8)) return 2;
+        s.resize(sn); if (sn && !readAll(s.data(), sn)) return 2;
+        size_t const r = zbh_decompress_usingDict(out.data(), cap, s.data(), sn, dn ? d.data() : NULL, dn);
+        unsigned long long h = 0;
+        if (r <= cap) for (size_t i = 0; i < r; i++) h += (unsigned long long)out[i] * (i + 1);
+        bool guard = true;
+        for (size_t i = 0; i < 16; i++) guard = guard && out[cap + i] == 0xA5;
+        printf("%zu %llu %d\n", r, h, guard ? 1 : 0);
+    }
+    return 0;
+}
+#endif

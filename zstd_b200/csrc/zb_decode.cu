@@ -7,9 +7,16 @@
  *   HUF_decompress4X1 / HUF_readDTableX1              (lib/decompress/huf_decompress.c:602, :383)
  * Any frame the format allows is accepted (this library's own and the reference encoder's, every level), window
  * sizes up to 128 MiB, raw-content and zstd-format dictionaries (ZSTD_decompress_usingDict, zstd_decompress.c:1133).
- * Offsets are kept in 28 bits: a frame whose offsets need more than 27 bits gets frameParameter_windowTooLarge (16)
- * whatever its header says (a window descriptor above 2^27 from the walk; a Single_Segment frame, which states no window,
- * from the first such offset code).
+ * Inputs the format does not allow are refused with a ZSTD error code, as the reference's ZSTD_decompress refuses them
+ * (tests/test_decode_invalid.py), except where this decoder is deliberately stricter; the reference's one-shot call
+ * accepts these:
+ *   - offsets are kept in 28 bits: a frame whose offsets need more than 27 bits gets frameParameter_windowTooLarge (16)
+ *     whatever its header says (a window descriptor above 2^27 from the walk; a Single_Segment frame, which states no
+ *     window, from the first such offset code);
+ *   - every block is bounded by Block_Maximum_Size = min(window, 128 KiB): a raw or RLE block larger than that, and a
+ *     compressed block that regenerates more, are corruption_detected (20), as in the reference's streaming decoder;
+ *   - a Huffman stream of the literals must end exactly at its first byte (corruption_detected).
+ * Device calls do not verify content checksums; host calls and ZSTD_decompressStream do.
  * The format-level functions are in zb_decode_core.cuh.
  *
  *   D0  walker    frames and blocks of the input: block headers, section headers, which earlier block a treeless /
@@ -166,7 +173,7 @@ zbd_sequences_kernel(const u8* __restrict__ src, const ZbdBlock* __restrict__ bl
             if (zbd_locateDescriptions(&b, sec, avail, desc, &bitstream, wk.norm[0])) e = ZBD_CORRUPT;
             else e = zbd_decodeSequences(seqs + b.seqPos, b.nbSeq, sec + bitstream, avail - bitstream, wk.table[0], wk.log[0], wk.table[1], wk.log[1],
                                          wk.table[2], wk.log[2], &sumLL, &sumML, &tr);
-            if (!e && (sumLL > b.litRegen || b.litRegen + sumML > ZB_BLOCK_MAX)) e = ZBD_CORRUPT;
+            if (!e && (sumLL > b.litRegen || b.litRegen + sumML > b.blockMax)) e = ZBD_CORRUPT;
         }
         o.regen = e ? 0u : b.litRegen + sumML; o.sumLL = sumLL; o.transfer = tr;
         if (e) o.err = e;
@@ -817,14 +824,16 @@ extern "C" size_t ZSTD_findFrameCompressedSize(const void* src, size_t srcSize)
  * The GPU decodes whole frames, so the stream front end collects compressed bytes until a frame is complete
  * (ZSTD_findFrameCompressedSize), decodes it, and hands the result out as the caller makes room.  Return value as in the
  * reference: 0 when a frame has been decoded and handed out completely, else a hint (> 0) for the next input size. */
-static size_t zbd_frameOutputBound(const u8* in, size_t size)          /* content size, or blocks x 128 KiB when the header does not say */
+/* the content size, capped at what the frame's blocks can regenerate (blocks x 128 KiB): a corrupt content-size field
+ * must not size the output buffer */
+static size_t zbd_frameOutputBound(const u8* in, size_t size)
 {
     ZbdFrameHeader h;
     if (zbd_readFrameHeader(&h, in, size) || h.skippable) return 0;
-    if (h.contentSize != ZBD_CONTENTSIZE_UNKNOWN) return (size_t)h.contentSize;
     size_t p = h.headerSize, blocks = 0;
     while (p + 3 <= size) { u32 const bh = zbd_le(in + p, 3); blocks++; p += 3u + (((bh >> 1) & 3u) == ZB_BT_RLE ? 1u : (bh >> 3)); if (bh & 1u) break; }
-    return blocks * (size_t)ZB_BLOCK_MAX;
+    size_t const most = blocks * (size_t)ZB_BLOCK_MAX;
+    return h.contentSize < (u64)most ? (size_t)h.contentSize : most;
 }
 extern "C" ZSTD_DStream* ZSTD_createDStream(void) { return ZSTD_createDCtx(); }
 extern "C" size_t ZSTD_freeDStream(ZSTD_DStream* zds) { return ZSTD_freeDCtx(zds); }
@@ -862,7 +871,8 @@ extern "C" size_t ZSTD_decompressStream(ZSTD_DStream* d, ZSTD_outBuffer* out, ZS
         }
         size_t const bound = zbd_frameOutputBound(d->dsIn->data(), fs);
         size_t const base = d->dsOut->size();
-        d->dsOut->resize(base + bound + 1);
+        try { d->dsOut->resize(base + bound + 1); }
+        catch (const std::exception&) { return ZB_ERR(ZB_error_memory_allocation); }     /* no C++ exception may cross the C ABI */
         size_t const r = ZSTD_decompressDCtx(d, d->dsOut->data() + base, bound, d->dsIn->data(), fs);
         if (ZSTD_isError(r)) { d->dsOut->resize(base); return r; }
         d->dsOut->resize(base + r);

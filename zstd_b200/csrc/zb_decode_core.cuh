@@ -181,7 +181,7 @@ typedef struct {
     u32 mode[3];           /* 0 = LL, 1 = OF, 2 = ML: 0 predefined, 1 RLE, 2 compressed, 3 repeat */
     u32 eff[3];            /* what a stream finally uses once repeat chains are resolved: 0 predefined, 1 RLE, 2 compressed */
     u32 fseSrc[3];         /* block whose sequences section holds that RLE byte / table description (itself unless repeat) */
-    u32 pad;
+    u32 blockMax;          /* Block_Maximum_Size of its frame, min(window, 128 KiB): bounds the block's regenerated size */
     u64 litPos;            /* where the block's literals go in the literal workspace (multiples of 16) */
     u64 seqPos;            /* index of its first decoded sequence in the sequence workspace */
 } ZbdBlock;
@@ -599,13 +599,14 @@ ZBD_HDN u32 zbd_walk(const u8* src, u64 size, ZbdBlock* blocks, u32 capB, ZbdFra
             if (bsz > blockMax) return ZBD_CORRUPT;               /* Block_Maximum_Size = min(window, 128 KiB) */
             if (p + 3u + csz > size) return 72u;
             ZbdBlock b; memset(&b, 0, sizeof(b));
-            b.srcOff = p + 3u; b.cSize = csz; b.type = type; b.rawSize = type == ZB_BT_COMPRESSED ? 0u : bsz; b.frame = nf;
+            b.srcOff = p + 3u; b.cSize = csz; b.type = type; b.rawSize = type == ZB_BT_COMPRESSED ? 0u : bsz; b.frame = nf; b.blockMax = (u32)blockMax;
             b.flags = (first ? ZB_FLAG_FIRST : 0u) | (last ? ZB_FLAG_LAST : 0u);
             b.hufSrc = ZBD_NONE; b.fseSrc[0] = b.fseSrc[1] = b.fseSrc[2] = ZBD_NONE;
             if (type == ZB_BT_COMPRESSED) {
                 const u8* const c = src + p + 3u;
                 if (csz < 2u) return ZBD_CORRUPT;
                 if (zbd_readLitHeader(&b, c, csz)) return ZBD_CORRUPT;
+                if (b.litRegen > blockMax) return ZBD_CORRUPT;   /* the whole regenerated size, literals + matches: D2 */
                 if (b.litType == 2u) lastHuf = nb;
                 if (b.litType >= 2u) { if (lastHuf == ZBD_NONE) return ZBD_CORRUPT; b.hufSrc = lastHuf; }
                 b.seqOff = b.litHdr + b.litComp;
