@@ -1,0 +1,112 @@
+"""Long-distance matching test helpers: the oracle's LDM frame (oracle/zb_ldm.c), the reference's LDM frame, the oracle's
+survivors, and the inputs the LDM tests share.  TEST INFRASTRUCTURE ONLY."""
+import ctypes
+
+import numpy as np
+
+import zref
+
+_sz, _vp = ctypes.c_size_t, ctypes.c_void_p
+PIECE = 1 << 20                       # A+B+A pieces: the copy lies beyond the parse's reach (128 KiB primed per chunk)
+
+
+class LdmParams(ctypes.Structure):
+    _fields_ = [("hashLog", ctypes.c_uint), ("minMatch", ctypes.c_uint), ("bucketSizeLog", ctypes.c_uint), ("hashRateLog", ctypes.c_uint)]
+
+
+def _o():
+    O = zref.oracle()
+    if not getattr(O, "_ldm_bound", False):
+        O.zbo_compress_ldm.restype = _sz
+        O.zbo_compress_ldm.argtypes = [_vp, _sz, _vp, _sz, ctypes.c_int, ctypes.POINTER(LdmParams)]
+        O.zbo_ldm_resolve.restype = LdmParams
+        O.zbo_ldm_resolve.argtypes = [ctypes.POINTER(LdmParams), ctypes.c_uint]
+        O.zbo_ldm_survivors.restype = _sz
+        O.zbo_ldm_survivors.argtypes = [_vp, _sz, ctypes.POINTER(LdmParams), _vp, _vp]
+        O._ldm_bound = True
+    return O
+
+
+def oracle_ldm(src: bytes, level: int, hash_log=0, min_match=0, bucket_size_log=0, hash_rate_log=0) -> bytes:
+    """zbo_compress_ldm: the frame the GPU must produce with ZSTD_c_enableLongDistanceMatching = 1."""
+    O = _o()
+    prm = LdmParams(hash_log, min_match, bucket_size_log, hash_rate_log)
+    cap = O.zbo_compressBound(len(src)) + 64
+    dst = ctypes.create_string_buffer(cap)
+    r = O.zbo_compress_ldm(dst, cap, src, len(src), level, ctypes.byref(prm))
+    if r > (1 << 63):
+        raise RuntimeError(f"oracle error {-(r - (1 << 64))}")
+    return dst.raw[:r]
+
+
+def resolve(window_log: int, hash_log=0, min_match=0, bucket_size_log=0, hash_rate_log=0) -> LdmParams:
+    prm = LdmParams(hash_log, min_match, bucket_size_log, hash_rate_log)
+    return _o().zbo_ldm_resolve(ctypes.byref(prm), window_log)
+
+
+def survivors(src: bytes, prm: LdmParams) -> np.ndarray:
+    """positions of the split points that survive the thinning (steps 1 and 2 of the rule)"""
+    cap = len(src) // prm.minMatch + 1
+    pos = np.zeros(cap, dtype=np.uint64)
+    v = np.zeros(cap, dtype=np.uint64)
+    n = _o().zbo_ldm_survivors(src, len(src), ctypes.byref(prm), pos.ctypes.data, v.ctypes.data)
+    return pos[:n]
+
+
+def ref_compress2(src: bytes, level: int, ldm: int) -> bytes:
+    """the reference's ZSTD_compress2 with ZSTD_c_enableLongDistanceMatching = ldm (1 enable, 2 disable)"""
+    R = zref.ref()
+    R.ZSTD_CCtx_setParameter.restype = _sz
+    R.ZSTD_CCtx_setParameter.argtypes = [_vp, ctypes.c_int, ctypes.c_int]
+    R.ZSTD_compress2.restype = _sz
+    R.ZSTD_compress2.argtypes = [_vp, _vp, _sz, _vp, _sz]
+    c = R.ZSTD_createCCtx()
+    try:
+        assert not R.ZSTD_isError(R.ZSTD_CCtx_setParameter(c, 100, level))
+        assert not R.ZSTD_isError(R.ZSTD_CCtx_setParameter(c, 160, ldm))
+        cap = R.ZSTD_compressBound(len(src))
+        dst = ctypes.create_string_buffer(cap)
+        r = R.ZSTD_compress2(c, dst, cap, src, len(src))
+        assert not R.ZSTD_isError(r), R.ZSTD_getErrorName(r)
+        return dst.raw[:r]
+    finally:
+        R.ZSTD_freeCCtx(c)
+
+
+def aba(piece: int = PIECE) -> bytes:
+    """A + B + A: the second A is a copy `2 * piece` bytes back"""
+    a, b = zref.synthetic(piece, seed=1), zref.synthetic(piece, seed=2)
+    return a + b + a
+
+
+def versions(size: int = 256 << 10, count: int = 16, edits: int = 400, seed: int = 3) -> bytes:
+    """`count` versions of one file, each `edits` random byte edits away from the one before"""
+    rng = np.random.default_rng(seed)
+    cur = np.frombuffer(zref.synthetic(size, seed=seed), dtype=np.uint8).copy()
+    out = []
+    for _ in range(count):
+        out.append(cur.tobytes())
+        idx = rng.integers(0, size, edits)
+        cur[idx] = rng.integers(0, 256, edits, dtype=np.uint8)
+    return b"".join(out)
+
+
+def period(n: int = 8 << 20, p: int = 4 << 10, seed: int = 5) -> bytes:
+    unit = zref.random_bytes(p, seed=seed)
+    return (unit * (n // p + 1))[:n]
+
+
+def inputs():
+    """name -> bytes: the inputs every LDM path is held to"""
+    return {
+        "aba": aba(),
+        "versions": versions(),
+        "zeros": bytes(8 << 20),
+        "random": zref.random_bytes(8 << 20, seed=4),
+        "period4k": period(),
+    }
+
+
+# parameter corners: minMatch 4 with hashRateLog 0, bucketSizeLog 1 and 8, hashLog 6 and 30
+CORNERS = [dict(min_match=4, hash_rate_log=0), dict(min_match=4, hash_rate_log=1), dict(bucket_size_log=1), dict(bucket_size_log=8),
+           dict(hash_log=6), dict(hash_log=30)]

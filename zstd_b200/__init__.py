@@ -234,7 +234,9 @@ class ZSTD_CCtx:
         return dst.raw[:r]
 
     # -- advanced one-shot API (lib/zstd.h:337-603) --
-    PARAMS = {"compression_level": 100, "content_size_flag": 200, "checksum_flag": 201, "dict_id_flag": 202, "nb_workers": 400}
+    PARAMS = {"compression_level": 100, "content_size_flag": 200, "checksum_flag": 201, "dict_id_flag": 202, "nb_workers": 400,
+              "enable_long_distance_matching": 160, "ldm_hash_log": 161, "ldm_min_match": 162, "ldm_bucket_size_log": 163,
+              "ldm_hash_rate_log": 164}
 
     def set_parameter(self, name_or_id, value: int) -> None:
         """ZSTD_CCtx_setParameter: sticky until ZSTD_CCtx_reset(parameters)."""

@@ -35,7 +35,9 @@ static const Row kRows[4][5] = {
     { {14,12,13,1,5,1,1}, {14,14,15,1,5,0,1}, {14,14,15,1,4,0,1}, {14,14,15,2,4,0,2}, {14,14,15,2,4,0,2} },
 };
 
-static ZbCParams zb_getCParams(int level, u64 srcSize, size_t dictSize)
+/* ldm: long-distance matching, whose window is ZSTD_LDM_DEFAULT_WINDOW_LOG before the size adjustment (ZSTD_getCParamsFromCCtxParams,
+ * zstd_compress.c:1639) */
+static ZbCParams zb_getCParams(int level, u64 srcSize, size_t dictSize, bool ldm = false)
 {
     u64 const rSize = srcSize + dictSize;
     u32 const tableID = (rSize <= 256u * 1024) + (rSize <= 128u * 1024) + (rSize <= 16u * 1024);
@@ -46,6 +48,7 @@ static ZbCParams zb_getCParams(int level, u64 srcSize, size_t dictSize)
         int const minLevel = -(int)ZB_BLOCK_MAX;                 /* ZSTD_minCLevel, zstd_compress.c:7038 */
         cp.targetLength = (u32)(-(level < minLevel ? minLevel : level));
     }
+    if (ldm) cp.windowLog = ZB_LDM_WINDOW_LOG;
     {   u64 const maxWindowResize = 1ull << 30;                  /* zstd_compress.c:1537-1547 */
         if (srcSize <= maxWindowResize && dictSize <= maxWindowResize) {
             u32 const tSize = (u32)(srcSize + dictSize);
@@ -154,6 +157,11 @@ struct ZSTD_CCtx_s {
     ZSTDB200_stats stats;
     /* advanced one-shot API (ZSTD_CCtx_setParameter + ZSTD_compress2, lib/zstd.h:337-603): sticky parameters */
     int advLevel, advChecksum, advNoDictID;
+    int advLdm;                    /* ZSTD_c_enableLongDistanceMatching: 1 = on (0 auto and 2 disable are off) */
+    u32 advLdmPrm[4];              /* ZSTD_c_ldmHashLog, ldmMinMatch, ldmBucketSizeLog, ldmHashRateLog; 0 = derived from the window */
+    /* long-distance matching workspace: the call's match list and per-block (first, count), one frame's scratch */
+    u64* d_ldmMatch; size_t d_ldmMatchCap; u64* d_ldmFirst; size_t d_ldmFirstCap; u32* d_ldmCnt; size_t d_ldmCntCap;
+    void* d_ldmScratch; size_t d_ldmScratchCap;
     ZSTD_CDict* advLocalDict;      /* ZSTD_CCtx_loadDictionary: owned copy, digested at its first use */
     const ZSTD_CDict* advRefCDict; /* ZSTD_CCtx_refCDict: borrowed */
     struct ZbPlan* plan;           /* the call's plan; its vectors are reused (a million records are 100 MB of descriptors: fresh pages cost more than filling them) */
@@ -281,6 +289,7 @@ extern "C" size_t ZSTD_freeCCtx(ZSTD_CCtx* c)
         zb_freeWaveEvents(c);
         cudaFree(c->d_in); cudaFree(c->d_out);
         cudaFree(c->d_seqIn); cudaFree(c->d_seqTile); cudaFree(c->d_seqBlk); cudaFree(c->d_seqCtrl);
+        cudaFree(c->d_ldmMatch); cudaFree(c->d_ldmFirst); cudaFree(c->d_ldmCnt); cudaFree(c->d_ldmScratch);
         for (u32 s = 0; s <= ZB_WAVE_SLOTS_MAX; s++) if (c->waveStream[s]) cudaStreamDestroy(c->waveStream[s]);
         cudaEventDestroy(c->evStart); cudaEventDestroy(c->evK0); cudaEventDestroy(c->evK1);
         cudaEventDestroy(c->evK2); cudaEventDestroy(c->evK3); cudaEventDestroy(c->evMid);
@@ -347,7 +356,7 @@ static size_t zb_ensureHeavy(ZSTD_CCtx* c, size_t nbSlotBlocks, const ZbStrides&
  * FSE tables are that block's "previous" entropy state (treeless literals, set_repeat sequence tables) and
  * its repcodes start the block.  Parsing: zb_dict.cu. */
 /* ------------------------------------------------------------------ planning (ZSTD_compress_frameChunk, zstd_compress.c:4527) */
-struct ZbGroup { ZbParams prm; u32 b0, b1, c0, c1; const u32* image; };   /* image: tables walked over the dictionary tail, or NULL */
+struct ZbGroup { ZbParams prm; u32 b0, b1, c0, c1; const u32* image; bool ldm; };   /* ldm: its frames have long-distance matches */   /* image: tables walked over the dictionary tail, or NULL */
 /* Descriptor arrays of a plan: page-locked (so that the upload of a million frames' descriptors is a DMA at PCIe speed, not a
  * staged copy of pageable memory) and kept across calls.  Without a CUDA device (the CPU tests' ZSTDB200_describePlan)
  * ordinary memory is used. */
@@ -376,9 +385,11 @@ template <typename T> struct ZbVec {
     T& operator[](size_t i) { return p[i]; }
     const T& operator[](size_t i) const { return p[i]; }
 };
+struct ZbLdmFrame { u32 frame; ZbLdmParams prm; u64 matchBase; };
 struct ZbPlan { ZbVec<ZbBlock> blocks; ZbVec<ZbChunk> chunks; ZbVec<ZbFrame> frames; std::vector<ZbGroup> groups; ZbStrides sd; bool unsupported;
+                std::vector<ZbLdmFrame> ldm; u64 ldmMatches;      /* frames with long-distance matching, their share of the match list */
                 u64 frameBytes, frameBlocks; u32 frameMaxBlock;   /* the whole frames, other ranks' blocks included: what decides the waves */
-                void reset() { blocks.clear(); chunks.clear(); frames.clear(); groups.clear(); unsupported = false;
+                void reset() { blocks.clear(); chunks.clear(); frames.clear(); groups.clear(); unsupported = false; ldm.clear(); ldmMatches = 0;
                                frameBytes = frameBlocks = 0; frameMaxBlock = 0; } };   /* keeps its memory: a context plans call after call */
 
 /* One compression call, as every entry point hands it to the executor (zb_compress) */
@@ -390,6 +401,7 @@ struct ZbCall {
     bool deviceMemory; cudaStream_t stream;                       /* stream: the caller's, or NULL; host-memory calls ignore it */
     bool checksum, noDictID;                                      /* frame header options */
     u64 partBegin = 0, partEnd = ~0ull;                           /* ZSTDB200_compressFramePart: this rank's share of the one frame */
+    const u32* ldm = nullptr;                                     /* long-distance matching: the 4 ldm parameters (0 = derived), or NULL */
 };
 
 static void zb_freePlan(ZbPlan* p) { delete p; }
@@ -398,6 +410,22 @@ static int g_strictLevels = 0;
  * by default they are served by the strongest doubleFast row of their size class (larger output than the reference's at
  * that level); after ZSTDB200_setStrictLevels(1) such calls fail with parameter_unsupported instead. */
 extern "C" void ZSTDB200_setStrictLevels(int on) { g_strictLevels = on; }
+
+/* ZSTD_ldm_adjustParameters (zstd_ldm.c:135) for a frame of window 2^windowLog; v = the 4 sticky values, 0 = derived */
+static ZbLdmParams zb_ldmResolve(const u32* v, u32 windowLog)
+{
+    ZbLdmParams p; memset(&p, 0, sizeof(p));
+    p.hashLog = v[0]; p.minMatch = v[1]; p.bucketSizeLog = v[2]; p.hashRateLog = v[3]; p.windowLog = windowLog;
+    if (!p.bucketSizeLog) p.bucketSizeLog = 3;                                       /* LDM_BUCKET_SIZE_LOG */
+    if (!p.minMatch) p.minMatch = 64;                                                /* LDM_MIN_MATCH_LENGTH */
+    if (!p.hashLog) p.hashLog = windowLog > 7u + 6u ? windowLog - 7u : 6u;           /* MAX(ZSTD_HASHLOG_MIN, windowLog - LDM_HASH_RLOG) */
+    if (!p.hashRateLog) p.hashRateLog = windowLog < p.hashLog ? 0u : windowLog - p.hashLog;
+    if (p.bucketSizeLog > p.hashLog) p.bucketSizeLog = p.hashLog;
+    u32 const maxBits = p.minMatch < 64u ? p.minMatch : 64u;                         /* ZSTD_ldm_gear_init, zstd_ldm.c:32-60 */
+    p.stopMask = (p.hashRateLog > 0u && p.hashRateLog <= maxBits) ? (((1ull << p.hashRateLog) - 1ull) << (maxBits - p.hashRateLog))
+                                                                   : ((1ull << p.hashRateLog) - 1ull);
+    return p;
+}
 
 /* partBegin / partEnd: only the blocks that start inside [partBegin, partEnd) of the (single) frame are planned — one rank's
  * share of a frame that several GPUs compress together (ZSTDB200_compressFramePart); the geometry is the whole frame's. */
@@ -429,8 +457,14 @@ static void zb_plan(ZbPlan& P, const ZbCall& a, size_t dictSize, size_t dictTail
             P.groups.back().c1 = (u32)P.chunks.size();
             continue;
         }
-        ZbCParams cp = zb_getCParams(level, fsz, dictSize);
+        bool const ldm = a.ldm && fsz > ZB_LDM_MIN_FRAME;        /* a frame of one chunk is parsed whole: compressed as without LDM */
+        ZbCParams cp = zb_getCParams(level, fsz, dictSize, ldm);
         ZbParams prm = zb_makeParams(cp);
+        if (ldm) {
+            ZbLdmFrame lf; lf.frame = (u32)f; lf.prm = zb_ldmResolve(a.ldm, cp.windowLog); lf.matchBase = P.ldmMatches;
+            P.ldm.push_back(lf);
+            P.ldmMatches += zb_ldm_survivor_cap(fsz, lf.prm.minMatch);
+        }
         if (dictRep) {                                           /* a zstd-format dictionary's repcodes (zstd_compress.c:5054-5056) */
             prm.codeRep[0] = dictRep[0]; prm.codeRep[1] = dictRep[1]; prm.codeRep[2] = dictRep[2];
             prm.startRep[0] = dictRep[0] <= dictTail ? dictRep[0] : 0u; prm.startRep[1] = dictRep[1] <= dictTail ? dictRep[1] : 0u;
@@ -474,8 +508,8 @@ static void zb_plan(ZbPlan& P, const ZbCall& a, size_t dictSize, size_t dictTail
         fr.nbBlocks = (u32)P.blocks.size() - fr.firstBlock;
         P.frames[f] = fr;
         if (fr.nbBlocks == 1u) { tplSize = fsz; tplFrame = fr; tplBlock = P.blocks.back(); tplChunk = P.chunks.back(); } else tplSize = ~0ull;
-        if (P.groups.empty() || memcmp(&P.groups.back().prm, &prm, sizeof(prm)) != 0) {
-            ZbGroup g; g.prm = prm; g.b0 = fr.firstBlock; g.b1 = (u32)P.blocks.size(); g.c0 = firstChunk; g.c1 = (u32)P.chunks.size(); g.image = NULL; P.groups.push_back(g);
+        if (P.groups.empty() || memcmp(&P.groups.back().prm, &prm, sizeof(prm)) != 0 || P.groups.back().ldm != ldm) {
+            ZbGroup g; g.prm = prm; g.b0 = fr.firstBlock; g.b1 = (u32)P.blocks.size(); g.c0 = firstChunk; g.c1 = (u32)P.chunks.size(); g.image = NULL; g.ldm = ldm; P.groups.push_back(g);
         } else { P.groups.back().b1 = (u32)P.blocks.size(); P.groups.back().c1 = (u32)P.chunks.size(); }
     }
     P.sd = zb_strides(maxBlock);
@@ -547,6 +581,38 @@ static size_t zb_buildDictImages(ZSTD_CDict* cd, ZbPlan& P, bool shared, cudaStr
     return 0;
 }
 
+/* Long-distance matching (zb_ldm.cu): every LDM frame's matches, by block index in the call, before the first wave (a block
+ * may copy from anywhere in its 2^27-byte window, i.e. from any earlier wave).  The frames run one after another on
+ * `stream` through one scratch area. */
+static size_t zb_runLdm(ZSTD_CCtx* c, const ZbPlan& P, const u8* d_src, cudaStream_t stream, unsigned* launches)
+{
+    size_t scratch = 0;
+    for (size_t i = 0; i < P.ldm.size(); i++) {
+        size_t const b = zb_ldm_scratch_bytes(P.frames[P.ldm[i].frame].srcSize, &P.ldm[i].prm);
+        if (b > scratch) scratch = b;
+    }
+    size_t const nbBlocks = P.blocks.size();
+    auto grow = [](void** p, size_t* cap, size_t bytes) -> size_t {
+        if (bytes <= *cap) return 0;
+        cudaFree(*p); *p = NULL; *cap = 0;
+        CK(cudaMalloc(p, bytes));
+        *cap = bytes;
+        return 0;
+    };
+    size_t e = grow((void**)&c->d_ldmMatch, &c->d_ldmMatchCap, P.ldmMatches * sizeof(u64)); if (zb_isErr(e)) return e;
+    e = grow((void**)&c->d_ldmFirst, &c->d_ldmFirstCap, nbBlocks * sizeof(u64)); if (zb_isErr(e)) return e;
+    e = grow((void**)&c->d_ldmCnt, &c->d_ldmCntCap, nbBlocks * sizeof(u32)); if (zb_isErr(e)) return e;
+    e = grow(&c->d_ldmScratch, &c->d_ldmScratchCap, scratch); if (zb_isErr(e)) return e;
+    for (size_t i = 0; i < P.ldm.size(); i++) {
+        ZbLdmFrame const& lf = P.ldm[i];
+        ZbFrame const& fr = P.frames[lf.frame];
+        CK(zb_launch_ldm(d_src + fr.srcOff, fr.srcSize, &lf.prm, c->d_ldmScratch, fr.nbBlocks, lf.matchBase, c->d_ldmMatch,
+                         c->d_ldmFirst + fr.firstBlock, c->d_ldmCnt + fr.firstBlock, stream));
+        *launches += 4u + 3u * ((lf.prm.hashLog - lf.prm.bucketSizeLog + 7u) / 8u);   /* split, scan, compact, radix passes, select */
+    }
+    return 0;
+}
+
 /* K1..K3 for blocks [b0, b1) = chunks [c0, c1) using workspace slot positions [slot0, slot0 + (b1-b0)); d_de: the
  * dictionary's entropy tables when it is zstd-format, else NULL */
 static size_t zb_runBlocks(ZSTD_CCtx* c, const ZbPlan& P, const u8* d_src, const u8* d_dictEnd, const ZbDictEntropy* d_de, u32 b0, u32 b1, u32 c0, u32 c1, size_t slot0,
@@ -561,10 +627,11 @@ static size_t zb_runBlocks(ZSTD_CCtx* c, const ZbPlan& P, const u8* d_src, const
             size_t const s = slot0 + (lo - b0);
             if (phase == 0) {
                 bool const df = G.prm.strategy == 2;
+                ZbLdmView lv; lv.match = c->d_ldmMatch; lv.first = c->d_ldmFirst + lo; lv.cnt = c->d_ldmCnt + lo;
                 CK(zb_launch_match(d_src, d_dictEnd, d_dictEnd ? G.image : (const u32*)0, c->d_blocks + lo, hi - lo, c->d_chunks + clo, chi - clo, lo, &G.prm, &P.sd,
                                    c->d_dist + s * P.sd.dist, c->d_far + s * P.sd.dist, df ? c->d_dist2 + s * P.sd.dist : (u16*)0, df ? c->d_far2 + s * P.sd.dist : (u32*)0,
                                    c->d_seqs + s * P.sd.seq, c->d_lits + s * P.sd.lit, c->d_meta + s, c->d_segmeta + s * ((P.sd.dist + ZB_PARSE_SEG - 1u) / ZB_PARSE_SEG),
-                                   (timed && P.groups.size() == 1) ? c->evMid : (cudaEvent_t)0, stream));
+                                   (timed && P.groups.size() == 1) ? c->evMid : (cudaEvent_t)0, stream, G.ldm ? &lv : nullptr));
                 *launches += df ? 4 : 3;       /* walk(s), parse, merge */
             } else if (phase == 1) {
                 CK(zb_launch_literals(c->d_blocks + lo, hi - lo, &G.prm, &P.sd, d_de, c->d_lits + s * P.sd.lit, c->d_body + s * P.sd.body, c->d_meta + s, stream));
@@ -708,10 +775,17 @@ static size_t zb_compress(ZSTD_CCtx* c, const ZbCall& a)
     if (single) CK(cudaEventRecord(c->evK0, sCopy));
     if (cd && (nbFrames >= 8 || shared)) { size_t const e = zb_buildDictImages(cd, P, shared, sCopy); if (zb_isErr(e)) return e; }   /* a per-call digest builds its images afresh on every call: only for 8 frames or more */
     cudaStream_t lastStream = sCopy;
+    bool const ldm = !P.ldm.empty();
+    if (ldm) {
+        /* host buffers: the whole input goes up first (a block may copy from any earlier wave), so this upload does not
+         * overlap the kernels as the per-wave uploads do */
+        if (!deviceMemory) CK(cudaMemcpyAsync(d_in, src, inEnd, cudaMemcpyHostToDevice, sCopy));
+        err = zb_runLdm(c, P, d_in, sCopy, &launches);
+    }
     for (u32 w = 0; w < nbWaves && !err; w++) {
         u32 const b0 = wb[w], b1 = wb[w + 1];
         size_t const s0 = (size_t)(w % slots) * maxWaveBlocks;
-        if (!deviceMemory) {
+        if (!deviceMemory && !ldm) {
             /* input bytes of the wave (frames are laid out in offset order; history was uploaded by earlier waves) */
             u64 lo = ~0ull, hi = 0;
             for (u32 b = b0; b < b1; b++) { u64 const s = P.blocks[b].srcOff, e = s + P.blocks[b].size; if (s < lo) lo = s; if (e > hi) hi = e; }
@@ -833,6 +907,9 @@ static size_t zb_digestCallDict(ZSTD_CCtx* c, const void* dict, size_t dictSize,
     return 0;
 }
 
+/* the sticky long-distance-matching parameters of a call that honours them, or NULL when LDM is off */
+static const u32* zb_ldmArg(const ZSTD_CCtx* c) { return c->advLdm ? c->advLdmPrm : nullptr; }
+
 extern "C" size_t ZSTDB200_compressFrames(ZSTD_CCtx* c, void* dst, size_t dstCapacity,
                                           const void* src, const size_t* frameOffsets, const size_t* frameSizes,
                                           size_t nbFrames, const void* dict, size_t dictSize,
@@ -841,8 +918,9 @@ extern "C" size_t ZSTDB200_compressFrames(ZSTD_CCtx* c, void* dst, size_t dstCap
     if (!c) return ZB_ERR(ZB_error_GENERIC);
     const ZSTD_CDict* cd;
     {   size_t const e = zb_digestCallDict(c, dict, dictSize, &cd); if (zb_isErr(e)) return e; }
-    ZbCall const a = { dst, dstCapacity, src, frameOffsets, frameSizes, nbFrames, cd, level, cSizes, deviceMemory != 0,
-                       (cudaStream_t)streamv, c->advChecksum != 0, c->advNoDictID != 0 };      /* the sticky frame parameters of ZSTD_CCtx_setParameter apply */
+    ZbCall a = { dst, dstCapacity, src, frameOffsets, frameSizes, nbFrames, cd, level, cSizes, deviceMemory != 0,
+                 (cudaStream_t)streamv, c->advChecksum != 0, c->advNoDictID != 0 };            /* the sticky frame parameters of ZSTD_CCtx_setParameter apply */
+    a.ldm = zb_ldmArg(c);
     return zb_compress(c, a);
 }
 
@@ -853,19 +931,21 @@ extern "C" size_t ZSTDB200_compressFrames_usingCDict(ZSTD_CCtx* c, void* dst, si
 {
     if (!cdict) return ZB_ERR(ZB_error_dictionary_wrong);                        /* zstd_compress.c:5753 */
     if (!c) return ZB_ERR(ZB_error_GENERIC);
-    ZbCall const a = { dst, dstCapacity, src, frameOffsets, frameSizes, nbFrames, cdict, cdict->level, cSizes, deviceMemory != 0,
-                       (cudaStream_t)streamv, c->advChecksum != 0, c->advNoDictID != 0 };
+    ZbCall a = { dst, dstCapacity, src, frameOffsets, frameSizes, nbFrames, cdict, cdict->level, cSizes, deviceMemory != 0,
+                 (cudaStream_t)streamv, c->advChecksum != 0, c->advNoDictID != 0 };
+    a.ldm = zb_ldmArg(c);
     return zb_compress(c, a);
 }
 
 /* ZSTD_compress_usingDict, ZSTD_compress_usingCDict, ZSTD_compress2: one frame from host buffers (c is not NULL) */
 static size_t zb_compressOne(ZSTD_CCtx* c, void* dst, size_t dstCapacity, const void* src, size_t srcSize,
-                             const ZSTD_CDict* cdict, int level, bool checksum, bool noDictID)
+                             const ZSTD_CDict* cdict, int level, bool checksum, bool noDictID, const u32* ldm = nullptr)
 {
     if (dstCapacity && !dst) return ZB_ERR(ZB_error_dstBuffer_null);
     if (dstCapacity < 18) return ZB_ERR(ZB_error_dstSize_tooSmall);             /* ZSTD_FRAMEHEADERSIZE_MAX, zstd_compress.c:4643 */
     size_t const off = 0;
-    ZbCall const a = { dst, dstCapacity, src, &off, &srcSize, 1, cdict, level, NULL, false, NULL, checksum, noDictID };
+    ZbCall a = { dst, dstCapacity, src, &off, &srcSize, 1, cdict, level, NULL, false, NULL, checksum, noDictID };
+    a.ldm = ldm;
     return zb_compress(c, a);
 }
 
@@ -932,6 +1012,7 @@ extern "C" size_t ZSTDB200_compressFramePart(ZSTD_CCtx* c, void* d_dst, size_t d
     if (!c) return ZB_ERR(ZB_error_GENERIC);
     if (partBegin % ZSTDB200_framePartAlignment() || partBegin + partSize > frameSize || (partSize == 0 && frameSize != 0)) return ZB_ERR(ZB_error_srcSize_wrong);
     if (c->advChecksum) return ZB_ERR(ZB_error_parameter_unsupported);          /* a content checksum needs the whole content in one place */
+    if (c->advLdm) return ZB_ERR(ZB_error_parameter_unsupported);               /* a rank holds a halo of 128 KiB, not the LDM window */
     size_t const halo = partBegin < ZB_PRIME_BYTES ? partBegin : ZB_PRIME_BYTES;
     const u8* const frameBase = (const u8*)d_part + halo - partBegin;          /* address frame offset 0 would have; only offsets >= partBegin - halo are touched */
     size_t const off = 0;
@@ -1024,8 +1105,16 @@ extern "C" size_t ZSTD_CCtx_setParameter(ZSTD_CCtx* c, ZSTD_cParameter paramE, i
         c->advDelims = value; return 0;
     case 1009: return (value == 0 || value == 1) ? 0 : ZB_ERR(ZB_error_parameter_unsupported);   /* ZSTD_c_validateSequences: validation always runs */
     case 101: case 102: case 103: case 104: case 105: case 106: case 107:                    /* windowLog .. strategy: default only */
-    case 160: case 161: case 162: case 163: case 164:                                        /* long distance matching: off only */
         return value == 0 ? 0 : ZB_ERR(ZB_error_parameter_unsupported);
+    case 160:                                                                                /* ZSTD_c_enableLongDistanceMatching: ZSTD_paramSwitch_e */
+        if (value < 0 || value > 2) return ZB_ERR(ZB_error_parameter_outOfBound);
+        c->advLdm = value == 1; return 0;                                                    /* auto: off (no level here is btopt or stronger, zstd_compress.c:277) */
+    case 161: case 162: case 163: case 164: {                                                /* ldmHashLog, ldmMinMatch, ldmBucketSizeLog, ldmHashRateLog */
+        static const int lo[4] = { 6, 4, 1, 0 }, hi[4] = { 30, 4096, 8, 25 };               /* lib/zstd.h:1267-1274; 0 = derived */
+        int const i = param - 161;
+        if (value != 0 && (value < lo[i] || value > hi[i])) return ZB_ERR(ZB_error_parameter_outOfBound);
+        c->advLdmPrm[i] = (u32)value; return 0;
+    }
     default: return ZB_ERR(ZB_error_parameter_unsupported);
     }
 }
@@ -1037,7 +1126,7 @@ extern "C" size_t ZSTD_CCtx_reset(ZSTD_CCtx* c, ZSTD_ResetDirective reset)      
     if (!c) return ZB_ERR(ZB_error_GENERIC);
     if (reset == 1 || reset == 3) { c->stInSize = 0; c->stOutSize = 0; c->stOutPos = 0; c->stFrames = 0; }   /* an unfinished stream is dropped */
     if (reset == 2 || reset == 3) {
-        c->advLevel = 3; c->advChecksum = 0; c->advNoDictID = 0; c->advDelims = 0;
+        c->advLevel = 3; c->advChecksum = 0; c->advNoDictID = 0; c->advDelims = 0; c->advLdm = 0; memset(c->advLdmPrm, 0, sizeof(c->advLdmPrm));
         ZSTD_freeCDict(c->advLocalDict); c->advLocalDict = NULL; c->advRefCDict = NULL;
     }
     return 0;
@@ -1065,7 +1154,7 @@ extern "C" size_t ZSTD_compress2(ZSTD_CCtx* c, void* dst, size_t dstCapacity, co
     if (!c) return ZB_ERR(ZB_error_GENERIC);
     const ZSTD_CDict* const cd = c->advRefCDict ? c->advRefCDict : c->advLocalDict;
     int const level = c->advRefCDict ? c->advRefCDict->level : c->advLevel;                  /* a referenced CDict brings its own level (:5836) */
-    return zb_compressOne(c, dst, dstCapacity, src, srcSize, cd, level, c->advChecksum != 0, c->advNoDictID != 0);
+    return zb_compressOne(c, dst, dstCapacity, src, srcSize, cd, level, c->advChecksum != 0, c->advNoDictID != 0, zb_ldmArg(c));
 }
 
 /* ------------------------------------------------------------------ sequence calls (lib/zstd.h:1555-1644)

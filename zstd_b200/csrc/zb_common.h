@@ -51,6 +51,7 @@ typedef uint64_t u64;
 #define ZB_error_dictionary_corrupted 30
 #define ZB_error_dictionary_wrong 32
 #define ZB_error_parameter_unsupported 40
+#define ZB_error_parameter_outOfBound 42
 #define ZB_error_tableLog_tooLarge 44
 #define ZB_error_maxSymbolValue_tooLarge 46
 #define ZB_error_stage_wrong 60
@@ -179,12 +180,34 @@ static inline ZB_HD ZbStrides zb_seq_strides(u32 maxBlock)
     sd.seq = M / 3u + 8u; sd.state = ((M + 2u) / 3u + 7u) & ~7u; sd.dist = 3u * sd.state;
     return sd;
 }
-#define ZB_SEQ_OFF_MAX ((1u << 24) - 4u)   /* largest offset of a sequence call: offBase = offset + 3 has 24 bits in a packed sequence */
-/* a final sequence as the sequences kernel reads it: offBase (24 bits), literal length (18 bits), match length (>= 4) */
+#define ZB_SEQ_OFF_MAX ((1u << 24) - 4u)   /* largest offset of a sequence call (the packed sequence holds 28 bits of offBase; sequence calls keep this bound) */
+/* a final sequence as the sequences kernel reads it: offBase (28 bits: long-distance offsets reach 2^27), literal length
+ * (18 bits), match length (18 bits, >= 3); both lengths are <= ZB_BLOCK_MAX */
 static inline ZB_HD u64 zb_pack_seq(u32 offBase, u32 litLen, u32 matchLen)
 {
-    return (u64)offBase | ((u64)litLen << 24) | ((u64)matchLen << 42);
+    return (u64)offBase | ((u64)litLen << 28) | ((u64)matchLen << 46);
 }
+#define ZB_SEQ_OFFBASE(q) ((u32)(q) & 0xFFFFFFFu)
+#define ZB_SEQ_LL(q)      ((u32)((q) >> 28) & 0x3FFFFu)
+#define ZB_SEQ_ML(q)      ((u32)((q) >> 46) & 0x3FFFFu)
+
+/* Long-distance matching (zb_ldm.cu; the rule: oracle/zb_ldm.c).  Frames of more than one chunk only. */
+#define ZB_LDM_WINDOW_LOG 27u                                  /* ZSTD_LDM_DEFAULT_WINDOW_LOG, zstd_ldm.h:25 */
+#define ZB_LDM_MIN_FRAME  (ZB_CHUNK_BLOCKS * ZB_BLOCK_MAX)
+#define ZB_LDM_GEAR_SEED  0x6C646D2D67656172ull                /* gear[i] = splitmix64 output i + 1 of this seed ("ldm-gear") */
+typedef struct {
+    u32 hashLog, minMatch, bucketSizeLog, hashRateLog;       /* resolved (ZSTD_ldm_adjustParameters) */
+    u32 windowLog, pad;
+    u64 stopMask;                                            /* zstd_ldm.c:32-60 */
+} ZbLdmParams;
+static inline ZB_HD u64 zb_ldm_survivor_cap(u64 n, u32 minMatch) { return n / minMatch + 1u; }   /* survivors are >= minMatch apart */
+/* an LDM match: offset (28 bits), length (18 bits), start relative to its block (18 bits) */
+static inline ZB_HD u64 zb_pack_ldm(u64 start, u64 len, u64 off) { return off | (len << 28) | (start << 46); }
+#define ZB_LDM_OFF(m)   ((u32)(m) & 0xFFFFFFFu)
+#define ZB_LDM_LEN(m)   ((u32)((m) >> 28) & 0x3FFFFu)
+#define ZB_LDM_START(m) ((u32)((m) >> 46))
+/* what K1c reads for the blocks of one launch: match[first[b] .. first[b] + cnt[b]) of block b */
+typedef struct { const u64* match; const u64* first; const u32* cnt; } ZbLdmView;
 
 #ifdef __CUDACC__
 /* host helpers of the compression and decompression drivers (zb_api.cu, zb_decode.cu) */

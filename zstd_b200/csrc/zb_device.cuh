@@ -104,4 +104,14 @@ __device__ __forceinline__ u32 zb_hash(u64 v, u32 mls, u32 hBits)
 
 __device__ __forceinline__ u32 zb_hb32(u32 v) { return 31u - (u32)__clz((int)v); }
 
+/* XXH64 rounds (lib/common/xxhash.h; XXH64 spec): the frame checksum (zb_stitch.cu) and the LDM split hash (zb_ldm.cu) */
+__device__ __forceinline__ u64 zbx_rotl(u64 x, int r) { return (x << r) | (x >> (64 - r)); }
+#define ZBX_P1 0x9E3779B185EBCA87ull
+#define ZBX_P2 0xC2B2AE3D27D4EB4Full
+#define ZBX_P3 0x165667B19E3779F9ull
+#define ZBX_P4 0x85EBCA77C2B2AE63ull
+#define ZBX_P5 0x27D4EB2F165667C5ull
+__device__ __forceinline__ u64 zbx_round(u64 acc, u64 in) { return zbx_rotl(acc + in * ZBX_P2, 31) * ZBX_P1; }
+__device__ __forceinline__ u64 zbx_merge(u64 h, u64 v) { return (h ^ zbx_round(0, v)) * ZBX_P1 + ZBX_P4; }
+
 #endif

@@ -21,7 +21,15 @@ cudaError_t zb_launch_dict_image(const u8* d_dictEnd, const ZbChunk* d_dictChunk
 cudaError_t zb_launch_match(const u8* d_src, const u8* d_dictEnd, const u32* d_image, const ZbBlock* d_blocks, u32 nbBlocks,
                             const ZbChunk* d_chunks, u32 nbChunks, u32 slotFirstBlock, const ZbParams* prm, const ZbStrides* sd,
                             u16* d_dist, u32* d_far, u16* d_dist2, u32* d_far2, u64* d_seqs, u8* d_lits, ZbBlockMeta* d_meta, ZbSegMeta* d_segmeta,
-                            cudaEvent_t evMid, cudaStream_t stream);
+                            cudaEvent_t evMid, cudaStream_t stream, const ZbLdmView* ldm = nullptr);
+/* ldm (K1c): the launch's blocks' long-distance matches (zb_launch_ldm), laid over the parse output; NULL = none */
+
+/* Long-distance matching of one frame of n bytes at d_frame (zb_ldm.cu): nbBlocks blocks of ZB_BLOCK_MAX bytes; block k's
+ * matches go to d_match[d_ldmFirst[k] .. + d_ldmCnt[k]), inside d_match[matchBase, matchBase + zb_ldm_survivor_cap(n, minMatch)).
+ * d_scratch: zb_ldm_scratch_bytes(n, prm) bytes, free again when the stream reaches the end of the launch. */
+size_t zb_ldm_scratch_bytes(u64 n, const ZbLdmParams* prm);
+cudaError_t zb_launch_ldm(const u8* d_frame, u64 n, const ZbLdmParams* prm, void* d_scratch, u32 nbBlocks,
+                          u64 matchBase, u64* d_match, u64* d_ldmFirst, u32* d_ldmCnt, cudaStream_t stream);
 
 /* K1s: caller-supplied sequences (ZSTD_Sequence[n], 16-byte aligned, device memory) in place of K1 (zb_seqimport.cu).
  * partition: per-tile sums (d_tileLen / d_tileEnds: one per 1024 sequences), scanned; d_ctrl[0] = sum of the lengths,

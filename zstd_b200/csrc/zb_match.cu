@@ -638,9 +638,89 @@ __device__ __forceinline__ u32 zb_rep_code(ZbRepHist& h, u32 off, u32 ll)
 #define MERGE_MIN_CTAS 6           /* 40 registers (parse + merge on the H100: 6.12 ms per GiB of config 2 against 6.22 with 5 and 6.41 with 4) */
 #endif
 #define SEG_SLOTS (ZB_PARSE_SEG / 4u)
+
+/* block-wide exclusive count of `flag` over the MERGE_THREADS entries of a round: returns the entries before this thread's,
+ * *total gets the round's count (wsum: MERGE_THREADS / 32 shared words) */
+__device__ __forceinline__ u32 zb_block_excl(bool flag, u32* wsum, u32* total)
+{
+    u32 const lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    u32 const bal = __ballot_sync(ZB_FULL, flag);
+    if (lane == 0u) wsum[warp] = __popc(bal);
+    __syncthreads();
+    u32 before = __popc(bal & ((1u << lane) - 1u)), t = 0;
+    for (u32 w = 0; w < MERGE_THREADS / 32u; w++) { if (w < warp) before += wsum[w]; t += wsum[w]; }
+    __syncthreads();
+    *total = t;
+    return before;
+}
+
+/* Overlay of a block's long-distance matches L[0, nL) (zb_pack_ldm, in position order) onto its parse output P[0, nP) (raw,
+ * compacted, in position order): an LDM match wins; a parse match that starts under one starts again at its end, one that
+ * runs into one is cut at its start, and a parse match shortened this way is kept only with >= 4 bytes left (the parse's
+ * shortest match: a block keeps at most size / 4 + 8 sequences).  Output: (offset, litLength, matchLength) triples in
+ * out[0, n), returns n.  kp: nP + 1 words of scratch.  oracle/zb_ldm.c (zbo_ldm_overlayBlock) is the same rule, serially. */
+__device__ __forceinline__ void zb_ldm_clip(u32 ms, u32 me, const u64* L, u32 nL, u32* ms2, u32* me2, u32* next, bool* kept)
+{
+    u32 lo = 0, hi = nL;                                          /* lo = LDM matches that start at or before ms */
+    while (lo < hi) { u32 const mid = (lo + hi) >> 1; if (ZB_LDM_START(L[mid]) <= ms) lo = mid + 1u; else hi = mid; }
+    bool clipped = false;
+    if (lo > 0u && ZB_LDM_START(L[lo - 1u]) + ZB_LDM_LEN(L[lo - 1u]) > ms) { ms = ZB_LDM_START(L[lo - 1u]) + ZB_LDM_LEN(L[lo - 1u]); clipped = true; }
+    if (lo < nL && ZB_LDM_START(L[lo]) < me) { me = ZB_LDM_START(L[lo]); clipped = true; }
+    *ms2 = ms; *me2 = me; *next = lo;
+    *kept = me > ms && (!clipped || me - ms >= 4u);
+}
+__device__ u32 zb_ldm_overlay(const u64* __restrict__ P, u32 nP, const u64* __restrict__ L, u32 nL, u32* __restrict__ kp, u64* __restrict__ out,
+                              u32* wsum, u32* sEnd, u32& carry)
+{
+    u32 const tid = threadIdx.x;
+    u32 base = 0;
+    for (u32 i0 = 0; i0 < nP; i0 += MERGE_THREADS) {              /* kp[i] = kept parse matches before i */
+        u32 const i = i0 + tid;
+        u32 ms2, me2, nx; bool kept = false;
+        if (i < nP) { u64 const r = P[i]; zb_ldm_clip(ZB_RAW_MS(r), ZB_RAW_MS(r) + ZB_RAW_MLEN(r), L, nL, &ms2, &me2, &nx, &kept); }
+        u32 t;
+        u32 const before = zb_block_excl(kept, wsum, &t);
+        if (i < nP) kp[i] = base + before;
+        base += t;
+    }
+    if (tid == 0) kp[nP] = base;
+    __syncthreads();
+    for (u32 i = tid; i < nP; i += MERGE_THREADS) {               /* parse matches and LDM matches to their places, absolute */
+        u64 const r = P[i];
+        u32 ms2, me2, nx; bool kept;
+        zb_ldm_clip(ZB_RAW_MS(r), ZB_RAW_MS(r) + ZB_RAW_MLEN(r), L, nL, &ms2, &me2, &nx, &kept);
+        if (kept) out[kp[i] + nx] = zb_pack_ldm(ms2, me2 - ms2, ZB_RAW_OFF(r));
+    }
+    for (u32 k = tid; k < nL; k += MERGE_THREADS) {               /* kept parse matches before it = those that start before it */
+        u32 const s = ZB_LDM_START(L[k]);
+        u32 lo = 0, hi = nP;
+        while (lo < hi) { u32 const mid = (lo + hi) >> 1; if (ZB_RAW_MS(P[mid]) < s) lo = mid + 1u; else hi = mid; }
+        out[k + kp[lo]] = L[k];
+    }
+    u32 const n = base + nL;
+    __syncthreads();
+    if (tid == 0) carry = 0;
+    for (u32 o0 = 0; o0 < n; o0 += MERGE_THREADS) {               /* absolute -> (offset, litLength, matchLength) */
+        u32 const o = o0 + tid;
+        u64 const m = o < n ? out[o] : 0ull;
+        sEnd[tid] = ZB_LDM_START(m) + ZB_LDM_LEN(m);
+        __syncthreads();
+        u32 const prevEnd = tid ? sEnd[tid - 1u] : carry;
+        if (o < n) out[o] = zb_pack_seq(ZB_LDM_OFF(m), ZB_LDM_START(m) - prevEnd, ZB_LDM_LEN(m));
+        __syncthreads();
+        if (tid == MERGE_THREADS - 1u) carry = sEnd[tid];
+        __syncthreads();
+    }
+    return n;
+}
+
+/* LDM: the variant that lays the block's long-distance matches over the parse output (ldm: rows of this launch; farScratch /
+ * distScratch: the candidate arrays, dead once the parse is done).  Without LDM the instruction stream is the kernel's own. */
+template <bool LDM>
 __global__ void __launch_bounds__(MERGE_THREADS, MERGE_MIN_CTAS)
 zb_merge_segments_kernel(const u8* __restrict__ src, const ZbBlock* __restrict__ blocks, ZbParams prm, ZbStrides sd, const ZbSegMeta* __restrict__ segmeta,
-                         u64* __restrict__ seqs, u8* __restrict__ lits, ZbBlockMeta* __restrict__ meta)
+                         u64* __restrict__ seqs, u8* __restrict__ lits, ZbBlockMeta* __restrict__ meta,
+                         ZbLdmView ldm, u32* __restrict__ farScratch, u16* __restrict__ distScratch)
 {
     __shared__ u32 sPos[MERGE_TILE], sLit[MERGE_TILE], sLen[MERGE_TILE], sOff[MERGE_TILE];
     __shared__ u32 wsumL[MERGE_THREADS / 32], wsumA[MERGE_THREADS / 32], wmaxU[MERGE_THREADS / 32], wmaxK[MERGE_THREADS / 32];
@@ -681,6 +761,25 @@ zb_merge_segments_kernel(const u8* __restrict__ src, const ZbBlock* __restrict__
         if (lane == 0u) gTotal = total;
     }
     __syncthreads();
+    u32 nbSeq;
+    if constexpr (LDM) {
+        /* ---- 2'. survivors (raw) to the scratch, then the overlay writes the triples ---- */
+        u64* const P = reinterpret_cast<u64*>(farScratch + (size_t)b * sd.dist);
+#pragma unroll 1
+        for (u32 k = 0; k < segs; k++) {
+            u32 const f = gFirst[k], cnt = gCnt[k];
+            const u64* const sfrom = myseq + (size_t)k * SEG_SLOTS + f;
+            for (u32 i = tid; i < cnt; i += MERGE_THREADS) {
+                u64 r = sfrom[i];
+                if (i == 0u) r = zb_pack_raw(ZB_RAW_OFF(r), gPl[k], gPm[k]);
+                P[gBase[k] + i] = r;
+            }
+        }
+        __syncthreads();
+        nbSeq = zb_ldm_overlay(P, gTotal, ldm.match + ldm.first[b], ldm.cnt[b], reinterpret_cast<u32*>(distScratch + (size_t)b * sd.dist), myseq,
+                               wsumA, sPos, carryEnd);
+        __syncthreads();
+    } else {
     /* ---- 2. survivors move down to be contiguous (in place: a destination never lies above its source) and become
      *         (offset, litLength, matchLength) ---- */
 #pragma unroll 1
@@ -703,7 +802,8 @@ zb_merge_segments_kernel(const u8* __restrict__ src, const ZbBlock* __restrict__
             __syncthreads();
         }
     }
-    u32 const nbSeq = gTotal;
+    nbSeq = gTotal;
+    }
     zb_merge_codes(prm.codeRep[0], prm.codeRep[1], prm.codeRep[2], (bd.flags & ZB_FLAG_FIRST) != 0u, myseq, mylit, in, nbSeq, bd.size, meta + b,
                    sPos, sLit, sLen, sOff, sR2, sRep, wsumL, wsumA, wmaxU, wmaxK, baseL, baseA);
 }
@@ -814,7 +914,7 @@ extern "C" cudaError_t zb_launch_dict_image(const u8* d_dictEnd, const ZbChunk* 
 extern "C" cudaError_t zb_launch_match(const u8* d_src, const u8* d_dictEnd, const u32* d_image, const ZbBlock* d_blocks, u32 nbBlocks,
                                        const ZbChunk* d_chunks, u32 nbChunks, u32 slotFirstBlock, const ZbParams* prm, const ZbStrides* sdp,
                                        u16* d_dist, u32* d_far, u16* d_dist2, u32* d_far2, u64* d_seqs, u8* d_lits, ZbBlockMeta* d_meta, ZbSegMeta* d_segmeta,
-                                       cudaEvent_t evMid, cudaStream_t stream)
+                                       cudaEvent_t evMid, cudaStream_t stream, const ZbLdmView* ldm)
 {
     if (nbBlocks == 0) return cudaSuccess;
     ZbStrides const sd = *sdp;
@@ -836,7 +936,9 @@ extern "C" cudaError_t zb_launch_match(const u8* d_src, const u8* d_dictEnd, con
     }
     if (segs == 1u && sd.dist <= 8192u)
         zb_merge_small_kernel<<<(nbBlocks + MERGE_THREADS / 32u - 1u) / (MERGE_THREADS / 32u), MERGE_THREADS, 0, stream>>>(d_src, d_blocks, nbBlocks, *prm, sd, d_segmeta, d_seqs, d_lits, d_meta);
+    else if (ldm)
+        zb_merge_segments_kernel<true><<<nbBlocks, MERGE_THREADS, 0, stream>>>(d_src, d_blocks, *prm, sd, d_segmeta, d_seqs, d_lits, d_meta, *ldm, d_far, d_dist);
     else
-        zb_merge_segments_kernel<<<nbBlocks, MERGE_THREADS, 0, stream>>>(d_src, d_blocks, *prm, sd, d_segmeta, d_seqs, d_lits, d_meta);
+        zb_merge_segments_kernel<false><<<nbBlocks, MERGE_THREADS, 0, stream>>>(d_src, d_blocks, *prm, sd, d_segmeta, d_seqs, d_lits, d_meta, ZbLdmView(), nullptr, nullptr);
     return cudaGetLastError();
 }

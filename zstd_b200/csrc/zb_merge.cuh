@@ -41,10 +41,10 @@ __device__ __forceinline__ void zb_merge_codes(u32 rep0, u32 rep1, u32 rep2, boo
         for (u32 j = 0; j < MERGE_PER; j++) {
             u32 const i = tid * MERGE_PER + j;
             u64 const q = (i < n) ? myseq[t0 + i] : 0ull;
-            ll[j] = (u32)((q >> 24) & 0x3FFFFu);
-            ml[j] = (u32)(q >> 42);
+            ll[j] = ZB_SEQ_LL(q);
+            ml[j] = ZB_SEQ_ML(q);
             adv[j] = ll[j] + ml[j];
-            off[j] = (u32)q & 0xFFFFFFu;
+            off[j] = ZB_SEQ_OFFBASE(q);
             if (i < n) sOff[i] = off[j];
             myL += ll[j]; myA += adv[j];
         }

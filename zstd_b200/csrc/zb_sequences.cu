@@ -73,9 +73,9 @@ struct ZbdSeq { u32 offBase, litLen, mlBase, llc, ofc, mlc, llBits, mlBits; };
 __device__ __forceinline__ ZbdSeq zbd_unpack(u64 q, const ZbdCodeLut& lut)
 {
     ZbdSeq s;
-    s.offBase = (u32)(q & 0xFFFFFFu);
-    s.litLen = (u32)((q >> 24) & 0x3FFFFu);
-    s.mlBase = (u32)((q >> 42) & 0x3FFFFu) - 3u;
+    s.offBase = ZB_SEQ_OFFBASE(q);
+    s.litLen = ZB_SEQ_LL(q);
+    s.mlBase = ZB_SEQ_ML(q) - 3u;
     u32 const le = lut.ll[s.litLen < 63u ? s.litLen : 63u], lh = zb_hb32(s.litLen | 1u);
     u32 const me = lut.ml[s.mlBase < 127u ? s.mlBase : 127u], mh = zb_hb32(s.mlBase | 1u);
     bool const lBig = s.litLen > 63u, mBig = s.mlBase > 127u;

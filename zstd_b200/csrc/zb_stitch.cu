@@ -187,15 +187,7 @@ extern "C" cudaError_t zb_launch_stitch(const u8* d_src, const ZbBlock* d_blocks
  * the reference computes it chunk by chunk on the host, zstd_compress.c:4544, :5297-5303).
  * XXH64 is four serial accumulator chains per input (acc = rotl(acc + x * P2, 31) * P1 over the 8-byte words of
  * every 32-byte stripe): nothing to split inside one frame, so one warp takes a frame — all lanes load 256 bytes,
- * lanes 0..3 run the chains — and the frames of a call are hashed side by side. */
-__device__ __forceinline__ u64 zbx_rotl(u64 x, int r) { return (x << r) | (x >> (64 - r)); }
-#define ZBX_P1 0x9E3779B185EBCA87ull
-#define ZBX_P2 0xC2B2AE3D27D4EB4Full
-#define ZBX_P3 0x165667B19E3779F9ull
-#define ZBX_P4 0x85EBCA77C2B2AE63ull
-#define ZBX_P5 0x27D4EB2F165667C5ull
-__device__ __forceinline__ u64 zbx_round(u64 acc, u64 in) { return zbx_rotl(acc + in * ZBX_P2, 31) * ZBX_P1; }
-__device__ __forceinline__ u64 zbx_merge(u64 h, u64 v) { return (h ^ zbx_round(0, v)) * ZBX_P1 + ZBX_P4; }
+ * lanes 0..3 run the chains — and the frames of a call are hashed side by side.  The rounds are in zb_device.cuh. */
 
 #define XXH_WARPS 4
 __global__ void __launch_bounds__(32 * XXH_WARPS)
