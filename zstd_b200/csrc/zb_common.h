@@ -222,6 +222,49 @@ static inline bool zb_isErr(size_t c) { return c > ZB_ERR(ZB_error_maxCode); }
 #define CK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { \
     if (getenv("ZSTDB200_DEBUG")) fprintf(stderr, "zstd_b200: CUDA error %s at %s:%d\n", cudaGetErrorString(e_), __FILE__, __LINE__); \
     cudaGetLastError(); return ZB_ERR(e_ == cudaErrorMemoryAllocation ? ZB_error_memory_allocation : ZB_error_GENERIC); } } while (0)
+/* a call that returns an error code passes it on */
+#define TRY(x) do { size_t const e_ = (x); if (zb_isErr(e_)) return e_; } while (0)
+
+/* An array of T in device memory (cudaMalloc) or page-locked host memory (cudaMallocHost) that a context owns: grown on
+ * demand, freed with the context.  cap counts elements. */
+template <typename T, bool Pinned> struct ZbBuf {
+    T* p = nullptr; size_t cap = 0;
+    ZbBuf() = default;
+    ZbBuf(const ZbBuf&) = delete; ZbBuf& operator=(const ZbBuf&) = delete;
+    ~ZbBuf() { release(); }
+    void release() { if (p) { if (Pinned) cudaFreeHost(p); else cudaFree(p); } p = nullptr; cap = 0; }
+    /* room for `need` elements; a larger need frees the array (its contents are not kept), then allocates need + headroom */
+    size_t ensure(size_t need, size_t headroom = 0) {
+        if (need <= cap) return 0;
+        release();
+        size_t const bytes = (need + headroom) * sizeof(T);
+        CK(Pinned ? cudaMallocHost((void**)&p, bytes) : cudaMalloc((void**)&p, bytes));
+        cap = need + headroom;
+        return 0;
+    }
+    operator T*() const { return p; }
+};
+template <typename T> using ZbDevBuf = ZbBuf<T, false>;
+template <typename T> using ZbHostBuf = ZbBuf<T, true>;
+
+/* a context's stream and events */
+static inline void zb_streamDestroy(cudaStream_t st, const cudaEvent_t* ev, int nbEvents)
+{
+    for (int i = 0; i < nbEvents; i++) if (ev[i]) cudaEventDestroy(ev[i]);
+    if (st) cudaStreamDestroy(st);
+}
+/* creates a non-blocking stream and nbEvents events on `dev`, all or nothing: after a failure none of them is left */
+static inline size_t zb_streamCreate(int dev, cudaStream_t* st, cudaEvent_t* ev, int nbEvents)
+{
+    CK(cudaSetDevice(dev));
+    *st = nullptr;
+    for (int i = 0; i < nbEvents; i++) ev[i] = nullptr;
+    cudaError_t e = cudaStreamCreateWithFlags(st, cudaStreamNonBlocking);
+    for (int i = 0; i < nbEvents && e == cudaSuccess; i++) e = cudaEventCreate(&ev[i]);
+    if (e != cudaSuccess) zb_streamDestroy(*st, ev, nbEvents);
+    CK(e);
+    return 0;
+}
 
 /* restores the calling thread's current device when a call returns (a context works on the device it was created for) */
 struct ZbDeviceGuard {

@@ -492,17 +492,18 @@ zbd_matches_kernel(const ZbdBlock* __restrict__ blocks, const ZbdFrame* __restri
 struct ZSTD_DCtx_s {
     int device, bindDevice;
     cudaStream_t stream;
-    ZbdBlock* d_blocks; ZbdFrame* d_frames; ZbdBlockOut* d_bout; size_t capBlocks, capFrames;
-    u8* d_lits; size_t capLits; u64* d_seqs; size_t capSeqs; u64* d_matchPos; size_t capMatchPos;
-    u32* d_tileFirst; size_t capTiles; u8* d_done; size_t capDone;
-    u8* d_in; size_t capIn; u8* d_out; size_t capOut;
-    u64* d_res; u32* d_execErr;
-    u64* h_res;                  /* pinned: walker / scan results */
+    ZbDevBuf<ZbdBlock> d_blocks; ZbDevBuf<ZbdFrame> d_frames;
+    ZbDevBuf<ZbdBlockOut> d_bout;  /* one more than d_blocks */
+    ZbDevBuf<u8> d_lits; ZbDevBuf<u64> d_seqs, d_matchPos;
+    ZbDevBuf<u32> d_tileFirst; ZbDevBuf<u8> d_done;
+    ZbDevBuf<u8> d_in, d_out;
+    ZbDevBuf<u64> d_res; u32* d_execErr;   /* walker / scan results; d_execErr lies in d_res[9] */
+    ZbHostBuf<u64> h_res;          /* their mirror */
     /* streaming front end (ZSTD_decompressStream): compressed bytes collected until a frame is complete, output waiting to be handed out */
-    std::vector<u8>* dsIn; std::vector<u8>* dsOut; size_t dsOutPos;
+    std::vector<u8> dsIn, dsOut; size_t dsOutPos;
     size_t hostWalkMax;          /* ZBD_HOSTWALK_MAX, or ZSTDB200_HOSTWALK_MAX from the environment (tests: 0 forces the kernel walk) */
-    u8* h_stage; size_t capStage; /* page-locked copy of a device-resident input's compressed bytes, for the header walk */
-    u8* d_dict; size_t capDict;  /* the call's dictionary, whole (header + content) */
+    ZbHostBuf<u8> h_stage;       /* copy of a device-resident input's compressed bytes, for the header walk */
+    ZbDevBuf<u8> d_dict;         /* the call's dictionary, whole (header + content) */
     ZbdDictInfo di; size_t dictSize;
     cudaEvent_t ev[7];
     ZSTDB200_dstats stats;
@@ -519,7 +520,7 @@ struct ZbdCall {
 
 extern "C" ZSTD_DCtx* ZSTD_createDCtx(void)                          /* lib/zstd.h:289 */
 {
-    ZSTD_DCtx* d = (ZSTD_DCtx*)calloc(1, sizeof(ZSTD_DCtx));
+    ZSTD_DCtx* d = new (std::nothrow) ZSTD_DCtx();                  /* value-initialised: every plain member is zero */
     if (!d) return NULL;
     d->device = -1;
     {   const char* const e = getenv("ZSTDB200_HOSTWALK_MAX"); d->hostWalkMax = e ? (size_t)strtoull(e, NULL, 10) : ZBD_HOSTWALK_MAX; }
@@ -529,52 +530,29 @@ extern "C" ZSTD_DCtx* ZSTD_createDCtx(void)                          /* lib/zstd
 extern "C" size_t ZSTD_freeDCtx(ZSTD_DCtx* d)                        /* accepts NULL, lib/zstd.h:290 */
 {
     if (!d) return 0;
-    if (d->device >= 0) {
-        ZbDeviceGuard guard;
-        cudaSetDevice(d->device);
-        cudaFree(d->d_blocks); cudaFree(d->d_frames); cudaFree(d->d_bout); cudaFree(d->d_lits); cudaFree(d->d_seqs); cudaFree(d->d_matchPos); cudaFree(d->d_tileFirst); cudaFree(d->d_done);
-        cudaFree(d->d_in); cudaFree(d->d_out); cudaFree(d->d_res); cudaFreeHost(d->h_res); cudaFree(d->d_dict); cudaFreeHost(d->h_stage);
-        for (int i = 0; i < 7; i++) cudaEventDestroy(d->ev[i]);
-        cudaStreamDestroy(d->stream);
-    }
-    delete d->dsIn; delete d->dsOut;
-    free(d);
+    if (d->device < 0) { delete d; return 0; }                       /* never reached a device: it holds nothing there */
+    ZbDeviceGuard guard;
+    cudaSetDevice(d->device);
+    zb_streamDestroy(d->stream, d->ev, 7);
+    delete d;                                                        /* its buffers free themselves, on its device */
     return 0;
 }
 static size_t zbd_ctxInit(ZSTD_DCtx* d)
 {
-    if (d->device >= 0) { CK(cudaSetDevice(d->device)); return 0; }
-    int n = 0;
-    if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) { cudaGetLastError(); return ZB_ERR(ZB_error_GENERIC); }
-    int const dev = d->bindDevice < 0 ? 0 : d->bindDevice;
-    CK(cudaSetDevice(dev));
-    /* everything or nothing: a partial failure leaves the context uninitialised (device stays -1) */
-    cudaStream_t st = nullptr; cudaEvent_t ev[7] = {}; u64* d_res = nullptr; u64* h_res = nullptr;
-    cudaError_t e = cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking);
-    for (int i = 0; i < 7 && e == cudaSuccess; i++) e = cudaEventCreate(&ev[i]);
-    if (e == cudaSuccess) e = cudaMalloc(&d_res, 16 * sizeof(u64));
-    if (e == cudaSuccess) e = cudaMallocHost(&h_res, 16 * sizeof(u64));
-    if (e != cudaSuccess) {
-        for (int i = 0; i < 7; i++) if (ev[i]) cudaEventDestroy(ev[i]);
-        if (st) cudaStreamDestroy(st);
-        cudaFree(d_res);
-        cudaGetLastError();
-        return ZB_ERR(e == cudaErrorMemoryAllocation ? ZB_error_memory_allocation : ZB_error_GENERIC);
+    if (d->device >= 0) CK(cudaSetDevice(d->device));
+    else {
+        int n = 0;
+        if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) { cudaGetLastError(); return ZB_ERR(ZB_error_GENERIC); }
+        int const dev = d->bindDevice < 0 ? 0 : d->bindDevice;
+        TRY(zb_streamCreate(dev, &d->stream, d->ev, 7));
+        d->device = dev;
     }
-    d->stream = st; memcpy(d->ev, ev, sizeof(ev));
-    d->d_res = d_res; d->h_res = h_res; d->d_execErr = (u32*)(d_res + 9);
-    d->device = dev;
+    TRY(d->d_res.ensure(16)); TRY(d->h_res.ensure(16));
+    d->d_execErr = (u32*)(d->d_res + 9);
     return 0;
 }
-template <typename T> static size_t zbd_grow(T** p, size_t* cap, size_t need)
-{
-    if (need <= *cap) return 0;
-    cudaFree(*p); *p = NULL; *cap = 0;
-    size_t const n = need + need / 8 + 64;
-    CK(cudaMalloc(p, n * sizeof(T)));
-    *cap = n;
-    return 0;
-}
+/* the decoder's arrays are allocated with slack (an eighth more, and 64): calls of similar sizes reuse them */
+template <typename T> static size_t zbd_reserve(ZbDevBuf<T>& b, size_t need) { return b.ensure(need, need / 8 + 64); }
 
 /* D1 .. D4 over descriptors that are already on the device; returns the output size */
 static size_t zbd_run(ZSTD_DCtx* d, u8* d_dst, size_t dstCapacity, const u8* d_src, u32 nb, u32 nf, u64 seqCount, cudaStream_t st)
@@ -594,8 +572,8 @@ static size_t zbd_run(ZSTD_DCtx* d, u8* d_dst, size_t dstCapacity, const u8* d_s
     CK(cudaEventRecord(d->ev[4], st));
     u32 const dictContent = d->dictSize ? (u32)(d->dictSize - d->di.contentOff) : 0u;
     const u8* const d_dictContent = d->dictSize ? d->d_dict + d->di.contentOff : (const u8*)NULL;
-    {   size_t const r = zbd_grow(&d->d_tileFirst, &d->capTiles, (total >> ZBD_TILE_LOG) + 4); if (zb_isErr(r)) return r; }
-    {   size_t const r = zbd_grow(&d->d_done, &d->capDone, (size_t)seqCount + 4); if (zb_isErr(r)) return r; }
+    TRY(zbd_reserve(d->d_tileFirst, (total >> ZBD_TILE_LOG) + 4));
+    TRY(zbd_reserve(d->d_done, (size_t)seqCount + 4));
     CK(cudaMemsetAsync(d->d_tileFirst, 0xFF, ((total >> ZBD_TILE_LOG) + 4) * sizeof(u32), st));
     CK(cudaMemsetAsync(d->d_done, 0, (size_t)seqCount + 4, st));
     zbd_place_kernel<<<grid, 32 * ZBD_WARPS, 0, st>>>(d_src, d->d_blocks, nb, d->d_lits, d->d_seqs, d->d_matchPos, d->d_tileFirst, d->d_bout, d_dst,
@@ -624,16 +602,12 @@ static size_t zbd_run(ZSTD_DCtx* d, u8* d_dst, size_t dstCapacity, const u8* d_s
 
 static size_t zbd_ensure(ZSTD_DCtx* d, u32 nb, u32 nf, u64 litBytes, u64 seqCount)
 {
-    if (nb > d->capBlocks) {
-        cudaFree(d->d_blocks); cudaFree(d->d_bout); d->d_blocks = NULL; d->d_bout = NULL; d->capBlocks = 0;
-        size_t const n = (size_t)nb + nb / 8 + 64;
-        CK(cudaMalloc(&d->d_blocks, n * sizeof(ZbdBlock))); CK(cudaMalloc(&d->d_bout, (n + 1) * sizeof(ZbdBlockOut)));
-        d->capBlocks = n;
-    }
-    {   size_t const e = zbd_grow(&d->d_frames, &d->capFrames, (size_t)nf); if (zb_isErr(e)) return e; }
-    {   size_t const e = zbd_grow(&d->d_lits, &d->capLits, (size_t)litBytes + 16); if (zb_isErr(e)) return e; }
-    {   size_t const e = zbd_grow(&d->d_seqs, &d->capSeqs, (size_t)seqCount + 1); if (zb_isErr(e)) return e; }
-    {   size_t const e = zbd_grow(&d->d_matchPos, &d->capMatchPos, (size_t)seqCount + 1); if (zb_isErr(e)) return e; }
+    TRY(zbd_reserve(d->d_blocks, nb));
+    TRY(d->d_bout.ensure((size_t)nb + 1, nb / 8 + 64));
+    TRY(zbd_reserve(d->d_frames, nf));
+    TRY(zbd_reserve(d->d_lits, (size_t)litBytes + 16));
+    TRY(zbd_reserve(d->d_seqs, (size_t)seqCount + 1));
+    TRY(zbd_reserve(d->d_matchPos, (size_t)seqCount + 1));
     return 0;
 }
 
@@ -646,7 +620,7 @@ static size_t zbd_setDict(ZSTD_DCtx* d, const void* dict, size_t dictSize, cudaS
     if (!dict || dictSize == 0) return 0;
     u32 const e = zbd_parseDict(&d->di, (const u8*)dict, dictSize);
     if (e) return ZB_ERR(e);
-    {   size_t const r = zbd_grow(&d->d_dict, &d->capDict, dictSize + 16); if (zb_isErr(r)) return r; }
+    TRY(zbd_reserve(d->d_dict, dictSize + 16));
     CK(cudaMemcpyAsync(d->d_dict, dict, dictSize, cudaMemcpyHostToDevice, st));
     CK(cudaStreamSynchronize(st));                                    /* the caller's dictionary buffer is pageable memory that may change after the call */
     d->dictSize = dictSize;
@@ -675,19 +649,14 @@ static size_t zbd_decompress(ZSTD_DCtx* d, const ZbdCall& c)
     if (!c.deviceMemory && !c.src) return ZB_ERR(ZB_error_srcSize_wrong);
     if (!c.deviceMemory && c.dstCapacity && !c.dst) return ZB_ERR(ZB_error_dstBuffer_null);
     ZbDeviceGuard guard;
-    {   size_t const e = zbd_ctxInit(d); if (zb_isErr(e)) return e; }
+    TRY(zbd_ctxInit(d));
     memset(&d->stats, 0, sizeof(d->stats));
     cudaStream_t const st = c.stream ? c.stream : d->stream;
-    {   size_t const e = zbd_setDict(d, c.dict, c.dictSize, st); if (zb_isErr(e)) return e; }
+    TRY(zbd_setDict(d, c.dict, c.dictSize, st));
     /* D0: block and frame descriptors */
     const u8* hostIn = c.deviceMemory ? NULL : (const u8*)c.src;
     if (c.deviceMemory && c.srcSize <= d->hostWalkMax) {
-        if (c.srcSize > d->capStage) {
-            cudaFreeHost(d->h_stage); d->h_stage = NULL; d->capStage = 0;
-            size_t const n = c.srcSize + c.srcSize / 4 + 4096;
-            CK(cudaMallocHost(&d->h_stage, n));
-            d->capStage = n;
-        }
+        TRY(d->h_stage.ensure(c.srcSize, c.srcSize / 4 + 4096));
         CK(cudaMemcpyAsync(d->h_stage, c.src, c.srcSize, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
         hostIn = d->h_stage;
@@ -698,12 +667,12 @@ static size_t zbd_decompress(ZSTD_DCtx* d, const ZbdCall& c)
     else {                                                            /* the walk kernel; once more if the arrays were too small */
         u32 capB = (u32)(c.srcSize / 4096u) + 1024u, capF = 1024u;
         for (int attempt = 0; attempt < 2; attempt++) {
-            {   size_t const r = zbd_ensure(d, capB, capF, 0, 0); if (zb_isErr(r)) return r; }
-            zbd_walk_kernel<<<1, 32, 0, st>>>((const u8*)c.src, (u64)c.srcSize, d->d_blocks, (u32)d->capBlocks, d->d_frames, (u32)d->capFrames, d->d_res, d->di.entropy, d->di.dictID);
+            TRY(zbd_ensure(d, capB, capF, 0, 0));
+            zbd_walk_kernel<<<1, 32, 0, st>>>((const u8*)c.src, (u64)c.srcSize, d->d_blocks, (u32)d->d_blocks.cap, d->d_frames, (u32)d->d_frames.cap, d->d_res, d->di.entropy, d->di.dictID);
             CK(cudaMemcpyAsync(d->h_res, d->d_res, 5 * sizeof(u64), cudaMemcpyDeviceToHost, st));
             CK(cudaStreamSynchronize(st));
             if (d->h_res[0]) return ZB_ERR((u32)d->h_res[0]);
-            if (d->h_res[1] <= d->capBlocks && d->h_res[2] <= d->capFrames) break;
+            if (d->h_res[1] <= d->d_blocks.cap && d->h_res[2] <= d->d_frames.cap) break;
             capB = (u32)d->h_res[1]; capF = (u32)d->h_res[2];
             if (attempt == 1) return ZB_ERR(ZB_error_GENERIC);
         }
@@ -717,13 +686,13 @@ static size_t zbd_decompress(ZSTD_DCtx* d, const ZbdCall& c)
         if (allKnown && known > c.dstCapacity) return ZB_ERR(ZB_error_dstSize_tooSmall);      /* refused before any upload */
         /* the output can not be larger than the blocks' maximum sizes */
         outCap = allKnown ? (size_t)known : (c.dstCapacity < (size_t)nb * ZB_BLOCK_MAX ? c.dstCapacity : (size_t)nb * ZB_BLOCK_MAX);
-        {   size_t const r = zbd_grow(&d->d_in, &d->capIn, c.srcSize + 16); if (zb_isErr(r)) return r; }
-        {   size_t const r = zbd_grow(&d->d_out, &d->capOut, outCap + 16); if (zb_isErr(r)) return r; }
+        TRY(zbd_reserve(d->d_in, c.srcSize + 16));
+        TRY(zbd_reserve(d->d_out, outCap + 16));
         CK(cudaEventRecord(d->ev[0], st));
         CK(cudaMemcpyAsync(d->d_in, c.src, c.srcSize, cudaMemcpyHostToDevice, st));
         runSrc = d->d_in; runDst = d->d_out;
     }
-    {   size_t const r = zbd_ensure(d, nb, nf, lit, seq); if (zb_isErr(r)) return r; }
+    TRY(zbd_ensure(d, nb, nf, lit, seq));                            /* the walk kernel's descriptors fit: d_blocks and d_frames keep them */
     if (hostIn) {
         CK(cudaMemcpyAsync(d->d_blocks, B.data(), (size_t)nb * sizeof(ZbdBlock), cudaMemcpyHostToDevice, st));
         CK(cudaMemcpyAsync(d->d_frames, F.data(), (size_t)nf * sizeof(ZbdFrame), cudaMemcpyHostToDevice, st));
@@ -840,8 +809,7 @@ extern "C" size_t ZSTD_freeDStream(ZSTD_DStream* zds) { return ZSTD_freeDCtx(zds
 extern "C" size_t ZSTD_initDStream(ZSTD_DStream* zds)
 {
     if (!zds) return ZB_ERR(ZB_error_GENERIC);
-    if (zds->dsIn) zds->dsIn->clear();
-    if (zds->dsOut) zds->dsOut->clear();
+    zds->dsIn.clear(); zds->dsOut.clear();
     zds->dsOutPos = 0;
     return 5;                                                          /* a frame header's first bytes, as the reference suggests (ZSTD_startingInputLength) */
 }
@@ -852,36 +820,35 @@ extern "C" size_t ZSTD_decompressStream(ZSTD_DStream* d, ZSTD_outBuffer* out, ZS
     if (!d || !out || !in) return ZB_ERR(ZB_error_GENERIC);
     if (out->pos > out->size) return ZB_ERR(ZB_error_dstSize_tooSmall);
     if (in->pos > in->size) return ZB_ERR(ZB_error_srcSize_wrong);
-    if (!d->dsIn) { d->dsIn = new (std::nothrow) std::vector<u8>(); d->dsOut = new (std::nothrow) std::vector<u8>(); if (!d->dsIn || !d->dsOut) return ZB_ERR(ZB_error_memory_allocation); }
     auto handOut = [&]() -> size_t {
-        size_t const have = d->dsOut->size() - d->dsOutPos, room = out->size - out->pos, n = have < room ? have : room;
-        if (n) { memcpy((u8*)out->dst + out->pos, d->dsOut->data() + d->dsOutPos, n); out->pos += n; d->dsOutPos += n; }
-        if (d->dsOutPos == d->dsOut->size()) { d->dsOut->clear(); d->dsOutPos = 0; }
-        return d->dsOut->size() - d->dsOutPos;
+        size_t const have = d->dsOut.size() - d->dsOutPos, room = out->size - out->pos, n = have < room ? have : room;
+        if (n) { memcpy((u8*)out->dst + out->pos, d->dsOut.data() + d->dsOutPos, n); out->pos += n; d->dsOutPos += n; }
+        if (d->dsOutPos == d->dsOut.size()) { d->dsOut.clear(); d->dsOutPos = 0; }
+        return d->dsOut.size() - d->dsOutPos;
     };
-    if (handOut() != 0) return d->dsOut->size() - d->dsOutPos;           /* room first: input is only taken while nothing is waiting */
-    d->dsIn->insert(d->dsIn->end(), (const u8*)in->src + in->pos, (const u8*)in->src + in->size);
+    if (handOut() != 0) return d->dsOut.size() - d->dsOutPos;            /* room first: input is only taken while nothing is waiting */
+    d->dsIn.insert(d->dsIn.end(), (const u8*)in->src + in->pos, (const u8*)in->src + in->size);
     in->pos = in->size;
     bool decoded = false;
-    while (!d->dsIn->empty()) {
-        size_t const fs = ZSTD_findFrameCompressedSize(d->dsIn->data(), d->dsIn->size());
+    while (!d->dsIn.empty()) {
+        size_t const fs = ZSTD_findFrameCompressedSize(d->dsIn.data(), d->dsIn.size());
         if (ZSTD_isError(fs)) {
             if (ZSTD_getErrorCode(fs) == ZB_error_srcSize_wrong) break;   /* the frame is not complete yet */
             return fs;
         }
-        size_t const bound = zbd_frameOutputBound(d->dsIn->data(), fs);
-        size_t const base = d->dsOut->size();
-        try { d->dsOut->resize(base + bound + 1); }
+        size_t const bound = zbd_frameOutputBound(d->dsIn.data(), fs);
+        size_t const base = d->dsOut.size();
+        try { d->dsOut.resize(base + bound + 1); }
         catch (const std::exception&) { return ZB_ERR(ZB_error_memory_allocation); }     /* no C++ exception may cross the C ABI */
-        size_t const r = ZSTD_decompressDCtx(d, d->dsOut->data() + base, bound, d->dsIn->data(), fs);
-        if (ZSTD_isError(r)) { d->dsOut->resize(base); return r; }
-        d->dsOut->resize(base + r);
-        d->dsIn->erase(d->dsIn->begin(), d->dsIn->begin() + (ptrdiff_t)fs);
+        size_t const r = ZSTD_decompressDCtx(d, d->dsOut.data() + base, bound, d->dsIn.data(), fs);
+        if (ZSTD_isError(r)) { d->dsOut.resize(base); return r; }
+        d->dsOut.resize(base + r);
+        d->dsIn.erase(d->dsIn.begin(), d->dsIn.begin() + (ptrdiff_t)fs);
         decoded = true;
     }
     size_t const waiting = handOut();
     if (waiting) return waiting;
     (void)decoded;
-    if (d->dsIn->empty()) return 0;                                      /* at a frame border with everything handed out */
+    if (d->dsIn.empty()) return 0;                                       /* at a frame border with everything handed out */
     return ZB_BLOCK_MAX + 3;                                             /* in the middle of a frame: more input, please */
 }
