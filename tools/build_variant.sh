@@ -14,7 +14,7 @@ mkdir -p ../variants /tmp/zbv_$name
 declare -A flags
 for spec in "$@"; do f=${spec%%:*}; fl=""; [[ "$spec" == *:* ]] && fl=${spec#*:}; flags[$f]="x$fl"; done
 objs=""
-for f in zb_api zb_dict zb_match zb_literals zb_sequences zb_stitch zb_decode; do
+for f in zb_api zb_dict zb_match zb_ldm zb_seqimport zb_literals zb_sequences zb_stitch zb_decode; do
   if [ -n "${flags[$f.cu]}" ]; then
     nvcc -O3 -std=c++17 -lineinfo -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC,-fvisibility=hidden -Xptxas -v ${flags[$f.cu]#x} -c $f.cu -o /tmp/zbv_$name/$f.o 2> /tmp/zbv_$name/$f.log
     grep "spill" /tmp/zbv_$name/$f.log | grep -v " 0 bytes spill stores, 0 bytes spill loads" | head -4 || true

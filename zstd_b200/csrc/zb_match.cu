@@ -22,10 +22,6 @@
 #include "zb_kernels.h"
 #include "zb_merge.cuh"
 
-#ifndef WALK_FAST_BC
-#define WALK_FAST_BC 1           /* development switch: 0 = entries and the second look through zb_walk_entry / zb_walk_cand */
-#endif
-
 /* matched bytes starting at rel positions (a, a - offset), never reading at or past `be` */
 template <bool DICT>
 __device__ __forceinline__ u32 zb_count_fwd(const ZbSeg& sg, u32 a, u32 offset, u32 be, u32 lane)
@@ -79,14 +75,14 @@ __device__ __forceinline__ u64 zb_pack_raw(u32 off, u32 mlen, u32 msRel) { retur
  * reversed: of all insertions of one batch into a bucket the LOWEST position has the largest key, and every batch beats
  * the batches before it — so one shared-memory atomicMax per insertion arbitrates a batch, whatever the thread order. */
 #define ZB_TAG_MASK ((1u << ZB_TAG_BITS) - 1u)
-__device__ __forceinline__ u32 zb_walk_key(u32 x) { return (x | (ZB_BATCH - 1u)) - (x & (ZB_BATCH - 1u)); }   /* its own inverse */
-__device__ __forceinline__ u32 zb_walk_entry(u32 h, u32 x) { return ((zb_walk_key(x) + 1u) << ZB_TAG_BITS) | (h & ZB_TAG_MASK); }
-/* candidate distance of the position at walk coordinate x given a bucket's content c (0 = no candidate).
- * An empty bucket (c = 0) decodes to a coordinate far above x. */
-__device__ __forceinline__ u32 zb_walk_cand(u32 c, u32 h, u32 x)
+__device__ __forceinline__ u32 zb_walk_key(u32 x) { return x ^ (ZB_BATCH - 1u); }   /* (x | B-1) - (x & B-1); its own inverse */
+/* candidate distance of the position at walk coordinate x given the content c its bucket had before x's batch (0 = no
+ * candidate).  Every entry then came from an earlier batch (or a dictionary image: coordinates below the frame's), so it
+ * lies below x: only emptiness and the tag decide.  Coordinates stay below 2^21, so (key + 1) << TAG_BITS does not wrap. */
+__device__ __forceinline__ u32 zb_walk_cand_prior(u32 c, u32 h, u32 x)
 {
     u32 const px = zb_walk_key((c >> ZB_TAG_BITS) - 1u);
-    return (((c ^ h) & ZB_TAG_MASK) == 0u && px < x) ? x - px : 0u;
+    return (((c ^ h) & ZB_TAG_MASK) == 0u && c != 0u) ? x - px : 0u;
 }
 
 /* which of the P consecutive positions starting at a position whose residue modulo `step` is r0 lie on the insertion
@@ -117,7 +113,10 @@ __device__ __forceinline__ u32 zb_walk_residue(u32 rel0, u32 step)
 /* One batch of the walk for one thread: P consecutive positions from walk coordinate xa.
  * INTERIOR: every position of the batch is walked, lies in the frame's own bytes and has its 8 bytes readable: no
  * activity predicates, bytes come from the words prefetched in wrd[].
- * Returns whether any position of the CTA found a candidate in phase A (the barrier between A and B carries the OR). */
+ * Returns whether any position of the CTA found a candidate in phase A (the barrier between A and B carries the OR).
+ * The walk is bound by instruction issue, not by memory (DESIGN.md section 2): the insertions are predicated, a batch
+ * without output (the history that primes the table) stops after its insertions, and the far distances are handled
+ * behind one warp vote. */
 #define ZB_WALK_NWR(P) ((P) == 1 ? 2 : ((P) + 7 + 3) / 4)        /* realigned words that hold a thread's P + 7 bytes */
 template <int MLS, int P, bool INTERIOR>
 __device__ __forceinline__ bool zb_walk_batch(u32* __restrict__ table, u32 xa, const u32 (&wrd)[ZB_WALK_NWR(P)], u32 pat,
@@ -129,86 +128,77 @@ __device__ __forceinline__ bool zb_walk_batch(u32* __restrict__ table, u32 xa, c
     /* ---- A: hash, read the bucket ---- */
     {   u32 const rel0 = xa - shift;
         bool const slow = !INTERIOR && ((xa < xLow) || (D != 0u && rel0 < D && rel0 + P + 7u > D) || (rel0 + P + 7u > total));
-        u32 old[P];
 #pragma unroll
         for (int i = 0; i < P; i++) {
             u32 const x = xa + (u32)i, rel = x - shift;
             act[i] = INTERIOR ? true : ((x >= xLow) && (rel + 8u <= total) && !(rel < D && rel + 8u > D));
-            u64 v;
-            if (slow) v = act[i] ? zb_ld64u((rel < D ? dbase : fbase) + rel) : 0ull;
+            u32 lo, hi;
+            if (slow) { u64 const v = act[i] ? zb_ld64u((rel < D ? dbase : fbase) + rel) : 0ull; lo = (u32)v; hi = (u32)(v >> 32); }
             else {
                 constexpr int NWR = ZB_WALK_NWR(P);
                 int const wi = i >> 2; u32 const sh = 8u * (u32)(i & 3);
                 int const w2 = wi + 2 < NWR ? wi + 2 : NWR - 1;           /* only read when i & 3: then wi + 2 < NWR */
-                u32 const lo = (i & 3) ? __funnelshift_r(wrd[wi], wrd[wi + 1], sh) : wrd[wi];
-                u32 const hi = (i & 3) ? __funnelshift_r(wrd[wi + 1], wrd[w2], sh) : wrd[wi + 1];
-                v = ((u64)hi << 32) | lo;
+                lo = (i & 3) ? __funnelshift_r(wrd[wi], wrd[wi + 1], sh) : wrd[wi];
+                hi = (i & 3) ? __funnelshift_r(wrd[wi + 1], wrd[w2], sh) : wrd[wi + 1];
             }
-            h[i] = zb_hash(v, MLS, 32u);
+            h[i] = zb_hash32<MLS>(lo, hi);
             bkt[i] = __umulhi(h[i], N);
-            old[i] = act[i] ? table[bkt[i]] : 0u;
+            dOld[i] = zb_walk_cand_prior(act[i] ? table[bkt[i]] : 0u, h[i], x);
         }
-#pragma unroll
-        for (int i = 0; i < P; i++) dOld[i] = zb_walk_cand(old[i], h[i], xa + (u32)i);
     }
     u32 anyOld = 0;
 #pragma unroll
     for (int i = 0; i < P; i++) anyOld |= dOld[i];
     bool const anyHit = __syncthreads_or(anyOld != 0u) != 0;
-    /* ---- B: insertions ---- */
-#if WALK_FAST_BC
-    /* a thread's first coordinate is a multiple of P, so the reversed in-batch offsets of its positions count down from
-     * position 0's: key(xa + i) = key(xa) - i; an entry is (Y1 - i) << TAG_BITS | tag with Y1 = key(xa) + 1 */
-    u32 const Y1 = zb_walk_key(xa) + 1u;
-#pragma unroll
-    for (int i = 0; i < P; i++)
-        if (act[i] && dOld[i] == 0u && ((pat >> i) & 1u)) atomicMax(&table[bkt[i]], ((Y1 - (u32)i) << ZB_TAG_BITS) | (h[i] & ZB_TAG_MASK));
-    __syncthreads();
-    /* ---- C: second look, output.  A position without a candidate can only have gained one from this batch's insertions
-     * (its bucket held no entry with its tag before, and what was there came from earlier batches): inside one batch the
-     * distance is the difference of the keys, so the look is shift, add, tag test, sign test ---- */
-    u32 d[P];
+    /* ---- B: insertions: positions that are walked, found no candidate and lie on the pattern.
+     * A thread's first coordinate is a multiple of P, so the reversed in-batch offsets of its positions count down from
+     * position 0's: key(xa + i) = key(xa) - i; an entry is (Y1 - i) << TAG_BITS | tag with Y1 = key(xa) + 1.
+     * Every position issues its atomicMax, one that does not insert with 0 (no effect on a maximum): ptxas wraps a
+     * conditional or predicated shared atomic in a divergence region of its own, which costs more issue slots than the
+     * select and the extra shared-memory traffic ---- */
+    u32 const Y1s = (zb_walk_key(xa) + 1u) << ZB_TAG_BITS;
+    u32 e[P];
 #pragma unroll
     for (int i = 0; i < P; i++) {
-        d[i] = dOld[i];
-        if (act[i] && d[i] == 0u) {
-            u32 const c = table[bkt[i]];
-            int const dd = (int)((c >> ZB_TAG_BITS) - Y1 + (u32)i);        /* key(candidate) - key(me) */
-            d[i] = ((((c ^ h[i]) & ZB_TAG_MASK) == 0u) && dd > 0) ? (u32)dd : 0u;
-        }
+        e[i] = (Y1s - ((u32)i << ZB_TAG_BITS)) | (h[i] & ZB_TAG_MASK);
+        atomicMax(&table[bkt[i]], (act[i] && dOld[i] == 0u && ((pat >> i) & 1u)) ? e[i] : 0u);
     }
-#else
-#pragma unroll
-    for (int i = 0; i < P; i++)
-        if (act[i] && dOld[i] == 0u && ((pat >> i) & 1u)) atomicMax(&table[bkt[i]], zb_walk_entry(h[i], xa + (u32)i));
-    __syncthreads();
-    /* ---- C: second look, output ---- */
-    u32 d[P];
+    __syncthreads();                                              /* also orders these insertions before the next batch's A */
+    if (!output) return anyHit;                                   /* CTA-uniform: priming batches only fill the table */
+    /* ---- C: second look.  A position without a candidate can only have gained one from this batch's insertions (its
+     * bucket held no entry with its tag before, and what was there came from earlier batches).  With equal tags the
+     * bucket's entry minus the position's own is the key difference << TAG_BITS, and inside one batch the key difference
+     * is the distance; unequal tags leave low bits that the rotation moves to the top.  So the rotated difference is the
+     * distance exactly when it is below ZB_BATCH: an entry of an earlier batch has the smaller key, and its difference
+     * wraps to 2^21 minus the keys' spread, far above ZB_BATCH (coordinates stay below 2^20).  A position that found a
+     * candidate in A never finds one here: every position of its bucket with its tag found the same entry and did not
+     * insert, so the look needs no test of dOld ---- */
+    u32 d[P], orD = 0;
 #pragma unroll
     for (int i = 0; i < P; i++) {
-        d[i] = dOld[i];
-        if (act[i] && d[i] == 0u) d[i] = zb_walk_cand(table[bkt[i]], h[i], xa + (u32)i);
+        u32 const c = table[bkt[i]] - e[i];
+        u32 const r = __funnelshift_r(c, c, ZB_TAG_BITS);
+        d[i] = (act[i] && r < ZB_BATCH) ? r : dOld[i];
+        orD |= d[i];
     }
-#endif
-    if (output && (INTERIOR || xa < xEnd)) {
-        u32 anyFar = 0;
+    /* ---- output.  Distances >= ZB_FAR are rare: one vote (the OR of a thread's distances is at least their maximum)
+     * decides whether the warp looks at them one by one ---- */
+    bool const mine = INTERIOR || xa < xEnd;
+    if (__any_sync(ZB_FULL, mine && orD >= ZB_FAR)) {
 #pragma unroll
-        for (int i = 0; i < P; i++) anyFar |= d[i] >= ZB_FAR ? 1u : 0u;
-        if (anyFar) {
+        for (int i = 0; i < P; i++) if (d[i] >= ZB_FAR) { if (mine && (INTERIOR || xa + (u32)i < xEnd)) farRow[i] = d[i]; d[i] = ZB_FAR; }
+    }
+    if (!mine) return anyHit;
+    auto pk = [&](int i) { return __byte_perm(d[i], d[i + 1], 0x5410); };   /* d[i] | d[i + 1] << 16: every d <= ZB_FAR here */
+    bool vec = false;
+    if constexpr (P == 16) { if (INTERIOR || xa + 16u <= xEnd) { uint4* const o4 = reinterpret_cast<uint4*>(distRow);
+                                 o4[0] = make_uint4(pk(0), pk(2), pk(4), pk(6)); o4[1] = make_uint4(pk(8), pk(10), pk(12), pk(14)); vec = true; } }
+    if constexpr (P == 8) { if (INTERIOR || xa + 8u <= xEnd) { *reinterpret_cast<uint4*>(distRow) = make_uint4(pk(0), pk(2), pk(4), pk(6)); vec = true; } }
+    if constexpr (P == 4) { if (INTERIOR || xa + 4u <= xEnd) { *reinterpret_cast<uint2*>(distRow) = make_uint2(pk(0), pk(2)); vec = true; } }
+    if constexpr (P == 2) { if (INTERIOR || xa + 2u <= xEnd) { *reinterpret_cast<u32*>(distRow) = pk(0); vec = true; } }
+    if (!vec) {
 #pragma unroll
-            for (int i = 0; i < P; i++) if (d[i] >= ZB_FAR) { if (INTERIOR || xa + (u32)i < xEnd) farRow[i] = d[i]; d[i] = ZB_FAR; }
-        }
-        bool vec = false;
-        if constexpr (P == 16) { if (INTERIOR || xa + 16u <= xEnd) { uint4* const o4 = reinterpret_cast<uint4*>(distRow);
-                                     o4[0] = make_uint4(d[0] | (d[1] << 16), d[2] | (d[3] << 16), d[4] | (d[5] << 16), d[6] | (d[7] << 16));
-                                     o4[1] = make_uint4(d[8] | (d[9] << 16), d[10] | (d[11] << 16), d[12] | (d[13] << 16), d[14] | (d[15] << 16)); vec = true; } }
-        if constexpr (P == 8) { if (INTERIOR || xa + 8u <= xEnd) { *reinterpret_cast<uint4*>(distRow) = make_uint4(d[0] | (d[1] << 16), d[2] | (d[3] << 16), d[4] | (d[5] << 16), d[6] | (d[7] << 16)); vec = true; } }
-        if constexpr (P == 4) { if (INTERIOR || xa + 4u <= xEnd) { *reinterpret_cast<uint2*>(distRow) = make_uint2(d[0] | (d[1] << 16), d[2] | (d[3] << 16)); vec = true; } }
-        if constexpr (P == 2) { if (INTERIOR || xa + 2u <= xEnd) { *reinterpret_cast<u32*>(distRow) = d[0] | (d[1] << 16); vec = true; } }
-        if (!vec) {
-#pragma unroll
-            for (int i = 0; i < P; i++) if (xa + (u32)i < xEnd) distRow[i] = (u16)d[i];
-        }
+        for (int i = 0; i < P; i++) if (xa + (u32)i < xEnd) distRow[i] = (u16)d[i];
     }
     return anyHit;
 }
@@ -223,10 +213,10 @@ __device__ __forceinline__ bool zb_walk_batch(u32* __restrict__ table, u32 xa, c
 #define WALK_STEADY 1            /* development switch: 0 = every batch takes the general path */
 #endif
 #ifndef WALK_P_SMALL
-#define WALK_P_SMALL 8           /* positions per thread for tables <= 56 KiB: 128 threads per CTA (on the H100 the walk takes 3.05 ms per GiB of config 2 with 8 and 3.03 with 4: equal within run-to-run spread; development knob: tools/build_variant.sh) */
+#define WALK_P_SMALL 8           /* positions per thread for tables <= 56 KiB: 128 threads per CTA (on the H100 the walk takes 2.54 ms per GiB of config 2 with 8, 2.80 with 4, 2.81 with 16; development knob: tools/build_variant.sh) */
 #endif
 #ifndef WALK_P_MID
-#define WALK_P_MID 4             /* tables of 56 .. 113 KiB: two CTAs per SM (walk on the H100, config 4: 8.22 ms with 4 positions per thread, 8.83 with 2) */
+#define WALK_P_MID 4             /* tables of 56 .. 113 KiB: two CTAs per SM (walk on the H100, config 4: 8.16 ms with 4 positions per thread, 9.25 with 8, 8.83 with 2 before the walk's instruction cut) */
 #endif
 #ifndef WALK_MINB_SMALL
 #define WALK_MINB_SMALL 4        /* CTAs per SM the register allocation of that variant leaves room for */
