@@ -13,6 +13,7 @@
 #include <stdlib.h>
 #include <string.h>
 #include <vector>
+#include <memory>
 #include <mutex>
 #include <thread>
 #include <new>
@@ -115,16 +116,18 @@ static std::atomic<int> g_device(-1);
  * or ZSTDB200_compressFrames are digested into the context's own object (ZSTD_CCtx_s::callDict) on every call. */
 struct ZSTD_CDict_s {
     int level;
-    const u8* content;             /* the whole dictionary: ZSTD_createCDict's copy behind the object (ZSTD_dlm_byCopy), or the caller's buffer */
+    std::unique_ptr<u8[]> copy;    /* ZSTD_createCDict's copy of the bytes (ZSTD_dlm_byCopy) */
+    const u8* content;             /* the whole dictionary: that copy, or the caller's buffer */
     size_t size;
     size_t contentOff, tail;       /* entropy header size, bytes of content that blocks can see */
     ZbDictEntropy entropy;         /* parsed on the host by zb_digestDict */
-    std::mutex* lock;              /* guards the device state below */
+    std::mutex lock;               /* guards the device state below */
     int device;                    /* -1 until the device buffers exist */
     bool resident;                 /* tail and entropy tables uploaded since the digest */
-    u8* d_dict; ZbDictEntropy* d_de; u8* d_image; ZbChunk* d_dictChunk;
+    ZbDevBuf<u8> d_dict; ZbDevBuf<ZbDictEntropy> d_de; ZbDevBuf<u8> d_image; ZbDevBuf<ZbChunk> d_dictChunk;
     u32 nbImages; ZbParams imagePrm[ZB_MAX_IMAGES];
 };
+struct ZbCDictFree { void operator()(ZSTD_CDict* cd) const { ZSTD_freeCDict(cd); } };
 
 struct ZbGroup { ZbParams prm; u32 b0, b1, c0, c1; const u32* image; bool ldm; };   /* ldm: its frames have long-distance matches */   /* image: tables walked over the dictionary tail, or NULL */
 /* Descriptor arrays of a plan: page-locked (so that the upload of a million frames' descriptors is a DMA at PCIe speed, not a
@@ -162,15 +165,17 @@ struct ZbPlan { ZbVec<ZbBlock> blocks; ZbVec<ZbChunk> chunks; ZbVec<ZbFrame> fra
                 void reset() { blocks.clear(); chunks.clear(); frames.clear(); groups.clear(); unsupported = false; ldm.clear(); ldmMatches = 0;
                                frameBytes = frameBlocks = 0; frameMaxBlock = 0; } };   /* keeps its memory: a context plans call after call */
 
+enum { EV_START, EV_K0, EV_K1, EV_K2, EV_K3, EV_MID, EV_KEND, EV_END, EV_PHASES };   /* a compression context's phase events */
+
 struct ZSTD_CCtx_s {
     int device;                    /* -1 until the first call created the stream and events on bindDevice */
     int bindDevice;                /* device captured by ZSTD_createCCtx */
-    cudaStream_t stream;
+    ZbStream stream;
     /* per-block workspace */
     ZbDevBuf<ZbChunk> d_chunks;
     ZbDevBuf<ZbSegMeta> d_segmeta; /* K1b -> K1c: per parse segment counts */
     u32 devWaveBlocks;             /* device-memory calls: blocks per wave (0 = always one wave) */
-    cudaStream_t waveStream[ZB_WAVE_SLOTS_MAX + 1];   /* one per workspace slot, then the host path's download stream */
+    ZbStream waveStream[ZB_WAVE_SLOTS_MAX + 1];       /* one per workspace slot, then the host path's download stream */
     u32 waveSlots;                 /* waves in flight, device-memory calls */
     u32 hostWaveSlots;             /* waves in flight, host-memory calls */
     u32 hostWaveBlocks;            /* host-memory calls: blocks per wave */
@@ -184,10 +189,9 @@ struct ZSTD_CCtx_s {
     ZbHostBuf<u64> h_totals;       /* mirror of d_totals */
     /* host-pointer path staging */
     ZbDevBuf<u8> d_in, d_out;
-    ZSTD_CDict* callDict;          /* digest of the dictionary bytes the current call passes; reads the caller's buffer in place */
-    cudaEvent_t evStart, evK0, evMid, evK1, evK2, evK3, evKEnd, evEnd;
-    cudaEvent_t* evWave;           /* per wave: uploaded, stitched, size copied, downloaded (4 runs of capEvWaves events) */
-    u32 capEvWaves; bool evWaveTimed;
+    std::unique_ptr<ZSTD_CDict, ZbCDictFree> callDict;   /* digest of the dictionary bytes the current call passes; reads the caller's buffer in place */
+    ZbEvents ev;                   /* EV_START .. EV_END */
+    ZbEvents evH2D, evStitch, evSize, evD2H;   /* per wave: uploaded, stitched, size copied, downloaded */
     ZSTDB200_stats stats;
     /* advanced one-shot API (ZSTD_CCtx_setParameter + ZSTD_compress2, lib/zstd.h:337-603): sticky parameters */
     int advLevel, advChecksum, advNoDictID;
@@ -195,7 +199,7 @@ struct ZSTD_CCtx_s {
     u32 advLdmPrm[4];              /* ZSTD_c_ldmHashLog, ldmMinMatch, ldmBucketSizeLog, ldmHashRateLog; 0 = derived from the window */
     /* long-distance matching workspace: the call's match list and per-block (first, count), one frame's scratch */
     ZbDevBuf<u64> d_ldmMatch, d_ldmFirst; ZbDevBuf<u32> d_ldmCnt; ZbDevBuf<u8> d_ldmScratch;
-    ZSTD_CDict* advLocalDict;      /* ZSTD_CCtx_loadDictionary: owned copy, digested at its first use */
+    std::unique_ptr<ZSTD_CDict, ZbCDictFree> advLocalDict;   /* ZSTD_CCtx_loadDictionary: owned copy, digested at its first use */
     const ZSTD_CDict* advRefCDict; /* ZSTD_CCtx_refCDict: borrowed */
     ZbPlan plan;                   /* the call's plan; its vectors are reused (a million records are 100 MB of descriptors: fresh pages cost more than filling them) */
     /* streaming front end (ZSTD_compressStream2 with ZSTD_e_continue / ZSTD_e_flush): input collected on the host, compressed
@@ -252,58 +256,26 @@ static size_t zb_ctxInit(ZSTD_CCtx* c)
     if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) { cudaGetLastError(); return ZB_ERR(ZB_error_GENERIC); }
     int dev = c->bindDevice;
     if (dev < 0) { if (cudaGetDevice(&dev) != cudaSuccess) dev = 0; }
-    /* everything or nothing: a partial failure leaves the context uninitialised (device stays -1) */
-    cudaStream_t st; cudaEvent_t ev[8];
-    TRY(zb_streamCreate(dev, &st, ev, 8));
+    CK(cudaSetDevice(dev));
+    /* everything or nothing: the stream and events are the context's only once every step succeeded (device stays -1
+     * until then); after a failure they are destroyed here */
+    ZbStream st; ZbEvents ev;
+    TRY(st.ensure());
+    TRY(ev.ensure(EV_PHASES, true));
     /* the predefined FSE tables live in device memory (one copy per device; re-uploading the same bytes is harmless) */
     static ZbdFseCTable defaults[3]; static std::once_flag once;
     std::call_once(once, [] { zb_buildDefaultTables(defaults); });
-    cudaError_t e = zb_upload_default_tables(defaults, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) zb_streamDestroy(st, ev, 8);
-    CK(e);
-    c->stream = st;
-    c->evStart = ev[0]; c->evK0 = ev[1]; c->evK1 = ev[2]; c->evK2 = ev[3]; c->evK3 = ev[4]; c->evMid = ev[5]; c->evKEnd = ev[6]; c->evEnd = ev[7];
+    CK(zb_upload_default_tables(defaults, st));
+    CK(cudaStreamSynchronize(st));
+    c->stream = std::move(st); c->ev = std::move(ev);
     c->device = dev;
     return 0;
 }
 
-static void zb_freeWaveEvents(ZSTD_CCtx* c)
-{
-    for (u32 i = 0; i < 4u * c->capEvWaves; i++) if (c->evWave[i]) cudaEventDestroy(c->evWave[i]);
-    free(c->evWave); c->evWave = NULL; c->capEvWaves = 0;
-}
-/* the events are created once and kept: a call creates none unless it has more waves than any call before it (or
- * ZSTDB200_TIMELINE changed, which wants timed events) */
-static size_t zb_ensureWaveEvents(ZSTD_CCtx* c, u32 nbWaves, bool timed)
-{
-    if (nbWaves <= c->capEvWaves && timed == c->evWaveTimed) return 0;
-    zb_freeWaveEvents(c);
-    c->evWave = (cudaEvent_t*)calloc(4u * nbWaves, sizeof(cudaEvent_t));
-    if (!c->evWave) return ZB_ERR(ZB_error_memory_allocation);
-    c->capEvWaves = nbWaves; c->evWaveTimed = timed;
-    for (u32 i = 0; i < 4u * nbWaves; i++) {
-        cudaError_t const e = cudaEventCreateWithFlags(&c->evWave[i], timed ? cudaEventDefault : cudaEventDisableTiming);
-        if (e != cudaSuccess) { zb_freeWaveEvents(c); CK(e); }
-    }
-    return 0;
-}
-
-extern "C" size_t ZSTD_freeCDict(ZSTD_CDict* cd);
 extern "C" size_t ZSTD_freeCCtx(ZSTD_CCtx* c)
 {
-    if (!c) return 0;
-    ZSTD_freeCDict(c->advLocalDict); ZSTD_freeCDict(c->callDict);
-    free(c->stIn); free(c->stOut);
-    if (c->device < 0) { delete c; return 0; }                  /* never reached a device: it holds nothing there */
-    ZbDeviceGuard guard;
-    cudaSetDevice(c->device);
-    zb_freeWaveEvents(c);
-    for (u32 s = 0; s <= ZB_WAVE_SLOTS_MAX; s++) if (c->waveStream[s]) cudaStreamDestroy(c->waveStream[s]);
-    cudaEvent_t const ev[8] = { c->evStart, c->evK0, c->evK1, c->evK2, c->evK3, c->evMid, c->evKEnd, c->evEnd };
-    zb_streamDestroy(c->stream, ev, 8);
-    delete c;                                                   /* its buffers free themselves, on its device */
-    return 0;
+    if (c) { free(c->stIn); free(c->stOut); }
+    return zb_deleteOnDevice(c);                                /* its dictionaries, streams, events and buffers free themselves */
 }
 
 /* descriptors (per block / per frame, small) and the heavy per-block workspace are sized separately:
@@ -483,12 +455,12 @@ static size_t zb_digestDict(ZSTD_CDict* cd, const u8* dict, size_t dictSize)
  * uploaded once per digest.  shared: other contexts may use cd right away, so the upload is complete when this returns. */
 static size_t zb_residentDict(ZSTD_CDict* cd, int device, bool shared, cudaStream_t stream)
 {
-    std::lock_guard<std::mutex> g(*cd->lock);
+    std::lock_guard<std::mutex> g(cd->lock);
     if (cd->device >= 0 && cd->device != device) return ZB_ERR(ZB_error_parameter_unsupported);   /* one device per CDict */
     if (cd->resident) return 0;
     if (cd->device < 0) {      /* content tail with 32 bytes of padding on both sides, entropy state, table images, pseudo chunk descriptors */
-        CK(cudaMalloc(&cd->d_dict, ZB_PRIME_BYTES + 64)); CK(cudaMalloc(&cd->d_de, sizeof(ZbDictEntropy)));
-        CK(cudaMalloc(&cd->d_image, (size_t)ZB_IMAGE_BYTES * ZB_MAX_IMAGES)); CK(cudaMalloc(&cd->d_dictChunk, ZB_MAX_IMAGES * sizeof(ZbChunk)));
+        TRY(cd->d_dict.ensure(ZB_PRIME_BYTES + 64)); TRY(cd->d_de.ensure(1));
+        TRY(cd->d_image.ensure((size_t)ZB_IMAGE_BYTES * ZB_MAX_IMAGES)); TRY(cd->d_dictChunk.ensure(ZB_MAX_IMAGES));
         cd->device = device;
     }
     CK(cudaMemsetAsync(cd->d_dict, 0, ZB_PRIME_BYTES + 64, stream));
@@ -507,7 +479,7 @@ static size_t zb_buildDictImages(ZSTD_CDict* cd, ZbPlan& P, bool shared, cudaStr
 {
     if (cd->tail < 8) return 0;
     const u8* const d_dictEnd = cd->d_dict + 32 + cd->tail;
-    std::lock_guard<std::mutex> g(*cd->lock);
+    std::lock_guard<std::mutex> g(cd->lock);
     bool built = false;
     for (size_t gi = 0; gi < P.groups.size(); gi++) {
         ZbParams const& prm = P.groups[gi].prm;
@@ -572,7 +544,7 @@ static size_t zb_runBlocks(ZSTD_CCtx* c, const ZbPlan& P, const u8* d_src, const
                 CK(zb_launch_match(d_src, d_dictEnd, d_dictEnd ? G.image : (const u32*)0, c->d_blocks + lo, hi - lo, c->d_chunks + clo, chi - clo, lo, &G.prm, &P.sd,
                                    c->d_dist + s * P.sd.dist, c->d_far + s * P.sd.dist, df ? c->d_dist2 + s * P.sd.dist : (u16*)0, df ? c->d_far2 + s * P.sd.dist : (u32*)0,
                                    c->d_seqs + s * P.sd.seq, c->d_lits + s * P.sd.lit, c->d_meta + s, c->d_segmeta + s * ((P.sd.dist + ZB_PARSE_SEG - 1u) / ZB_PARSE_SEG),
-                                   (timed && P.groups.size() == 1) ? c->evMid : (cudaEvent_t)0, stream, G.ldm ? &lv : nullptr));
+                                   (timed && P.groups.size() == 1) ? c->ev[EV_MID] : (cudaEvent_t)0, stream, G.ldm ? &lv : nullptr));
                 *launches += df ? 4 : 3;       /* walk(s), parse, merge */
             } else if (phase == 1) {
                 CK(zb_launch_literals(c->d_blocks + lo, hi - lo, &G.prm, &P.sd, d_de, c->d_lits + s * P.sd.lit, c->d_body + s * P.sd.body, c->d_meta + s, stream));
@@ -583,7 +555,7 @@ static size_t zb_runBlocks(ZSTD_CCtx* c, const ZbPlan& P, const u8* d_src, const
                 *launches += 1;
             }
         }
-        if (timed) CK(cudaEventRecord(phase == 0 ? c->evK1 : (phase == 1 ? c->evK2 : c->evK3), stream));
+        if (timed) CK(cudaEventRecord(c->ev[EV_K1 + phase], stream));
     }
     return 0;
 }
@@ -635,7 +607,7 @@ static size_t zb_compress(ZSTD_CCtx* c, const ZbCall& a)
     /* the dictionary: a caller's ZSTD_CDict, which other contexts may share (its device state is guarded by cd->lock), or
      * the context's digest of this call's bytes */
     ZSTD_CDict* const cd = (a.cdict && a.cdict->size >= 8) ? const_cast<ZSTD_CDict*>(a.cdict) : NULL;   /* zstd_compress.c:5130 : tiny dictionaries are ignored */
-    bool const shared = cd != c->callDict;
+    bool const shared = cd != c->callDict.get();
     if (cd) TRY(zb_residentDict(cd, c->device, shared, sCopy));
     const ZbDictEntropy* const de = (cd && cd->entropy.present) ? &cd->entropy : NULL;
     const u8* const d_dictEnd = cd ? cd->d_dict + 32 + cd->tail : NULL;
@@ -687,31 +659,29 @@ static size_t zb_compress(ZSTD_CCtx* c, const ZbCall& a)
     TRY(zb_ensureDesc(c, nbBlocks, nbFrames, nbWaves, P.chunks.size()));
     {   bool d2 = false; for (size_t g = 0; g < P.groups.size(); g++) d2 |= (P.groups[g].prm.strategy == 2);
         TRY(zb_ensureHeavy(c, (size_t)slots * maxWaveBlocks, P.sd, d2)); }
-    TRY(zb_ensureWaveEvents(c, nbWaves, timeline));
-    cudaEvent_t* const evH2D = c->evWave, * const evStitch = evH2D + c->capEvWaves, * const evSize = evStitch + c->capEvWaves, * const evD2H = evSize + c->capEvWaves;
-    /* streams are created on first use: every stream beyond the hardware queue count (8 by default) shares a
+    /* the wave events are created once and kept: a call creates none unless it has more waves than any call before it (or
+     * ZSTDB200_TIMELINE changed, which wants timed events) */
+    TRY(c->evH2D.ensure(nbWaves, timeline)); TRY(c->evStitch.ensure(nbWaves, timeline));
+    TRY(c->evSize.ensure(nbWaves, timeline)); TRY(c->evD2H.ensure(nbWaves, timeline));
+    /* wave streams are created on first use: every stream beyond the hardware queue count (8 by default) shares a
      * queue with another one, and a download queued behind another wave's kernels stalls the whole pipeline */
-    auto getStream = [&](u32 i, cudaStream_t* out) -> size_t {
-        if (!c->waveStream[i]) CK(cudaStreamCreateWithFlags(&c->waveStream[i], cudaStreamNonBlocking));
-        *out = c->waveStream[i];
-        return 0;
-    };
     u8* d_in; u8* d_out; cudaStream_t sD2H = (cudaStream_t)0;
     if (deviceMemory) { d_in = (u8*)src; d_out = dst; }
     else {
         TRY(c->d_in.ensure(inEnd + 16)); TRY(c->d_out.ensure(outCap + 16));
         d_in = c->d_in; d_out = c->d_out;
-        TRY(getStream(ZB_WAVE_SLOTS_MAX, &sD2H));
+        TRY(c->waveStream[ZB_WAVE_SLOTS_MAX].ensure());
+        sD2H = c->waveStream[ZB_WAVE_SLOTS_MAX];
     }
     std::vector<double> hostDone(nbWaves, 0.0);
     double const hostT0 = zb_now();
     unsigned launches = 0;
     size_t err = 0;
-    if (!single) CK(cudaEventRecord(c->evStart, sCopy));
+    if (!single) CK(cudaEventRecord(c->ev[EV_START], sCopy));
     CK(cudaMemcpyAsync(c->d_blocks, P.blocks.data(), nbBlocks * sizeof(ZbBlock), cudaMemcpyHostToDevice, sCopy));
     CK(cudaMemcpyAsync(c->d_frames, P.frames.data(), nbFrames * sizeof(ZbFrame), cudaMemcpyHostToDevice, sCopy));
     CK(cudaMemcpyAsync(c->d_chunks, P.chunks.data(), P.chunks.size() * sizeof(ZbChunk), cudaMemcpyHostToDevice, sCopy));
-    if (single) CK(cudaEventRecord(c->evK0, sCopy));
+    if (single) CK(cudaEventRecord(c->ev[EV_K0], sCopy));
     if (cd && (nbFrames >= 8 || shared)) TRY(zb_buildDictImages(cd, P, shared, sCopy));   /* a per-call digest builds its images afresh on every call: only for 8 frames or more */
     cudaStream_t lastStream = sCopy;
     bool const ldm = !P.ldm.empty();
@@ -732,23 +702,24 @@ static size_t zb_compress(ZSTD_CCtx* c, const ZbCall& a)
         }
         cudaStream_t st = sCopy;
         if (!single) {
-            CK(cudaEventRecord(evH2D[w], sCopy));
-            TRY(getStream(w % slots, &st));
-            CK(cudaStreamWaitEvent(st, evH2D[w], 0));
+            CK(cudaEventRecord(c->evH2D[w], sCopy));
+            TRY(c->waveStream[w % slots].ensure());
+            st = c->waveStream[w % slots];
+            CK(cudaStreamWaitEvent(st, c->evH2D[w], 0));
         }
         lastStream = st;
-        err = zb_runBlocks(c, P, d_in, d_dictEnd, de ? cd->d_de : NULL, b0, b1, wc[w], wc[w + 1], s0, st, single, &launches);
+        err = zb_runBlocks(c, P, d_in, d_dictEnd, de ? cd->d_de.p : NULL, b0, b1, wc[w], wc[w + 1], s0, st, single, &launches);
         if (err) break;
-        if (w > 0) CK(cudaStreamWaitEvent(st, evStitch[w - 1], 0));
+        if (w > 0) CK(cudaStreamWaitEvent(st, c->evStitch[w - 1], 0));
         CK(zb_launch_stitch(d_in, c->d_blocks + b0, b1 - b0, c->d_frames, c->d_body + s0 * P.sd.body, P.sd.body, c->d_meta + s0,
                             c->d_outOffsets + b0, w > 0 ? c->d_totals + (w - 1) : NULL, c->d_totals + w, d_out, outCap, st));
         launches += 2;
-        if (!single) CK(cudaEventRecord(evStitch[w], st));
+        if (!single) CK(cudaEventRecord(c->evStitch[w], st));
         /* the wave's size goes to the host behind the event the next wave's stitch waits for: a store into mapped
          * host memory from inside the scan kernel would add a PCIe round trip to every link of that chain */
         if (download || timeline) {
             CK(cudaMemcpyAsync(c->h_totals + w, c->d_totals + w, sizeof(u64), cudaMemcpyDeviceToHost, st));
-            CK(cudaEventRecord(evSize[w], st));
+            CK(cudaEventRecord(c->evSize[w], st));
         }
     }
     double const hostEnq = zb_now() - hostT0;
@@ -772,19 +743,19 @@ static size_t zb_compress(ZSTD_CCtx* c, const ZbCall& a)
     if (download || timeline) {
         /* drain: as each wave's size becomes known, ship its bytes */
         for (u32 w = 0; w < nbWaves && !err; w++) {
-            CK(cudaEventSynchronize(evSize[w]));
+            CK(cudaEventSynchronize(c->evSize[w]));
             hostDone[w] = zb_now() - hostT0;
             total = c->h_totals[w];
             if (download && total <= outCap && total > prev) CK(cudaMemcpyAsync(dst + prev, d_out + prev, total - prev, cudaMemcpyDeviceToHost, sD2H));
             if (total <= outCap) prev = total;
-            if (timeline) CK(cudaEventRecord(evD2H[w], download ? sD2H : lastStream));
+            if (timeline) CK(cudaEventRecord(c->evD2H[w], download ? sD2H : lastStream));
         }
     }
     if (!err && wantSizes) {
         CK(zb_launch_frame_sizes(c->d_frames, (u32)nbFrames, c->d_outOffsets, c->d_frameSizes, lastStream));
         if (single) launches++;                                          /* a multi-wave call's count leaves this kernel out */
     }
-    if (single) CK(cudaEventRecord(c->evKEnd, lastStream));
+    if (single) CK(cudaEventRecord(c->ev[EV_KEND], lastStream));
     if (!err && !download && !timeline) CK(cudaMemcpyAsync(c->h_totals + nbWaves - 1, c->d_totals + nbWaves - 1, sizeof(u64), cudaMemcpyDeviceToHost, lastStream));
     if (!err && wantSizes) {
         fsz.resize(nbFrames);
@@ -793,8 +764,8 @@ static size_t zb_compress(ZSTD_CCtx* c, const ZbCall& a)
         if (a.cSizes) for (size_t f = 0; f < nbFrames; f++) a.cSizes[f] = (size_t)fsz[f];
     }
     /* the last wave's stitch is ordered behind every earlier one (evStitch chain) */
-    if (download) { CK(cudaEventRecord(c->evEnd, sD2H)); CK(cudaStreamSynchronize(sD2H)); }
-    else if (!single) CK(cudaEventRecord(c->evEnd, lastStream));
+    if (download) { CK(cudaEventRecord(c->ev[EV_END], sD2H)); CK(cudaStreamSynchronize(sD2H)); }
+    else if (!single) CK(cudaEventRecord(c->ev[EV_END], lastStream));
     if (!single) for (u32 s = 0; s < slots; s++) if (c->waveStream[s]) CK(cudaStreamSynchronize(c->waveStream[s]));
     CK(cudaStreamSynchronize(sCopy));
     if (!err) total = c->h_totals[nbWaves - 1];
@@ -812,8 +783,8 @@ static size_t zb_compress(ZSTD_CCtx* c, const ZbCall& a)
                 deviceMemory ? "device buffers" : "per-wave downloads");
         for (u32 w = 0; w < nbWaves; w++) {
             float up = 0, st = 0, dn = 0;
-            cudaEventElapsedTime(&up, c->evStart, evH2D[w]); cudaEventElapsedTime(&st, c->evStart, evStitch[w]);
-            cudaEventElapsedTime(&dn, c->evStart, evD2H[w]);
+            cudaEventElapsedTime(&up, c->ev[EV_START], c->evH2D[w]); cudaEventElapsedTime(&st, c->ev[EV_START], c->evStitch[w]);
+            cudaEventElapsedTime(&dn, c->ev[EV_START], c->evD2H[w]);
             fprintf(stderr, "  wave %2u blocks %5u..%5u : uploaded %7.3f  stitched %7.3f (host saw it %7.3f)  downloaded %7.3f\n",
                     w, wb[w], wb[w + 1], up, st, 1e3 * hostDone[w], dn);
         }
@@ -821,13 +792,13 @@ static size_t zb_compress(ZSTD_CCtx* c, const ZbCall& a)
     if (err) return err;
     float ms = 0;
     if (single) {
-        cudaEventElapsedTime(&ms, c->evK0, c->evKEnd); c->stats.kernel_ms = ms;
-        cudaEventElapsedTime(&ms, c->evK0, c->evK1); c->stats.match_ms = ms;
-        if (P.groups.size() == 1) { cudaEventElapsedTime(&ms, c->evK0, c->evMid); c->stats.cand_ms = ms; cudaEventElapsedTime(&ms, c->evMid, c->evK1); c->stats.parse_ms = ms; }
-        cudaEventElapsedTime(&ms, c->evK1, c->evK2); c->stats.literals_ms = ms;
-        cudaEventElapsedTime(&ms, c->evK2, c->evK3); c->stats.sequences_ms = ms;
-        cudaEventElapsedTime(&ms, c->evK3, c->evKEnd); c->stats.stitch_ms = ms;
-    } else { cudaEventElapsedTime(&ms, c->evStart, c->evEnd); c->stats.kernel_ms = ms; }
+        cudaEventElapsedTime(&ms, c->ev[EV_K0], c->ev[EV_KEND]); c->stats.kernel_ms = ms;
+        cudaEventElapsedTime(&ms, c->ev[EV_K0], c->ev[EV_K1]); c->stats.match_ms = ms;
+        if (P.groups.size() == 1) { cudaEventElapsedTime(&ms, c->ev[EV_K0], c->ev[EV_MID]); c->stats.cand_ms = ms; cudaEventElapsedTime(&ms, c->ev[EV_MID], c->ev[EV_K1]); c->stats.parse_ms = ms; }
+        cudaEventElapsedTime(&ms, c->ev[EV_K1], c->ev[EV_K2]); c->stats.literals_ms = ms;
+        cudaEventElapsedTime(&ms, c->ev[EV_K2], c->ev[EV_K3]); c->stats.sequences_ms = ms;
+        cudaEventElapsedTime(&ms, c->ev[EV_K3], c->ev[EV_KEND]); c->stats.stitch_ms = ms;
+    } else { cudaEventElapsedTime(&ms, c->ev[EV_START], c->ev[EV_END]); c->stats.kernel_ms = ms; }
     c->stats.total_ms = c->stats.kernel_ms;
     c->stats.launches = launches; c->stats.nbBlocks = nbBlocks;
     if (!deviceMemory) { c->stats.h2d_bytes = inEnd; c->stats.d2h_bytes = (size_t)total; }
@@ -840,9 +811,10 @@ static size_t zb_digestCallDict(ZSTD_CCtx* c, const void* dict, size_t dictSize,
 {
     *out = NULL;
     if (!dict) return 0;
-    if (!c->callDict && !(c->callDict = ZSTD_createCDict(NULL, 0, 0))) return ZB_ERR(ZB_error_memory_allocation);
-    TRY(zb_digestDict(c->callDict, (const u8*)dict, dictSize));
-    *out = c->callDict;
+    if (!c->callDict) c->callDict.reset(ZSTD_createCDict(NULL, 0, 0));
+    if (!c->callDict) return ZB_ERR(ZB_error_memory_allocation);
+    TRY(zb_digestDict(c->callDict.get(), (const u8*)dict, dictSize));
+    *out = c->callDict.get();
     return 0;
 }
 
@@ -892,29 +864,17 @@ static size_t zb_compressOne(ZSTD_CCtx* c, void* dst, size_t dstCapacity, const 
 extern "C" ZSTD_CDict* ZSTD_createCDict(const void* dict, size_t dictSize, int level)     /* zstd_compress.c:5633 */
 {
     size_t const size = dict ? dictSize : 0;
-    if (size > (size_t)-1 - sizeof(ZSTD_CDict)) return NULL;
-    ZSTD_CDict* cd = (ZSTD_CDict*)calloc(1, sizeof(ZSTD_CDict) + size);         /* the object, then its copy of the bytes (ZSTD_dlm_byCopy) */
+    ZSTD_CDict* cd = new (std::nothrow) ZSTD_CDict();                          /* value-initialised: every plain member is zero */
     if (!cd) return NULL;
     cd->level = level == 0 ? 3 : level;                                          /* ZSTD_CLEVEL_DEFAULT, :5640 */
     cd->device = -1;
-    cd->lock = new (std::nothrow) std::mutex();
-    u8* const copy = (u8*)(cd + 1);
-    if (size) memcpy(copy, dict, size);
-    if (!cd->lock || zb_isErr(zb_digestDict(cd, copy, size))) { ZSTD_freeCDict(cd); return NULL; }   /* corrupted entropy tables: creation fails (:5600-5612) */
+    cd->copy.reset(new (std::nothrow) u8[size]);
+    if (cd->copy && size) memcpy(cd->copy.get(), dict, size);
+    if (!cd->copy || zb_isErr(zb_digestDict(cd, cd->copy.get(), size))) { delete cd; return NULL; }   /* corrupted entropy tables: creation fails (:5600-5612) */
     return cd;
 }
 
-extern "C" size_t ZSTD_freeCDict(ZSTD_CDict* cd)                                            /* accepts NULL, zstd_compress.c:5655 */
-{
-    if (!cd) return 0;
-    if (cd->device >= 0) {
-        ZbDeviceGuard guard;
-        cudaSetDevice(cd->device);
-        cudaFree(cd->d_dict); cudaFree(cd->d_de); cudaFree(cd->d_image); cudaFree(cd->d_dictChunk);
-    }
-    delete cd->lock; free(cd);
-    return 0;
-}
+extern "C" size_t ZSTD_freeCDict(ZSTD_CDict* cd) { return zb_deleteOnDevice(cd); }           /* accepts NULL, zstd_compress.c:5655 */
 
 extern "C" unsigned ZSTD_getDictID_fromCDict(const ZSTD_CDict* cd)                           /* zstd_compress.c:5738 */
 {
@@ -1066,7 +1026,7 @@ extern "C" size_t ZSTD_CCtx_reset(ZSTD_CCtx* c, ZSTD_ResetDirective reset)      
     if (reset == 1 || reset == 3) { c->stInSize = 0; c->stOutSize = 0; c->stOutPos = 0; c->stFrames = 0; }   /* an unfinished stream is dropped */
     if (reset == 2 || reset == 3) {
         c->advLevel = 3; c->advChecksum = 0; c->advNoDictID = 0; c->advDelims = 0; c->advLdm = 0; memset(c->advLdmPrm, 0, sizeof(c->advLdmPrm));
-        ZSTD_freeCDict(c->advLocalDict); c->advLocalDict = NULL; c->advRefCDict = NULL;
+        c->advLocalDict.reset(); c->advRefCDict = NULL;
     }
     return 0;
 }
@@ -1074,16 +1034,16 @@ extern "C" size_t ZSTD_CCtx_reset(ZSTD_CCtx* c, ZSTD_ResetDirective reset)      
 extern "C" size_t ZSTD_CCtx_loadDictionary(ZSTD_CCtx* c, const void* dict, size_t dictSize)  /* zstd_compress.c:1260: copied, sticky */
 {
     if (!c) return ZB_ERR(ZB_error_GENERIC);
-    ZSTD_freeCDict(c->advLocalDict); c->advLocalDict = NULL; c->advRefCDict = NULL;
+    c->advLocalDict.reset(); c->advRefCDict = NULL;
     if (!dict || dictSize == 0) return 0;                                                    /* NULL / 0: back to no dictionary */
-    c->advLocalDict = ZSTD_createCDict(dict, dictSize, c->advLevel);
+    c->advLocalDict.reset(ZSTD_createCDict(dict, dictSize, c->advLevel));
     return c->advLocalDict ? 0 : ZB_ERR(ZB_error_dictionary_corrupted);
 }
 
 extern "C" size_t ZSTD_CCtx_refCDict(ZSTD_CCtx* c, const ZSTD_CDict* cdict)                  /* zstd_compress.c:1330: borrowed, sticky */
 {
     if (!c) return ZB_ERR(ZB_error_GENERIC);
-    ZSTD_freeCDict(c->advLocalDict); c->advLocalDict = NULL;
+    c->advLocalDict.reset();
     c->advRefCDict = cdict;
     return 0;
 }
@@ -1091,7 +1051,7 @@ extern "C" size_t ZSTD_CCtx_refCDict(ZSTD_CCtx* c, const ZSTD_CDict* cdict)     
 extern "C" size_t ZSTD_compress2(ZSTD_CCtx* c, void* dst, size_t dstCapacity, const void* src, size_t srcSize)     /* zstd_compress.c:6365 */
 {
     if (!c) return ZB_ERR(ZB_error_GENERIC);
-    const ZSTD_CDict* const cd = c->advRefCDict ? c->advRefCDict : c->advLocalDict;
+    const ZSTD_CDict* const cd = c->advRefCDict ? c->advRefCDict : c->advLocalDict.get();
     int const level = c->advRefCDict ? c->advRefCDict->level : c->advLevel;                  /* a referenced CDict brings its own level (:5836) */
     return zb_compressOne(c, dst, dstCapacity, src, srcSize, cd, level, c->advChecksum != 0, c->advNoDictID != 0, zb_ldmArg(c));
 }
@@ -1125,7 +1085,7 @@ static size_t zb_compressSeqs(ZSTD_CCtx* c, void* dst, size_t dstCapacity, const
     ZbDeviceGuard guard;
     TRY(zb_ctxInit(c));
     memset(&c->stats, 0, sizeof(c->stats));
-    const ZSTD_CDict* const cdArg = c->advRefCDict ? c->advRefCDict : c->advLocalDict;
+    const ZSTD_CDict* const cdArg = c->advRefCDict ? c->advRefCDict : c->advLocalDict.get();
     int const level = c->advRefCDict ? c->advRefCDict->level : c->advLevel;
     ZSTD_CDict* const cd = (cdArg && cdArg->size >= 8) ? const_cast<ZSTD_CDict*>(cdArg) : NULL;
     if (g_strictLevels && level > 4) return ZB_ERR(ZB_error_parameter_unsupported);
@@ -1155,7 +1115,7 @@ static size_t zb_compressSeqs(ZSTD_CCtx* c, void* dst, size_t dstCapacity, const
     u64 ctrl[4] = { 0, 0, ~0ull, 0 };
     CK(cudaMemcpyAsync(c->d_seqCtrl, ctrl, sizeof(ctrl), cudaMemcpyHostToDevice, st));
     CK(cudaStreamSynchronize(st));                                 /* the pageable sources above are staged */
-    CK(cudaEventRecord(c->evK0, st));
+    CK(cudaEventRecord(c->ev[EV_K0], st));
     /* K1s-a */
     u32 const nbTiles = (u32)((n + 1023) / 1024);
     TRY(c->d_seqTile.ensure((size_t)nbTiles * 12 + 16));
@@ -1216,28 +1176,28 @@ static size_t zb_compressSeqs(ZSTD_CCtx* c, void* dst, size_t dstCapacity, const
     for (u32 w = 0; w < nbWaves; w++) {
         u32 const b0 = w * waveBlocks, nb = (b0 + waveBlocks <= nbBlocks) ? waveBlocks : nbBlocks - b0;
         CK(zb_launch_seq_convert(d_src, c->d_blocks + b0, nb, d_first + b0, d_firstPos + b0, d_seqs, (u32)n, &prm, &sd, c->d_seqs, c->d_lits, c->d_meta, st));
-        if (w == 0) CK(cudaEventRecord(c->evK1, st));
-        CK(zb_launch_literals(c->d_blocks + b0, nb, &prm, &sd, de ? cd->d_de : NULL, c->d_lits, c->d_body, c->d_meta, st));
-        if (timed) CK(cudaEventRecord(c->evK2, st));
-        CK(zb_launch_sequences(d_src, c->d_blocks + b0, nb, &prm, &sd, de ? cd->d_de : NULL, c->d_seqs, c->d_dist, c->d_body, c->d_meta, st));
-        if (timed) CK(cudaEventRecord(c->evK3, st));
+        if (w == 0) CK(cudaEventRecord(c->ev[EV_K1], st));
+        CK(zb_launch_literals(c->d_blocks + b0, nb, &prm, &sd, de ? cd->d_de.p : NULL, c->d_lits, c->d_body, c->d_meta, st));
+        if (timed) CK(cudaEventRecord(c->ev[EV_K2], st));
+        CK(zb_launch_sequences(d_src, c->d_blocks + b0, nb, &prm, &sd, de ? cd->d_de.p : NULL, c->d_seqs, c->d_dist, c->d_body, c->d_meta, st));
+        if (timed) CK(cudaEventRecord(c->ev[EV_K3], st));
         CK(zb_launch_stitch(d_src, c->d_blocks + b0, nb, c->d_frames, c->d_body, sd.body, c->d_meta, c->d_outOffsets + b0,
                             w > 0 ? c->d_totals + (w - 1) : NULL, c->d_totals + w, d_out, outCap, st));
         launches += 5;
     }
     if (c->advChecksum) { CK(zb_launch_checksums(d_src, c->d_frames, 1, c->d_outOffsets, d_out, outCap, st)); launches++; }
-    CK(cudaEventRecord(c->evKEnd, st));
+    CK(cudaEventRecord(c->ev[EV_KEND], st));
     u64 total = 0;
     CK(cudaMemcpyAsync(&total, c->d_totals + nbWaves - 1, sizeof(u64), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     if (!deviceMemory && total <= dstCapacity) CK(cudaMemcpy(dst, d_out, total, cudaMemcpyDeviceToHost));
     float ms = 0;
-    cudaEventElapsedTime(&ms, c->evK0, c->evKEnd); c->stats.kernel_ms = ms; c->stats.total_ms = ms;
-    cudaEventElapsedTime(&ms, c->evK0, c->evK1); c->stats.match_ms = ms;     /* the first wave's import */
+    cudaEventElapsedTime(&ms, c->ev[EV_K0], c->ev[EV_KEND]); c->stats.kernel_ms = ms; c->stats.total_ms = ms;
+    cudaEventElapsedTime(&ms, c->ev[EV_K0], c->ev[EV_K1]); c->stats.match_ms = ms;     /* the first wave's import */
     if (timed) {
-        cudaEventElapsedTime(&ms, c->evK1, c->evK2); c->stats.literals_ms = ms;
-        cudaEventElapsedTime(&ms, c->evK2, c->evK3); c->stats.sequences_ms = ms;
-        cudaEventElapsedTime(&ms, c->evK3, c->evKEnd); c->stats.stitch_ms = ms;
+        cudaEventElapsedTime(&ms, c->ev[EV_K1], c->ev[EV_K2]); c->stats.literals_ms = ms;
+        cudaEventElapsedTime(&ms, c->ev[EV_K2], c->ev[EV_K3]); c->stats.sequences_ms = ms;
+        cudaEventElapsedTime(&ms, c->ev[EV_K3], c->ev[EV_KEND]); c->stats.stitch_ms = ms;
     }
     c->stats.launches = launches; c->stats.nbBlocks = nbBlocks;
     if (!deviceMemory) { c->stats.h2d_bytes = srcSize + seqBytes; c->stats.d2h_bytes = total <= dstCapacity ? (size_t)total : 0; }

@@ -214,6 +214,8 @@ typedef struct { const u64* match; const u64* first; const u32* cnt; } ZbLdmView
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdlib.h>
+#include <utility>
+#include <vector>
 
 static inline bool zb_isErr(size_t c) { return c > ZB_ERR(ZB_error_maxCode); }
 
@@ -247,24 +249,38 @@ template <typename T, bool Pinned> struct ZbBuf {
 template <typename T> using ZbDevBuf = ZbBuf<T, false>;
 template <typename T> using ZbHostBuf = ZbBuf<T, true>;
 
-/* a context's stream and events */
-static inline void zb_streamDestroy(cudaStream_t st, const cudaEvent_t* ev, int nbEvents)
-{
-    for (int i = 0; i < nbEvents; i++) if (ev[i]) cudaEventDestroy(ev[i]);
-    if (st) cudaStreamDestroy(st);
-}
-/* creates a non-blocking stream and nbEvents events on `dev`, all or nothing: after a failure none of them is left */
-static inline size_t zb_streamCreate(int dev, cudaStream_t* st, cudaEvent_t* ev, int nbEvents)
-{
-    CK(cudaSetDevice(dev));
-    *st = nullptr;
-    for (int i = 0; i < nbEvents; i++) ev[i] = nullptr;
-    cudaError_t e = cudaStreamCreateWithFlags(st, cudaStreamNonBlocking);
-    for (int i = 0; i < nbEvents && e == cudaSuccess; i++) e = cudaEventCreate(&ev[i]);
-    if (e != cudaSuccess) zb_streamDestroy(*st, ev, nbEvents);
-    CK(e);
-    return 0;
-}
+/* A non-blocking stream that a context owns, created by ensure() and destroyed with its owner.  Move-assignable, so that a
+ * context can take over a stream that was created together with its events, all or nothing. */
+struct ZbStream {
+    cudaStream_t s = nullptr;
+    ZbStream() = default;
+    ZbStream& operator=(ZbStream&& o) { std::swap(s, o.s); return *this; }
+    ~ZbStream() { if (s) cudaStreamDestroy(s); }
+    size_t ensure() { if (!s) CK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking)); return 0; }
+    operator cudaStream_t() const { return s; }
+};
+
+/* Events that a context owns, all timed or all untimed.  ensure(n, timed) keeps them until a call needs more of them or the
+ * other kind; they are destroyed with their owner. */
+struct ZbEvents {
+    std::vector<cudaEvent_t> ev; bool timed = false;
+    ZbEvents() = default;
+    ZbEvents& operator=(ZbEvents&& o) { ev.swap(o.ev); std::swap(timed, o.timed); return *this; }
+    ~ZbEvents() { release(); }
+    void release() { for (cudaEvent_t e : ev) cudaEventDestroy(e); ev.clear(); }
+    size_t ensure(size_t n, bool timing) {
+        if (n <= ev.size() && timing == timed) return 0;
+        release();
+        timed = timing;
+        while (ev.size() < n) {
+            cudaEvent_t e;
+            CK(cudaEventCreateWithFlags(&e, timing ? cudaEventDefault : cudaEventDisableTiming));
+            ev.push_back(e);
+        }
+        return 0;
+    }
+    cudaEvent_t operator[](size_t i) const { return ev[i]; }
+};
 
 /* restores the calling thread's current device when a call returns (a context works on the device it was created for) */
 struct ZbDeviceGuard {
@@ -272,6 +288,19 @@ struct ZbDeviceGuard {
     ZbDeviceGuard() : prev(-1) { if (cudaGetDevice(&prev) != cudaSuccess) { prev = -1; cudaGetLastError(); } }
     ~ZbDeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
 };
+
+/* deletes a context or digested dictionary on its device, where its members free what they own.  One that never reached a
+ * device (device < 0) is deleted without a device switch: it holds nothing there, so its deletion makes no CUDA call (but
+ * for the arrays a CDict's failed first upload left, which free themselves) */
+template <typename T> static inline size_t zb_deleteOnDevice(T* x)
+{
+    if (!x) return 0;
+    if (x->device < 0) { delete x; return 0; }
+    ZbDeviceGuard guard;
+    cudaSetDevice(x->device);
+    delete x;
+    return 0;
+}
 
 /* the device a new context belongs to, chosen when it is created (zb_api.cu): ZSTDB200_setDevice's value, else the calling
  * thread's current device */
