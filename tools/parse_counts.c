@@ -1,0 +1,145 @@
+/* parse_counts.c — dynamic counts of the fast greedy parse (K1b, zb_parse_kernel) on one input, CPU only.
+ *
+ *   make -C oracle oracle && cc -O2 -o /tmp/parse_counts tools/parse_counts.c -Loracle -lzb_oracle -Wl,-rpath,$PWD/oracle
+ *   oracle/_ref/datagen -g256MB -P50 > /tmp/p50 && /tmp/parse_counts /tmp/p50 1
+ *
+ * The input is compressed as one frame.  The candidates come from the oracle's walk (zbo_walkChunk, bit-exact with
+ * K1a); the parse below makes the same steps, lanes and winners as parse_fast_segment in oracle/zb_match.c (the rule
+ * both the kernel and the oracle follow) and counts, per segment, what the kernel does on its way:
+ *   steps             probe steps (32 lanes each);
+ *   hits by type      repcode 2 (lane 0 at the anchor), repcode 1, table;
+ *   tried             table lanes the kernel tries: a lane whose repcodes failed and whose candidate is non-zero and, if
+ *                     below 0xFFFF, does not reach in front of the history — the far ones are tried whatever their reach;
+ *   tag false         tried lanes whose first 4 bytes differ (the walk only checks an 11-bit tag);
+ *   far               tried lanes with a distance >= 0xFFFF (the kernel fetches the 32-bit distance for each), far winners;
+ *   fwd rounds        256-byte rounds of forward compares per match (floor(counted / 256) + 1, counted from the probe for
+ *                     a table hit, from probe + 4 for a repcode hit);
+ *   back rounds       32-byte rounds of backward catch-up per match (floor(back / 32) + 1);
+ *   back > 4          matches whose catch-up exceeds 4 bytes (the in-lane repcode-1 catch-up of the kernel before stopped there).
+ * From these it prints the dependent memory round trips per segment of the kernel before and after the change that
+ * gave each step one round trip (DESIGN.md section 2, K1b). */
+#include <stdio.h>
+#include <stdlib.h>
+#include <string.h>
+#include "../oracle/zb_oracle.h"
+
+static u32 rd32(const u8* p) { u32 v; memcpy(&v, p, 4); return v; }
+static size_t count_eq(const u8* a, const u8* b, const u8* end) { const u8* s = a; while (a < end && *a == *b) { a++; b++; } return (size_t)(a - s); }
+
+typedef struct {
+    double segs, steps, matches, h3, h2, h1, tried, tagFalse, farTried, farLost, farWon, fwdRounds, backRounds, back4,
+           fwdExtra, backExtra, backRoundsTable, rep1Coop;
+} counts;
+
+static void parse_segment(const zbo_plan* plan, const u8* frame, const u32* dist, size_t bs, size_t be, size_t ss, size_t se,
+                          size_t lowLimit, counts* c)
+{
+    size_t ip = ss, anchor = ss, searchStart = ss;
+    u32 rep1 = 0, rep2 = 0;
+    c->segs++;
+    while (ip < se && ip + 8 <= be) {
+        u32 const step = plan->stepSize + (u32)((ip - searchStart) >> 7);
+        int winner = -1, wtype = 0, l;
+        size_t probe = 0; u32 offset = 0;
+        c->steps++;
+        for (l = 0; l < (int)ZB_WARP && winner < 0; l++) {
+            size_t const p = ip + (size_t)(l >> 1) * step + (size_t)(l & 1);
+            u32 cur, d;
+            if (p >= se || p + 8 > be) break;
+            cur = rd32(frame + p);
+            d = dist[p - bs];
+            if (l == 0 && ip == anchor && rep2 && rd32(frame + p - rep2) == cur) { winner = l; wtype = 3; probe = p; offset = rep2; }
+            else if (rep1 && p >= lowLimit + rep1 && rd32(frame + p - rep1) == cur) { winner = l; wtype = 2; probe = p; offset = rep1; }
+            else if (d && (d >= 0xFFFFu || p >= lowLimit + d)) {
+                c->tried++;
+                if (d >= 0xFFFFu) c->farTried++;
+                if (p < lowLimit + d) { c->farLost++; continue; }
+                if (rd32(frame + p - d) != cur) { c->tagFalse++; continue; }
+                winner = l; wtype = 1; probe = p; offset = d;
+                if (d >= 0xFFFFu) c->farWon++;
+            }
+        }
+        if (winner < 0) { ip += (size_t)(ZB_WARP / 2) * step; continue; }
+        {   size_t ms = probe, mm = probe - offset, mlen, fwd, back;
+            if (wtype != 3)
+                while (ms > anchor && mm > lowLimit && frame[ms - 1] == frame[mm - 1]) { ms--; mm--; }
+            fwd = count_eq(frame + probe + 4, frame + probe - offset + 4, frame + be);
+            mlen = (probe - ms) + 4 + fwd;
+            back = probe - ms;
+            c->matches++;
+            if (wtype == 3) c->h3++; else if (wtype == 2) c->h2++; else c->h1++;
+            {   size_t const counted = (wtype == 1) ? fwd + 4 : fwd;
+                c->fwdRounds += (double)(counted / 256 + 1);
+                c->fwdExtra += (double)(counted / 256);
+            }
+            c->backRounds += (double)(back / 32 + 1);
+            c->backExtra += (double)(back / 32);
+            if (wtype == 1) c->backRoundsTable += (double)(back / 32 + 1);
+            if (back > 4) { c->back4++; if (wtype == 2) c->rep1Coop += (double)((back - 4) / 32 + 1); }
+            if (wtype == 3) { u32 const t = rep2; rep2 = rep1; rep1 = t; }
+            else if (wtype == 1) { rep2 = rep1; rep1 = offset; }
+            ip = ms + mlen; anchor = ip; searchStart = ip;
+        }
+    }
+}
+
+int main(int argc, char** argv)
+{
+    FILE* f;
+    u8* src;
+    size_t n, bs;
+    int level = argc > 2 ? atoi(argv[2]) : 1;
+    zbo_cparams cp;
+    zbo_plan plan;
+    zbo_chunkCand cc;
+    counts c;
+    if (argc < 2) { fprintf(stderr, "usage: %s <input> [level]\n", argv[0]); return 2; }
+    f = fopen(argv[1], "rb");
+    if (!f) { perror(argv[1]); return 1; }
+    fseek(f, 0, SEEK_END); n = (size_t)ftell(f); fseek(f, 0, SEEK_SET);
+    src = (u8*)malloc(n + 16);
+    if (fread(src, 1, n, f) != n) { fprintf(stderr, "short read\n"); return 1; }
+    fclose(f);
+    cp = zbo_getCParams(level, n, 0);
+    if (cp.strategy != 1) { fprintf(stderr, "level %d is not the fast strategy\n", level); return 2; }
+    zbo_makePlan(&plan, &cp);
+    memset(&c, 0, sizeof c);
+    memset(&cc, 0, sizeof cc);
+    {   size_t const chunkBytes = (size_t)plan.chunkBlocks * ZB_BLOCK_MAX;
+        for (bs = 0; bs < n; bs += ZB_BLOCK_MAX) {
+            size_t const be = bs + ZB_BLOCK_MAX < n ? bs + ZB_BLOCK_MAX : n, W = (size_t)1 << plan.windowLog;
+            size_t lowLimit, ss;
+            if (bs % chunkBytes == 0) {
+                size_t const ce = bs + chunkBytes < n ? bs + chunkBytes : n;
+                zbo_freeChunk(&cc);
+                zbo_walkChunk(&plan, src, n, bs, ce, &cc);
+            }
+            if (be - bs < 7) continue;                           /* raw block, no parse */
+            lowLimit = cc.low;                                   /* oracle/zb_match.c block_low */
+            if (be > W && be - W > lowLimit) lowLimit = be - W;
+            for (ss = bs; ss < be; ss += ZB_PARSE_SEG)
+                parse_segment(&plan, src, cc.dS + (bs - cc.start), bs, be, ss, ss + ZB_PARSE_SEG < be ? ss + ZB_PARSE_SEG : be, lowLimit, &c);
+        }
+        zbo_freeChunk(&cc);
+    }
+    {   double const S = c.segs, M = c.matches;
+        /* before: 2 round trips per step (the dist row, then the windows and the far distance); per match the forward
+         * rounds and the backward rounds of a table hit or of a repcode-1 hit with more than 4 bytes of catch-up, plus one
+         * for the repcode-1 in-lane catch-up's window; one forward round per tried false positive.
+         * after: 1 per step, 1 per far lane tried; per match and per tried false positive the first forward and backward
+         * rounds, which go out together but wait twice in the sm_90a SASS (the compare of the current window is scheduled
+         * before the loads of the candidate window and of the catch-up bytes), then the extra rounds of each */
+        double const rtOld = 2 * c.steps + c.fwdRounds + c.backRoundsTable + c.h2 + c.rep1Coop + c.tagFalse;
+        double const rtNew = c.steps + c.farTried + 2 * (M + c.tagFalse) + c.fwdExtra + c.backExtra;
+        printf("{\"input_bytes\": %zu, \"level\": %d, \"segments\": %.0f, \"per_segment\": {\"steps\": %.2f, \"matches\": %.2f, "
+               "\"rep2\": %.2f, \"rep1\": %.2f, \"table\": %.2f, \"tried\": %.2f, \"tag_false\": %.3f, \"far_tried\": %.3f, "
+               "\"far_out_of_reach\": %.3f, \"far_won\": %.3f, \"back_gt4\": %.2f, \"fwd_rounds\": %.2f, \"back_rounds\": %.2f}, "
+               "\"per_match\": {\"steps\": %.3f, \"fwd_rounds\": %.3f, \"back_rounds\": %.3f}, "
+               "\"round_trips_per_segment\": {\"before\": %.1f, \"after\": %.1f}}\n",
+               n, level, S, c.steps / S, M / S, c.h3 / S, c.h2 / S, c.h1 / S, c.tried / S, c.tagFalse / S, c.farTried / S,
+               c.farLost / S, c.farWon / S, c.back4 / S, c.fwdRounds / S, c.backRounds / S,
+               c.steps / M, c.fwdRounds / M, c.backRounds / M, rtOld / S, rtNew / S);
+    }
+    free(src);
+    return 0;
+}

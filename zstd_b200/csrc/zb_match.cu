@@ -387,7 +387,6 @@ zb_parse_kernel(const u8* __restrict__ src, const u8* __restrict__ dictEnd, cons
     u32 const b = g / segs, k = g % segs;
     if (b >= nbBlocks) return;
     ZbBlock const bd = blocks[b];
-    u64* const myseq = seqs + (size_t)b * sd.seq + (size_t)k * (ZB_PARSE_SEG / 4u);
     const u16* const mydist = dist + (size_t)b * sd.dist;
     const u32* const myfar = far + (size_t)b * sd.dist;
     const u8* const base = src + bd.srcOff - bd.histLen;          /* base + rel addresses the frame's own bytes */
@@ -411,66 +410,70 @@ zb_parse_kernel(const u8* __restrict__ src, const u8* __restrict__ dictEnd, cons
     u32 const se = min(ss + ZB_PARSE_SEG, blockEnd);
     u32 const be = blockEnd;
 
-    u32 ip = ss, anchor = ss, searchStart = ss;
+    u32 ip = ss, anchor = ss;                                  /* the search restarts at the anchor: it is searchStart too */
     u32 rep1 = 0, rep2 = 0, nbSeq = 0;
     if ((bd.flags & ZB_FLAG_FIRST) && k == 0u) { rep1 = prm.startRep[0]; rep2 = prm.startRep[1]; }   /* a zstd-format dictionary's repcodes, zstd_compress.c:5054-5056 */
 
+    /* the 4 bytes at rel position x; x + 8 <= be */
+    auto ld4 = [&](u32 x) { return DICT ? (u32)zb_seg_ld64x<DICT>(sg, x) : zb_ld32w2(sg.hi + x); };
     while (ip < se && ip + 8u <= be) {
-        u32 const step = prm.stepSize + ((ip - searchStart) >> 7);           /* kSearchStrength = 8 */
+        u32 const step = prm.stepSize + ((ip - anchor) >> 7);                /* kSearchStrength = 8 */
         u32 const p = ip + (lane >> 1) * step + (lane & 1u);
         bool const act = (p < se) && (p + 8u <= be);
         u32 const pp = act ? p : ip;                         /* a position every lane may load from (ip + 8 <= be) */
-        /* the candidate row and the windows are independent loads: all of them go out before the first is looked at (the
-         * rare far distance costs one more round trip, below) */
+        /* one round trip per step: the candidate row, the current window and both repcode windows are independent loads
+         * and all go out before the first is looked at.  dist[] only holds tag-verified candidates, so a step needs no
+         * random load: every window is contiguous across lanes.  A far distance (d16 == ZB_FAR) counts as a table
+         * candidate here; its 32-bit value is fetched only when its lane is tried, below */
         u32 const d16 = act ? (u32)mydist[pp - bs] : 0u;
         bool const v3 = (lane == 0u) && (ip == anchor) && (rep2 != 0u);
         bool const v2 = act && rep1 != 0u && p >= rep1;
-        /* dist[] only holds tag-verified candidates, so a step needs no random load: the current window and the
-         * repcode window are contiguous across lanes.  The repcode window's 4 bytes in front of the position are only
-         * needed by a lane whose repcode matched: asked for there */
-        u32 pre, cur;
-        zb_seg_pre_cur<DICT>(sg, pp, &pre, &cur);
-        u32 const cur2 = DICT ? zb_seg_ld32<DICT>(sg, v2 ? pp - rep1 : pp) : zb_ld32w2(sg.hi + (v2 ? pp - rep1 : pp));
+        u32 const cur = ld4(pp);
+        u32 const cur2 = ld4(v2 ? pp - rep1 : pp);
         u32 cur3 = ~cur;
-        if (ip == anchor && rep2 != 0u) cur3 = (u32)zb_seg_ld64x<DICT>(sg, v3 ? pp - rep2 : pp);     /* warp-uniform condition */
-        u32 const d = d16 == ZB_FAR ? myfar[pp - bs] : d16;
-        bool const v1 = act && d != 0u && p >= d;
+        if (ip == anchor && rep2 != 0u) cur3 = ld4(v3 ? pp - rep2 : pp);      /* warp-uniform condition */
+        bool const v1 = act && d16 != 0u && (d16 == ZB_FAR || p >= d16);
         u32 const hit = (v3 && cur3 == cur) ? 3u : ((v2 && cur2 == cur) ? 2u : (v1 ? 1u : 0u));
-        /* backward catch-up (zstd_fast.c:387-391) of a repcode-1 hit: first 4 bytes in-lane from the windows */
-        u32 myback = 0, mymore = 0;
-        if (hit == 2u) {
-            u32 pre2, unused;
-            zb_seg_pre_cur<DICT>(sg, p - rep1, &pre2, &unused);
-            u32 const x = pre ^ pre2;
-            u32 const bm = x ? ((u32)__clz((int)x) >> 3) : 4u;
-            u32 lim = p - anchor; lim = lim < 4u ? lim : 4u;
-            u32 const src0 = p - rep1; lim = lim < src0 ? lim : src0;
-            myback = bm < lim ? bm : lim;
-            mymore = (bm == 4u && lim == 4u) ? 1u : 0u;
-        }
+        u32 const hd = (d16 << 2) | hit;                     /* what the winner's lane hands out: one register through the tries */
         u32 tent = __ballot_sync(ZB_FULL, hit != 0u);
-        /* lowest lane first.  A table hit (type 1) is only tag-verified by K1a: its bytes are checked while
-         * the match is extended (one round trip, this lane only); a false positive drops out and the next
-         * lane is tried — the result is "lowest lane whose hit is real", what the oracle computes. */
+        /* lowest lane first.  A table hit (type 1) is only tag-verified by K1a: its bytes are checked while the match is
+         * extended; a false positive drops out and the next lane is tried — the result is "lowest lane whose hit is real",
+         * what the oracle computes.  So does a far candidate that reaches in front of the history (a lane whose repcodes
+         * had matched would not be a type-1 hit). */
         u32 probe = 0, wtype = 0, offset = 0, back = 0, fwdFrom4 = 0;
         bool found = false;
         while (tent) {
-            int const winner = __ffs((int)tent) - 1;
-            probe = __shfl_sync(ZB_FULL, p, winner);
-            wtype = __shfl_sync(ZB_FULL, hit, winner);
-            u32 const wd = __shfl_sync(ZB_FULL, d, winner);
-            back = __shfl_sync(ZB_FULL, myback, winner);
-            u32 more = __shfl_sync(ZB_FULL, mymore, winner);
-            offset = (wtype == 3u) ? rep2 : ((wtype == 2u) ? rep1 : wd);
-            if (wtype == 1u) {
-                u32 const f0 = zb_count_fwd<DICT>(sg, probe, offset, be, lane);          /* from the probe itself */
-                if (f0 < 4u) { tent &= ~(1u << winner); continue; }                   /* tag collision */
-                fwdFrom4 = f0 - 4u;
-                more = 1u;
-            } else {
-                fwdFrom4 = zb_count_fwd<DICT>(sg, probe + 4u, offset, be, lane);
+            u32 const winner = (u32)__ffs((int)tent) - 1u;
+            probe = ip + (winner >> 1) * step + (winner & 1u);
+            u32 const w = __shfl_sync(ZB_FULL, hd, winner);
+            wtype = w & 3u;
+            offset = (wtype == 3u) ? rep2 : ((wtype == 2u) ? rep1 : w >> 2);
+            if (wtype == 1u && offset == ZB_FAR) {                                /* rare: one more round trip */
+                offset = myfar[probe - bs];
+                if (probe < offset) { tent &= tent - 1u; continue; }
             }
-            if (more) back += zb_back_coop<DICT>(sg, probe - back, offset, anchor, lane);   /* table hit, or a repcode hit with > 4 bytes of catch-up */
+            /* one round trip for the first forward round and the first backward round (zstd_fast.c:387-391) together: a
+             * table hit is counted from the probe itself (its first 4 bytes are not verified yet), a repcode hit from
+             * probe + 4.  A repcode-2 hit sits at the anchor: it has nothing to catch up */
+            u32 const a = (wtype == 1u) ? probe : probe + 4u;
+            u32 const kb = lane + 1u;                     /* backward: bytes probe - kb and probe - offset - kb */
+            bool const bIn = (probe >= anchor + kb) && (probe >= offset + kb);
+            u32 const b0 = bIn ? zb_seg_byte<DICT>(sg, probe - kb) : 0u;
+            u32 const b1 = bIn ? zb_seg_byte<DICT>(sg, probe - offset - kb) : 0u;
+            u32 const pa = a + 8u * lane;                 /* forward: this lane's 8 bytes, read at q so that no lane branches */
+            u32 const q = min(pa, be - 8u);               /* (probe + 8 <= be, so q >= probe >= offset) */
+            u64 const xf = zb_seg_ld64x<DICT>(sg, q) ^ zb_seg_ld64x<DICT>(sg, q - offset);
+            u64 const xs = xf >> (8u * min(pa - q, 7u));
+            u32 m = xs ? (u32)((__ffsll((long long)xs) - 1) >> 3) : 8u;
+            m = pa >= be ? 0u : min(m, be - pa);
+            u32 const okb = __ballot_sync(ZB_FULL, bIn && b0 == b1);
+            u32 const inc = __ballot_sync(ZB_FULL, m != 8u);
+            u32 fwd;
+            if (inc == 0u) fwd = 256u + zb_count_fwd<DICT>(sg, a + 256u, offset, be, lane);
+            else { int const f = __ffs((int)inc) - 1; fwd = 8u * (u32)f + __shfl_sync(ZB_FULL, m, f); }
+            if (wtype == 1u && fwd < 4u) { tent &= tent - 1u; continue; }      /* tag collision */
+            fwdFrom4 = (wtype == 1u) ? fwd - 4u : fwd;
+            back = (okb == ZB_FULL) ? 32u + zb_back_coop<DICT>(sg, probe - 32u, offset, anchor, lane) : (u32)(__ffs((int)~okb) - 1);
             found = true;
             break;
         }
@@ -479,11 +482,12 @@ zb_parse_kernel(const u8* __restrict__ src, const u8* __restrict__ dictEnd, cons
         u32 const mlen = back + 4u + fwdFrom4;
         if (wtype == 3u) { u32 const t = rep2; rep2 = rep1; rep1 = t; }
         else if (wtype == 1u) { rep2 = rep1; rep1 = offset; }
-        if (lane == 0) myseq[nbSeq] = zb_pack_raw(offset, mlen, ms - bs);
+        if (lane == 0) seqs[(size_t)b * sd.seq + k * (ZB_PARSE_SEG / 4u) + nbSeq] = zb_pack_raw(offset, mlen, ms - bs);   /* the address is rebuilt per match: it would not stay in a register */
         nbSeq++;
-        ip = ms + mlen; anchor = ip; searchStart = ip;
+        ip = ms + mlen; anchor = ip;
     }
-    if (lane == 0) { ZbSegMeta z; z.nbSeq = nbSeq; z.pad[0] = z.pad[1] = z.pad[2] = 0; segmeta[(size_t)b * segs + k] = z; }
+    /* b * segs + k = g, recomputed: nothing of the record's address stays live through the loop */
+    if (lane == 0) { ZbSegMeta z; z.nbSeq = nbSeq; z.pad[0] = z.pad[1] = z.pad[2] = 0; segmeta[blockIdx.x * PARSE_WARPS + (threadIdx.x >> 5)] = z; }
 }
 
 /* ------------------------------------------------------------------------------------------------
