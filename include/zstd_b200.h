@@ -177,6 +177,46 @@ ZSTDB200_API size_t     ZSTD_decompress_usingDict(ZSTD_DCtx* dctx, void* dst, si
 /* lib/zstd.h:195-227 — header readers (host code).  ZSTD_CONTENTSIZE_UNKNOWN = (0ULL - 1), ZSTD_CONTENTSIZE_ERROR = (0ULL - 2). */
 ZSTDB200_API unsigned long long ZSTD_getFrameContentSize(const void* src, size_t srcSize);
 ZSTDB200_API size_t     ZSTD_findFrameCompressedSize(const void* src, size_t srcSize);
+/* lib/zstd.h:1120 — the dictionary ID a frame names (host code): 0 when it names none, for a skippable frame, and when the
+ * header can not be read (too short, not a frame). */
+ZSTDB200_API unsigned   ZSTD_getDictID_fromFrame(const void* src, size_t srcSize);
+
+/* lib/zstd.h:1000-1030 — digested dictionary of the decoder.  ZSTD_createDDict copies and parses the dictionary on the host
+ * (no GPU is needed to create or query one); its first use uploads it whole (header and content) to the device of the
+ * context using it, where it stays resident: later calls with it make no copy and no synchronisation for the dictionary.
+ * Any number of contexts on that one device may use it; a context on another device gets ZSTD_error_parameter_unsupported
+ * (40).  ZSTD_createDDict returns NULL for a zstd-format dictionary with corrupted entropy tables, and also where this
+ * decoder refuses more than the reference: a Huffman tree description with a table log above 11 (the reference's limit is
+ * 12), or whose weights' FSE description gives a probability to a symbol above 12; it accepts Huffman weights with fewer
+ * than two 1s, which the reference refuses (DESIGN.md section 4).  ZSTD_freeDDict
+ * accepts NULL.  ZSTD_decompress_usingDDict with NULL decodes without a dictionary. */
+typedef struct ZSTD_DDict_s ZSTD_DDict;
+ZSTDB200_API ZSTD_DDict* ZSTD_createDDict(const void* dictBuffer, size_t dictSize);
+ZSTDB200_API size_t      ZSTD_freeDDict(ZSTD_DDict* ddict);
+ZSTDB200_API size_t      ZSTD_decompress_usingDDict(ZSTD_DCtx* dctx, void* dst, size_t dstCapacity, const void* src, size_t srcSize,
+                                                    const ZSTD_DDict* ddict);
+ZSTDB200_API unsigned    ZSTD_getDictID_fromDDict(const ZSTD_DDict* ddict);                  /* lib/zstd.h:1113 */
+
+/* lib/zstd.h:609-650, 1160-1210 (zstd_decompress.c:1697-1960) — the context's sticky dictionary and parameters, used by
+ * ZSTD_decompressDCtx (hence ZSTD_decompressStream) and ZSTDB200_decompressDevice.  ZSTD_DCtx_loadDictionary copies and
+ * digests the dictionary (a corrupted one returns ZSTD_error_memory_allocation, 64, as in the reference), ZSTD_DCtx_refDDict
+ * borrows a DDict (NULL: none); both are sticky.  ZSTD_DCtx_refPrefix borrows raw content for the next call only (in
+ * streaming: the next frame).  Each replaces what was there.
+ * ZSTD_d_windowLogMax: 0 means the default 27; [10, 31], else ZSTD_error_parameter_outOfBound (42).  As in the reference it
+ * applies to ZSTD_decompressStream only, which refuses a frame whose window (at least 1 KiB; a Single_Segment frame's is
+ * its content size) is larger with ZSTD_error_frameParameter_windowTooLarge (16), decided from its header.  A frame that
+ * arrives whole with one call whose output buffer has room for its content size is decoded in one pass, without the limit,
+ * as the reference does.  Windows above 2^27 stay refused everywhere.  Other parameters return
+ * ZSTD_error_parameter_unsupported (40).
+ * ZSTD_DCtx_reset: ZSTD_reset_session_only drops an unfinished stream and keeps dictionary and parameters;
+ * ZSTD_reset_parameters drops both.  ZSTD_initDStream drops the dictionary too.  Setting a parameter or a dictionary (or
+ * resetting parameters) while ZSTD_decompressStream is inside a frame returns ZSTD_error_stage_wrong (60). */
+typedef enum { ZSTD_d_windowLogMax = 100 } ZSTD_dParameter;
+ZSTDB200_API size_t ZSTD_DCtx_setParameter(ZSTD_DCtx* dctx, ZSTD_dParameter param, int value);
+ZSTDB200_API size_t ZSTD_DCtx_reset(ZSTD_DCtx* dctx, ZSTD_ResetDirective reset);
+ZSTDB200_API size_t ZSTD_DCtx_loadDictionary(ZSTD_DCtx* dctx, const void* dict, size_t dictSize);
+ZSTDB200_API size_t ZSTD_DCtx_refDDict(ZSTD_DCtx* dctx, const ZSTD_DDict* ddict);
+ZSTDB200_API size_t ZSTD_DCtx_refPrefix(ZSTD_DCtx* dctx, const void* prefix, size_t prefixSize);
 
 /* lib/zstd.h:880-924 — streaming decompression.  Whole frames are decoded on the GPU: compressed bytes are collected in
  * the context until a frame is complete, then decoded and handed out as the caller makes room.  Returns 0 when a frame has

@@ -136,6 +136,27 @@ def lib() -> ctypes.CDLL:
         L.ZSTDB200_decompressDevice.argtypes = [_vp, _vp, _sz, _vp, _sz, _vp]
         L.ZSTDB200_getLastDStats.restype = None
         L.ZSTDB200_getLastDStats.argtypes = [_vp, ctypes.POINTER(DStats)]
+    if hasattr(L, "ZSTD_createDDict"):                                                  # absent from older development builds
+        L.ZSTD_createDDict.restype = _vp
+        L.ZSTD_createDDict.argtypes = [_vp, _sz]
+        L.ZSTD_freeDDict.restype = _sz
+        L.ZSTD_freeDDict.argtypes = [_vp]
+        L.ZSTD_decompress_usingDDict.restype = _sz
+        L.ZSTD_decompress_usingDDict.argtypes = [_vp, _vp, _sz, _vp, _sz, _vp]
+        L.ZSTD_getDictID_fromDDict.restype = ctypes.c_uint
+        L.ZSTD_getDictID_fromDDict.argtypes = [_vp]
+        L.ZSTD_getDictID_fromFrame.restype = ctypes.c_uint
+        L.ZSTD_getDictID_fromFrame.argtypes = [_vp, _sz]
+        L.ZSTD_DCtx_setParameter.restype = _sz
+        L.ZSTD_DCtx_setParameter.argtypes = [_vp, ctypes.c_int, ctypes.c_int]
+        L.ZSTD_DCtx_reset.restype = _sz
+        L.ZSTD_DCtx_reset.argtypes = [_vp, ctypes.c_int]
+        L.ZSTD_DCtx_loadDictionary.restype = _sz
+        L.ZSTD_DCtx_loadDictionary.argtypes = [_vp, _vp, _sz]
+        L.ZSTD_DCtx_refDDict.restype = _sz
+        L.ZSTD_DCtx_refDDict.argtypes = [_vp, _vp]
+        L.ZSTD_DCtx_refPrefix.restype = _sz
+        L.ZSTD_DCtx_refPrefix.argtypes = [_vp, _vp, _sz]
     _lib = L
     return L
 
@@ -343,8 +364,36 @@ def sequence_bound(src_size: int) -> int:
     return int(lib().ZSTD_sequenceBound(src_size))
 
 
+class ZSTD_DDict:
+    """Digested dictionary of the decoder (lib/zstd.h:1000-1030): parsed on the host when created, resident on the GPU from
+    its first use.  Raises ZstdError(30) for a zstd-format dictionary whose entropy tables the decoder refuses."""
+
+    def __init__(self, dict_bytes):
+        p, n, keep = _buf(dict_bytes)
+        self._h = lib().ZSTD_createDDict(p, n)
+        if not self._h:
+            raise ZstdError(30, "ZSTD_createDDict failed (dictionary corrupted or out of memory)")
+
+    @property
+    def dict_id(self) -> int:
+        return int(lib().ZSTD_getDictID_fromDDict(self._h))
+
+    def close(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h and _lib is not None:
+            _lib.ZSTD_freeDDict(h)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:      # interpreter teardown
+            pass
+
+
 class ZSTD_DCtx:
     """Reusable decompression context (lib/zstd.h:289-299): owns the device workspace and a stream."""
+
+    PARAMS = {"window_log_max": 100}
 
     def __init__(self, device: Optional[int] = None):
         L = lib()
@@ -377,6 +426,49 @@ class ZSTD_DCtx:
         dst = ctypes.create_string_buffer(max(max_size, 1))
         r = _check(lib().ZSTD_decompressDCtx(self._h, dst, max_size, p, n))
         return dst.raw[:r]
+
+    def decompress_using_ddict(self, frames, ddict: Optional["ZSTD_DDict"], max_size: Optional[int] = None) -> bytes:
+        """ZSTD_decompress_usingDDict (lib/zstd.h:1017); max_size as for decompress."""
+        p, n, keep = _buf(frames)
+        if max_size is None:
+            max_size = self._content_size(p, n)
+        dst = ctypes.create_string_buffer(max(max_size, 1))
+        r = _check(lib().ZSTD_decompress_usingDDict(self._h, dst, max_size, p, n, ddict._h if ddict is not None else None))
+        return dst.raw[:r]
+
+    @staticmethod
+    def _content_size(p, n) -> int:
+        cs = lib().ZSTD_getFrameContentSize(p, n)
+        if cs >= (1 << 64) - 2:
+            raise ZstdError(72, "content size unknown: pass max_size")
+        return cs
+
+    # -- sticky dictionary and parameters (lib/zstd.h:609-650, 1160-1210) --
+    def set_parameter(self, name_or_id, value: int) -> None:
+        """ZSTD_DCtx_setParameter: "window_log_max" (100) only; sticky until reset(parameters)."""
+        pid = self.PARAMS.get(name_or_id, name_or_id)
+        _check(lib().ZSTD_DCtx_setParameter(self._h, int(pid), int(value)))
+
+    def reset(self, directive: int = 3) -> None:
+        """ZSTD_DCtx_reset: 1 session only, 2 parameters (and dictionary), 3 both."""
+        _check(lib().ZSTD_DCtx_reset(self._h, directive))
+
+    def load_dictionary(self, dict_bytes) -> None:
+        """ZSTD_DCtx_loadDictionary: a copy, sticky; None or b"" clears it."""
+        p, n, keep = (None, 0, None) if not dict_bytes else _buf(dict_bytes)
+        _check(lib().ZSTD_DCtx_loadDictionary(self._h, p, n))
+
+    def ref_ddict(self, ddict: Optional["ZSTD_DDict"]) -> None:
+        """ZSTD_DCtx_refDDict: borrowed (keep the DDict alive while the context uses it), sticky; None clears it."""
+        self._ddict = ddict
+        _check(lib().ZSTD_DCtx_refDDict(self._h, ddict._h if ddict is not None else None))
+
+    def ref_prefix(self, prefix) -> None:
+        """ZSTD_DCtx_refPrefix: raw content for the next call only.  The context reads the bytes in place, so this object
+        keeps them until that call."""
+        p, n, keep = (None, 0, None) if not prefix else _buf(prefix)
+        _check(lib().ZSTD_DCtx_refPrefix(self._h, p, n))
+        self._prefix = keep
 
     def decompress_device(self, d_dst: int, dst_capacity: int, d_src: int, src_size: int, stream: int = 0) -> int:
         """Frames in device memory -> device memory (ints, e.g. torch.Tensor.data_ptr()).  Returns the decompressed size."""

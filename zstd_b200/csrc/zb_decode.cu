@@ -45,6 +45,8 @@
 #include <stdlib.h>
 #include <string.h>
 #include <vector>
+#include <memory>
+#include <mutex>
 #include <new>
 #include "../../include/zstd_b200.h"
 #include "zb_common.h"
@@ -489,6 +491,26 @@ zbd_matches_kernel(const ZbdBlock* __restrict__ blocks, const ZbdFrame* __restri
 }
 
 /* ------------------------------------------------------------------------------------------------ host driver */
+/* Digested dictionary of the decoder (lib/zstd.h:1000-1030, zstd_ddict.c): parsed on the host when it is digested
+ * (zbd_parseDict), uploaded whole (header and content) to the device of the first context that uses it, and resident there
+ * from then on.  The one form in which the decoder sees a dictionary: a ZSTD_createDDict object, which any number of contexts
+ * on one device may use; a context's sticky dictionary (ZSTD_DCtx_loadDictionary, ZSTD_DCtx_refPrefix); and the bytes a call
+ * passes with ZSTD_decompress_usingDict, digested into the context's own object (ZSTD_DCtx_s::callDict) on every call.
+ * The compressor's ZSTD_CDict_s keeps a 128 KiB tail of the content; the decoder needs all of it. */
+struct ZSTD_DDict_s {
+    std::unique_ptr<u8[]> copy;    /* ZSTD_createDDict's copy of the bytes (ZSTD_dlm_byCopy) */
+    const u8* bytes;               /* the whole dictionary: that copy, or the caller's buffer */
+    size_t size;
+    ZbdDictInfo di;
+    mutable std::mutex lock;       /* guards the device state below */
+    mutable int device;            /* -1 until the device buffer exists */
+    mutable bool resident;         /* uploaded since the digest */
+    mutable ZbDevBuf<u8> d_dict;
+};
+struct ZbdDDictFree { void operator()(ZSTD_DDict* dd) const { ZSTD_freeDDict(dd); } };
+typedef std::unique_ptr<ZSTD_DDict, ZbdDDictFree> ZbdDDictPtr;
+enum ZbdDictUses { ZBD_DICT_DONT_USE, ZBD_DICT_USE_ONCE, ZBD_DICT_USE_ALWAYS };    /* ZSTD_dictUses_e, zstd_decompress_internal.h */
+
 struct ZSTD_DCtx_s {
     int device, bindDevice;
     ZbStream stream;
@@ -503,8 +525,12 @@ struct ZSTD_DCtx_s {
     std::vector<u8> dsIn, dsOut; size_t dsOutPos;
     size_t hostWalkMax;          /* ZBD_HOSTWALK_MAX, or ZSTDB200_HOSTWALK_MAX from the environment (tests: 0 forces the kernel walk) */
     ZbHostBuf<u8> h_stage;       /* copy of a device-resident input's compressed bytes, for the header walk */
-    ZbDevBuf<u8> d_dict;         /* the call's dictionary, whole (header + content) */
-    ZbdDictInfo di; size_t dictSize;
+    /* the sticky dictionary (zstd_decompress.c:316-322, :1178-1193): ddict is localDict or a borrowed DDict, NULL for none */
+    ZbdDDictPtr localDict;       /* ZSTD_DCtx_loadDictionary's copy, or ZSTD_DCtx_refPrefix's digest of the caller's bytes */
+    const ZSTD_DDict* ddict;
+    int dictUses;                /* ZbdDictUses; a prefix is used by the next call (in streaming, the next frame) only */
+    ZbdDDictPtr callDict;        /* digest of the dictionary bytes the current call passes; reads the caller's buffer in place */
+    size_t maxWindow;            /* ZSTD_d_windowLogMax: ZSTD_decompressStream refuses frames whose window is larger */
     ZbEvents ev;
     ZSTDB200_dstats stats;
 };
@@ -513,16 +539,20 @@ struct ZSTD_DCtx_s {
 struct ZbdCall {
     void* dst; size_t dstCapacity;
     const void* src; size_t srcSize;
-    const void* dict; size_t dictSize;  /* host memory; NULL / 0: none */
+    const void* dict; size_t dictSize;  /* bytes to digest into the context's callDict (host memory); NULL / 0: none */
+    const ZSTD_DDict* ddict;            /* otherwise: a digested dictionary, or NULL for none */
     bool deviceMemory;                  /* dst and src are device memory */
     cudaStream_t stream;                /* device calls: the caller's stream, NULL for the context's */
 };
+
+#define ZBD_WINDOW_DEFAULT ((size_t)1 << 27)    /* ZSTD_WINDOWLOG_LIMIT_DEFAULT */
 
 extern "C" ZSTD_DCtx* ZSTD_createDCtx(void)                          /* lib/zstd.h:289 */
 {
     ZSTD_DCtx* d = new (std::nothrow) ZSTD_DCtx();                  /* value-initialised: every plain member is zero */
     if (!d) return NULL;
     d->device = -1;
+    d->maxWindow = ZBD_WINDOW_DEFAULT;
     {   const char* const e = getenv("ZSTDB200_HOSTWALK_MAX"); d->hostWalkMax = e ? (size_t)strtoull(e, NULL, 10) : ZBD_HOSTWALK_MAX; }
     d->bindDevice = zb_contextDevice();
     return d;
@@ -549,24 +579,36 @@ static size_t zbd_ctxInit(ZSTD_DCtx* d)
 /* the decoder's arrays are allocated with slack (an eighth more, and 64): calls of similar sizes reuse them */
 template <typename T> static size_t zbd_reserve(ZbDevBuf<T>& b, size_t need) { return b.ensure(need, need / 8 + 64); }
 
-/* D1 .. D4 over descriptors that are already on the device; returns the output size */
-static size_t zbd_run(ZSTD_DCtx* d, u8* d_dst, size_t dstCapacity, const u8* d_src, u32 nb, u32 nf, u64 seqCount, cudaStream_t st)
+/* the dictionary description the kernels take: dd's, or none */
+static ZbdDictInfo zbd_dictInfo(const ZSTD_DDict* dd)
 {
+    ZbdDictInfo di;
+    if (dd) di = dd->di; else memset(&di, 0, sizeof(di));
+    return di;
+}
+
+/* D1 .. D4 over descriptors that are already on the device, with the resident dictionary dd (NULL: none); returns the
+ * output size */
+static size_t zbd_run(ZSTD_DCtx* d, u8* d_dst, size_t dstCapacity, const u8* d_src, u32 nb, u32 nf, u64 seqCount, const ZSTD_DDict* dd,
+                      cudaStream_t st)
+{
+    ZbdDictInfo const di = zbd_dictInfo(dd);
+    const u8* const d_dict = dd ? (const u8*)dd->d_dict : (const u8*)NULL;
     CK(cudaMemsetAsync(d->d_execErr, 0, sizeof(u32), st));
     CK(cudaEventRecord(d->ev[1], st));
     u32 const grid = (nb + ZBD_WARPS - 1u) / ZBD_WARPS;
-    zbd_literals_kernel<<<grid, 32 * ZBD_WARPS, 0, st>>>(d_src, d->d_blocks, nb, d->d_lits, d->d_bout, d->d_dict, d->di);
+    zbd_literals_kernel<<<grid, 32 * ZBD_WARPS, 0, st>>>(d_src, d->d_blocks, nb, d->d_lits, d->d_bout, d_dict, di);
     CK(cudaEventRecord(d->ev[2], st));
-    zbd_sequences_kernel<<<grid, 32 * ZBD_WARPS, 0, st>>>(d_src, d->d_blocks, nb, d->d_seqs, d->d_bout, d->d_dict, d->di);
+    zbd_sequences_kernel<<<grid, 32 * ZBD_WARPS, 0, st>>>(d_src, d->d_blocks, nb, d->d_seqs, d->d_bout, d_dict, di);
     CK(cudaEventRecord(d->ev[3], st));
-    zbd_scan_kernel<<<1, SCAN_THREADS, 0, st>>>(d->d_blocks, nb, d->d_frames, nf, d->d_bout, (u64)dstCapacity, d->d_res, d->di);
+    zbd_scan_kernel<<<1, SCAN_THREADS, 0, st>>>(d->d_blocks, nb, d->d_frames, nf, d->d_bout, (u64)dstCapacity, d->d_res, di);
     CK(cudaMemcpyAsync(d->h_res, d->d_res, 2 * sizeof(u64), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));                                  /* nothing is written to dst before the sizes are known to fit */
     if (d->h_res[0]) return ZB_ERR((u32)d->h_res[0]);
     size_t const total = (size_t)d->h_res[1];
     CK(cudaEventRecord(d->ev[4], st));
-    u32 const dictContent = d->dictSize ? (u32)(d->dictSize - d->di.contentOff) : 0u;
-    const u8* const d_dictContent = d->dictSize ? d->d_dict + d->di.contentOff : (const u8*)NULL;
+    u32 const dictContent = dd ? (u32)(dd->size - di.contentOff) : 0u;
+    const u8* const d_dictContent = dd ? d_dict + di.contentOff : (const u8*)NULL;
     TRY(zbd_reserve(d->d_tileFirst, (total >> ZBD_TILE_LOG) + 4));
     TRY(zbd_reserve(d->d_done, (size_t)seqCount + 4));
     CK(cudaMemsetAsync(d->d_tileFirst, 0xFF, ((total >> ZBD_TILE_LOG) + 4) * sizeof(u32), st));
@@ -607,29 +649,68 @@ static size_t zbd_ensure(ZSTD_DCtx* d, u32 nb, u32 nf, u64 litBytes, u64 seqCoun
 }
 
 
-/* the call's dictionary: parsed on the host (zbd_parseDict), uploaded whole; NULL / 0 = none.  A dictionary without the
- * magic number — or shorter than 8 bytes — is raw content (zstd_decompress.c:1541-1560). */
-static size_t zbd_setDict(ZSTD_DCtx* d, const void* dict, size_t dictSize, cudaStream_t st)
+/* Digests dict[0 .. size) into dd, which reads those bytes in place.  A dictionary without the magic number, shorter than 8
+ * bytes, or a prefix (rawContent) is raw content (zstd_ddict.c:95-107); a zstd-format one is parsed on the host. */
+static size_t zbd_digestDict(ZSTD_DDict* dd, const u8* dict, size_t size, bool rawContent)
 {
-    memset(&d->di, 0, sizeof(d->di)); d->dictSize = 0;
-    if (!dict || dictSize == 0) return 0;
-    u32 const e = zbd_parseDict(&d->di, (const u8*)dict, dictSize);
-    if (e) return ZB_ERR(e);
-    TRY(zbd_reserve(d->d_dict, dictSize + 16));
-    CK(cudaMemcpyAsync(d->d_dict, dict, dictSize, cudaMemcpyHostToDevice, st));
-    CK(cudaStreamSynchronize(st));                                    /* the caller's dictionary buffer is pageable memory that may change after the call */
-    d->dictSize = dictSize;
+    dd->bytes = dict; dd->size = dict ? size : 0; dd->resident = false;
+    memset(&dd->di, 0, sizeof(dd->di));
+    if (rawContent || dd->size == 0) return 0;
+    u32 const e = zbd_parseDict(&dd->di, dict, size);
+    return e ? ZB_ERR(e) : 0;
+}
+
+/* A DDict that reads dict in place (byCopy = false) or its own copy of it; NULL when the entropy tables are corrupted or
+ * memory runs out */
+static ZSTD_DDict* zbd_createDDict(const void* dict, size_t dictSize, bool byCopy, bool rawContent)
+{
+    size_t const size = dict ? dictSize : 0;
+    ZSTD_DDict* dd = new (std::nothrow) ZSTD_DDict();                   /* value-initialised: every plain member is zero */
+    if (!dd) return NULL;
+    dd->device = -1;
+    const u8* bytes = (const u8*)dict;
+    if (byCopy && size) {
+        dd->copy.reset(new (std::nothrow) u8[size]);
+        if (!dd->copy) { delete dd; return NULL; }
+        memcpy(dd->copy.get(), dict, size);
+        bytes = dd->copy.get();
+    }
+    if (zb_isErr(zbd_digestDict(dd, bytes, size, rawContent))) { delete dd; return NULL; }
+    return dd;
+}
+
+/* Makes dd resident on `device`, zb_residentDict's rule: the buffer is allocated on the first device that uses dd (one device
+ * per DDict: another gets parameter_unsupported), the bytes are uploaded once per digest, and the upload has completed
+ * before another context can use dd.  A resident DDict costs a call nothing: no copy, no synchronisation. */
+static size_t zbd_residentDict(const ZSTD_DDict* dd, int device, cudaStream_t st)
+{
+    std::lock_guard<std::mutex> g(dd->lock);
+    if (dd->device >= 0 && dd->device != device) return ZB_ERR(ZB_error_parameter_unsupported);
+    if (dd->resident) return 0;
+    TRY(zbd_reserve(dd->d_dict, dd->size + 16));
+    dd->device = device;
+    CK(cudaMemcpyAsync(dd->d_dict, dd->bytes, dd->size, cudaMemcpyHostToDevice, st));
+    CK(cudaStreamSynchronize(st));                                    /* the source is pageable memory that may change after the call */
+    dd->resident = true;
     return 0;
 }
 
+/* dictionary bytes passed to a call, digested into the context's callDict */
+static size_t zbd_digestCallDict(ZSTD_DCtx* d, const void* dict, size_t dictSize)
+{
+    if (!d->callDict) d->callDict.reset(zbd_createDDict(NULL, 0, false, false));
+    if (!d->callDict) return ZB_ERR(ZB_error_memory_allocation);
+    return zbd_digestDict(d->callDict.get(), (const u8*)dict, dictSize, false);
+}
+
 /* D0 on a host-readable copy of the compressed bytes: count the blocks and frames, then describe them into B and F */
-static u32 zbd_walkHost(const ZSTD_DCtx* d, const u8* in, size_t size, std::vector<ZbdBlock>& B, std::vector<ZbdFrame>& F,
+static u32 zbd_walkHost(const ZbdDictInfo& di, const u8* in, size_t size, std::vector<ZbdBlock>& B, std::vector<ZbdFrame>& F,
                         u32* nb, u32* nf, u64* lit, u64* seq)
 {
-    u32 const e = zbd_walk(in, size, NULL, 0, NULL, 0, nb, nf, lit, seq, d->di.entropy != 0, d->di.dictID);
+    u32 const e = zbd_walk(in, size, NULL, 0, NULL, 0, nb, nf, lit, seq, di.entropy != 0, di.dictID);
     if (e) return e;
     B.resize(*nb ? *nb : 1); F.resize(*nf ? *nf : 1);
-    return zbd_walk(in, size, B.data(), *nb, F.data(), *nf, nb, nf, lit, seq, d->di.entropy != 0, d->di.dictID);
+    return zbd_walk(in, size, B.data(), *nb, F.data(), *nf, nb, nf, lit, seq, di.entropy != 0, di.dictID);
 }
 
 /* Every decompression call.  The frame and block headers have to be followed one after the other wherever they are read:
@@ -647,7 +728,11 @@ static size_t zbd_decompress(ZSTD_DCtx* d, const ZbdCall& c)
     TRY(zbd_ctxInit(d));
     memset(&d->stats, 0, sizeof(d->stats));
     cudaStream_t const st = c.stream ? c.stream : d->stream;
-    TRY(zbd_setDict(d, c.dict, c.dictSize, st));
+    const ZSTD_DDict* dd = c.ddict;
+    if (c.dict && c.dictSize) { TRY(zbd_digestCallDict(d, c.dict, c.dictSize)); dd = d->callDict.get(); }
+    if (dd && dd->size == 0) dd = NULL;                               /* an empty dictionary is none */
+    if (dd) TRY(zbd_residentDict(dd, d->device, st));
+    ZbdDictInfo const di = zbd_dictInfo(dd);
     /* D0: block and frame descriptors */
     const u8* hostIn = c.deviceMemory ? NULL : (const u8*)c.src;
     if (c.deviceMemory && c.srcSize <= d->hostWalkMax) {
@@ -658,12 +743,12 @@ static size_t zbd_decompress(ZSTD_DCtx* d, const ZbdCall& c)
     }
     std::vector<ZbdBlock> B; std::vector<ZbdFrame> F;
     u32 nb = 0, nf = 0; u64 lit = 0, seq = 0;
-    if (hostIn) { u32 const e = zbd_walkHost(d, hostIn, c.srcSize, B, F, &nb, &nf, &lit, &seq); if (e) return ZB_ERR(e); }
+    if (hostIn) { u32 const e = zbd_walkHost(di, hostIn, c.srcSize, B, F, &nb, &nf, &lit, &seq); if (e) return ZB_ERR(e); }
     else {                                                            /* the walk kernel; once more if the arrays were too small */
         u32 capB = (u32)(c.srcSize / 4096u) + 1024u, capF = 1024u;
         for (int attempt = 0; attempt < 2; attempt++) {
             TRY(zbd_ensure(d, capB, capF, 0, 0));
-            zbd_walk_kernel<<<1, 32, 0, st>>>((const u8*)c.src, (u64)c.srcSize, d->d_blocks, (u32)d->d_blocks.cap, d->d_frames, (u32)d->d_frames.cap, d->d_res, d->di.entropy, d->di.dictID);
+            zbd_walk_kernel<<<1, 32, 0, st>>>((const u8*)c.src, (u64)c.srcSize, d->d_blocks, (u32)d->d_blocks.cap, d->d_frames, (u32)d->d_frames.cap, d->d_res, di.entropy, di.dictID);
             CK(cudaMemcpyAsync(d->h_res, d->d_res, 5 * sizeof(u64), cudaMemcpyDeviceToHost, st));
             CK(cudaStreamSynchronize(st));
             if (d->h_res[0]) return ZB_ERR((u32)d->h_res[0]);
@@ -693,7 +778,7 @@ static size_t zbd_decompress(ZSTD_DCtx* d, const ZbdCall& c)
         CK(cudaMemcpyAsync(d->d_frames, F.data(), (size_t)nf * sizeof(ZbdFrame), cudaMemcpyHostToDevice, st));
         CK(cudaStreamSynchronize(st));                               /* B and F are pageable: the copies end before a return can free them */
     }
-    size_t const total = zbd_run(d, runDst, outCap, runSrc, nb, nf, seq, st);
+    size_t const total = zbd_run(d, runDst, outCap, runSrc, nb, nf, seq, dd, st);
     if (zb_isErr(total) || c.deviceMemory) return total;
     if (total > c.dstCapacity) return ZB_ERR(ZB_error_dstSize_tooSmall);
     if (total) CK(cudaMemcpy(c.dst, d->d_out, total, cudaMemcpyDeviceToHost));
@@ -721,15 +806,105 @@ static size_t zbd_decompress(ZSTD_DCtx* d, const ZbdCall& c)
     return total;
 }
 
+/* ------------------------------------------------------------------------------------------------ dictionaries and parameters
+ * (lib/zstd.h:1000-1030, :1160-1210; zstd_decompress.c:1697-1960) */
+extern "C" ZSTD_DDict* ZSTD_createDDict(const void* dict, size_t dictSize)                  /* zstd_ddict.c:178 */
+{
+    return zbd_createDDict(dict, dictSize, true, false);
+}
+extern "C" size_t ZSTD_freeDDict(ZSTD_DDict* dd) { return zb_deleteOnDevice(dd); }           /* accepts NULL, zstd_ddict.c:212 */
+extern "C" unsigned ZSTD_getDictID_fromDDict(const ZSTD_DDict* dd) { return dd ? dd->di.dictID : 0u; }      /* zstd_ddict.c:236 */
+extern "C" unsigned ZSTD_getDictID_fromFrame(const void* src, size_t srcSize)               /* zstd_decompress.c:1642 */
+{
+    ZbdFrameHeader h;
+    if (zbd_readFrameHeader(&h, (const u8*)src, srcSize) || h.skippable) return 0;
+    return h.dictID;
+}
+
+static void zbd_clearDict(ZSTD_DCtx* d) { d->localDict.reset(); d->ddict = NULL; d->dictUses = ZBD_DICT_DONT_USE; }
+/* the sticky dictionary for the next call (or frame); a prefix is handed out once */
+static const ZSTD_DDict* zbd_getDDict(ZSTD_DCtx* d)
+{
+    switch (d->dictUses) {
+    case ZBD_DICT_USE_ALWAYS: return d->ddict;
+    case ZBD_DICT_USE_ONCE: d->dictUses = ZBD_DICT_DONT_USE; return d->ddict;
+    default: zbd_clearDict(d); return NULL;
+    }
+}
+/* ZSTD_decompressStream holds part of a frame, or output of one that is still to be handed out (streamStage != zdss_init) */
+static bool zbd_midFrame(const ZSTD_DCtx* d) { return !d->dsIn.empty() || d->dsOutPos < d->dsOut.size(); }
+
+static size_t zbd_loadDict(ZSTD_DCtx* d, const void* dict, size_t dictSize, bool byCopy, bool rawContent)
+{
+    if (!d) return ZB_ERR(ZB_error_GENERIC);
+    if (zbd_midFrame(d)) return ZB_ERR(ZB_error_stage_wrong);
+    zbd_clearDict(d);
+    if (dict && dictSize) {
+        d->localDict.reset(zbd_createDDict(dict, dictSize, byCopy, rawContent));
+        if (!d->localDict) return ZB_ERR(ZB_error_memory_allocation);    /* corrupted entropy tables too, as in the reference (:1705-1706) */
+        d->ddict = d->localDict.get(); d->dictUses = ZBD_DICT_USE_ALWAYS;
+    }
+    return 0;
+}
+extern "C" size_t ZSTD_DCtx_loadDictionary(ZSTD_DCtx* d, const void* dict, size_t dictSize)    /* :1718 */
+{
+    return zbd_loadDict(d, dict, dictSize, true, false);
+}
+extern "C" size_t ZSTD_DCtx_refPrefix(ZSTD_DCtx* d, const void* prefix, size_t prefixSize)     /* :1730 */
+{
+    TRY(zbd_loadDict(d, prefix, prefixSize, false, true));
+    d->dictUses = ZBD_DICT_USE_ONCE;
+    return 0;
+}
+extern "C" size_t ZSTD_DCtx_refDDict(ZSTD_DCtx* d, const ZSTD_DDict* ddict)                    /* :1778 */
+{
+    if (!d) return ZB_ERR(ZB_error_GENERIC);
+    if (zbd_midFrame(d)) return ZB_ERR(ZB_error_stage_wrong);
+    zbd_clearDict(d);
+    if (ddict) { d->ddict = ddict; d->dictUses = ZBD_DICT_USE_ALWAYS; }
+    return 0;
+}
+extern "C" size_t ZSTD_DCtx_setParameter(ZSTD_DCtx* d, ZSTD_dParameter param, int value)       /* :1904 */
+{
+    if (!d) return ZB_ERR(ZB_error_GENERIC);
+    if (zbd_midFrame(d)) return ZB_ERR(ZB_error_stage_wrong);
+    if (param != ZSTD_d_windowLogMax) return ZB_ERR(ZB_error_parameter_unsupported);
+    if (value == 0) value = 27;                                          /* ZSTD_WINDOWLOG_LIMIT_DEFAULT */
+    if (value < 10 || value > 31) return ZB_ERR(ZB_error_parameter_outOfBound);   /* ZSTD_WINDOWLOG_ABSOLUTEMIN, ZSTD_WINDOWLOG_MAX */
+    d->maxWindow = (size_t)1 << value;
+    return 0;
+}
+extern "C" size_t ZSTD_DCtx_reset(ZSTD_DCtx* d, ZSTD_ResetDirective reset)                     /* :1945 */
+{
+    if (!d) return ZB_ERR(ZB_error_GENERIC);
+    if (reset == ZSTD_reset_session_only || reset == ZSTD_reset_session_and_parameters) {
+        d->dsIn.clear(); d->dsOut.clear(); d->dsOutPos = 0;
+    }
+    if (reset == ZSTD_reset_parameters || reset == ZSTD_reset_session_and_parameters) {
+        if (zbd_midFrame(d)) return ZB_ERR(ZB_error_stage_wrong);
+        zbd_clearDict(d);
+        d->maxWindow = ZBD_WINDOW_DEFAULT;
+    }
+    return 0;
+}
+
+/* ------------------------------------------------------------------------------------------------ one-shot calls */
 extern "C" size_t ZSTD_decompress_usingDict(ZSTD_DCtx* d, void* dst, size_t dstCapacity, const void* src, size_t srcSize,
                                             const void* dict, size_t dictSize)                                            /* lib/zstd.h:955 */
 {
-    ZbdCall const c = { dst, dstCapacity, src, srcSize, dict, dictSize, false, NULL };
+    ZbdCall const c = { dst, dstCapacity, src, srcSize, dict, dictSize, NULL, false, NULL };
+    return zbd_decompress(d, c);
+}
+extern "C" size_t ZSTD_decompress_usingDDict(ZSTD_DCtx* d, void* dst, size_t dstCapacity, const void* src, size_t srcSize,
+                                             const ZSTD_DDict* ddict)                                                     /* lib/zstd.h:1017 */
+{
+    ZbdCall const c = { dst, dstCapacity, src, srcSize, NULL, 0, ddict, false, NULL };
     return zbd_decompress(d, c);
 }
 extern "C" size_t ZSTD_decompressDCtx(ZSTD_DCtx* d, void* dst, size_t dstCapacity, const void* src, size_t srcSize)      /* lib/zstd.h:299 */
 {
-    return ZSTD_decompress_usingDict(d, dst, dstCapacity, src, srcSize, NULL, 0);
+    if (!d) return ZB_ERR(ZB_error_GENERIC);
+    return ZSTD_decompress_usingDDict(d, dst, dstCapacity, src, srcSize, zbd_getDDict(d));     /* zstd_decompress.c:1195 */
 }
 
 extern "C" size_t ZSTD_decompress(void* dst, size_t dstCapacity, const void* src, size_t compressedSize)                  /* lib/zstd.h:170 */
@@ -744,12 +919,14 @@ extern "C" size_t ZSTD_decompress(void* dst, size_t dstCapacity, const void* src
 extern "C" size_t ZSTDB200_decompressDevice_usingDict(ZSTD_DCtx* d, void* d_dst, size_t dstCapacity, const void* d_src, size_t srcSize,
                                                       const void* dict, size_t dictSize, void* stream)
 {
-    ZbdCall const c = { d_dst, dstCapacity, d_src, srcSize, dict, dictSize, true, (cudaStream_t)stream };
+    ZbdCall const c = { d_dst, dstCapacity, d_src, srcSize, dict, dictSize, NULL, true, (cudaStream_t)stream };
     return zbd_decompress(d, c);
 }
 extern "C" size_t ZSTDB200_decompressDevice(ZSTD_DCtx* d, void* d_dst, size_t dstCapacity, const void* d_src, size_t srcSize, void* stream)
 {
-    return ZSTDB200_decompressDevice_usingDict(d, d_dst, dstCapacity, d_src, srcSize, NULL, 0, stream);
+    if (!d) return ZB_ERR(ZB_error_GENERIC);
+    ZbdCall const c = { d_dst, dstCapacity, d_src, srcSize, NULL, 0, zbd_getDDict(d), true, (cudaStream_t)stream };
+    return zbd_decompress(d, c);
 }
 
 extern "C" void ZSTDB200_getLastDStats(const ZSTD_DCtx* d, ZSTDB200_dstats* out) { if (d && out) *out = d->stats; }
@@ -806,7 +983,8 @@ extern "C" size_t ZSTD_initDStream(ZSTD_DStream* zds)
     if (!zds) return ZB_ERR(ZB_error_GENERIC);
     zds->dsIn.clear(); zds->dsOut.clear();
     zds->dsOutPos = 0;
-    return 5;                                                          /* a frame header's first bytes, as the reference suggests (ZSTD_startingInputLength) */
+    zbd_clearDict(zds);                                                /* ZSTD_DCtx_refDDict(zds, NULL), zstd_decompress.c:1752 */
+    return 5;                                                         /* a frame header's first bytes, as the reference suggests (ZSTD_startingInputLength) */
 }
 extern "C" size_t ZSTD_DStreamInSize(void) { return ZB_BLOCK_MAX + 3; }  /* lib/zstd.h:922 */
 extern "C" size_t ZSTD_DStreamOutSize(void) { return ZB_BLOCK_MAX; }
@@ -822,15 +1000,26 @@ extern "C" size_t ZSTD_decompressStream(ZSTD_DStream* d, ZSTD_outBuffer* out, ZS
         return d->dsOut.size() - d->dsOutPos;
     };
     if (handOut() != 0) return d->dsOut.size() - d->dsOutPos;            /* room first: input is only taken while nothing is waiting */
+    size_t carried = d->dsIn.size();                                     /* bytes that came with earlier calls */
     d->dsIn.insert(d->dsIn.end(), (const u8*)in->src + in->pos, (const u8*)in->src + in->size);
     in->pos = in->size;
     bool decoded = false;
     while (!d->dsIn.empty()) {
         size_t const fs = ZSTD_findFrameCompressedSize(d->dsIn.data(), d->dsIn.size());
-        if (ZSTD_isError(fs)) {
-            if (ZSTD_getErrorCode(fs) == ZB_error_srcSize_wrong) break;   /* the frame is not complete yet */
-            return fs;
+        bool const incomplete = ZSTD_isError(fs) && ZSTD_getErrorCode(fs) == ZB_error_srcSize_wrong;
+        if (ZSTD_isError(fs) && !incomplete) return fs;
+        /* ZSTD_d_windowLogMax, decided from the header once it is complete (zstd_decompress.c:2227-2229).  As in the reference,
+         * a frame that arrives whole with one call whose output buffer has room for its stated content size is decoded in
+         * one pass, which does not apply the limit (:2183-2199). */
+        {   ZbdFrameHeader h;
+            if (!zbd_readFrameHeader(&h, d->dsIn.data(), d->dsIn.size()) && !h.skippable) {
+                size_t const free = out->size - out->pos, room = free > d->dsOut.size() ? free - d->dsOut.size() : 0;   /* behind earlier frames' output */
+                bool const onePass = !incomplete && carried == 0 && h.contentSize != ZBD_CONTENTSIZE_UNKNOWN && (u64)room >= h.contentSize;
+                u64 const window = h.windowSize < 1024u ? 1024u : h.windowSize;
+                if (!onePass && window > (u64)d->maxWindow) return ZB_ERR(16);        /* frameParameter_windowTooLarge */
+            }
         }
+        if (incomplete) break;                                           /* the frame is not complete yet */
         size_t const bound = zbd_frameOutputBound(d->dsIn.data(), fs);
         size_t const base = d->dsOut.size();
         try { d->dsOut.resize(base + bound + 1); }
@@ -839,6 +1028,7 @@ extern "C" size_t ZSTD_decompressStream(ZSTD_DStream* d, ZSTD_outBuffer* out, ZS
         if (ZSTD_isError(r)) { d->dsOut.resize(base); return r; }
         d->dsOut.resize(base + r);
         d->dsIn.erase(d->dsIn.begin(), d->dsIn.begin() + (ptrdiff_t)fs);
+        carried = carried > fs ? carried - fs : 0;
         decoded = true;
     }
     size_t const waiting = handOut();
