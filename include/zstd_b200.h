@@ -77,8 +77,30 @@ ZSTDB200_API unsigned    ZSTD_getDictID_fromDict(const void* dict, size_t dictSi
  * (512 KiB) has a 2^27-byte window (before the adjustment to its size) and its blocks may copy from anywhere in it; smaller
  * frames are compressed exactly as with LDM off.  Honoured by ZSTD_compress2, ZSTD_compressStream2,
  * ZSTDB200_compressFrames[_usingCDict] and ZSTDB200_compressDevice; ignored by the simple API and the sequence calls;
- * ZSTDB200_compressFramePart returns 40.  Unlike the reference, dictionary content is not searched for long matches (it
- * still serves the first chunk's history).  Host-buffer calls upload their whole input before the first kernel. */
+ * ZSTDB200_compressFramePart returns 40.  A prefix (ZSTD_CCtx_refPrefix, below) is searched for long matches; unlike the
+ * reference, the content of a loaded dictionary or CDict is not (it still serves the first chunk's history).  Host-buffer
+ * calls upload their whole input before the first kernel.
+ *
+ * ZSTD_CCtx_refPrefix (lib/zstd.h:1104-1125) — compress the next frame against a prefix, e.g. the previous version of a file
+ * (what `zstd --patch-from` does); the decoder needs the same bytes (ZSTD_DCtx_refPrefix, ZSTD_decompress_usingDict).  As in
+ * the reference: the bytes are borrowed, not copied, and must stay valid until that frame is made; they are raw content
+ * even when they begin with the dictionary magic; the frame names dictionary ID 0; the prefix serves the NEXT FRAME ONLY
+ * and is then forgotten (also when that call fails); NULL / 0 clears it; it replaces a loaded dictionary or referenced
+ * CDict and those replace it; inside an unfinished stream it returns ZSTD_error_stage_wrong (60).
+ * ZSTD_CCtx_reset(ZSTD_reset_session_only) keeps a pending prefix, the directives that reset parameters drop it.  A prefix of
+ * less than 8 bytes is ignored, as every dictionary that short.
+ * Honoured by ZSTD_compress2, ZSTD_compressStream2 (the first frame the session emits; frames the front end cuts later
+ * have none) and ZSTDB200_compressDevice; the simple API ignores it (it stays pending); ZSTDB200_compressFrames[_usingCDict],
+ * ZSTDB200_compressFramePart and the sequence calls return 40 while one is pending.
+ * Without LDM the prefix is a raw-content dictionary: its last 128 KiB are the first chunk's history.  With
+ * ZSTD_c_enableLongDistanceMatching = 1 and more than 512 KiB of prefix and input together, the prefix's last 2^27 bytes are
+ * indexed along with the frame and every block that ends within the window (2^27 bytes, less when prefix + input are
+ * smaller) of a prefix position may copy from it.  Matches are found in the prefix and in the frame, never across the seam
+ * between them; blocks beyond 2^27 bytes into the frame take nothing from the prefix (the format's window), and prefix bytes
+ * more than 2^27 from its end are never used.  Cost per call with P = min(prefixSize, 2^27) indexed bytes, n input bytes and
+ * m = ZSTD_c_ldmMinMatch (64): the LDM workspace grows from about 36 (n / m + 1) + 16 (n / 4096 + 1)(4096 / m + 1) bytes to the
+ * same of P + n, the match list from 8 (n / m + 1) to 8 ((P + n) / m + 1) bytes; a host prefix is uploaded (P bytes of device
+ * memory and of PCIe traffic, counted in h2d_bytes), a device prefix (ZSTDB200_CCtx_refPrefixDevice) is read in place. */
 typedef enum {
     ZSTD_c_compressionLevel = 100, ZSTD_c_windowLog = 101, ZSTD_c_hashLog = 102, ZSTD_c_chainLog = 103, ZSTD_c_searchLog = 104,
     ZSTD_c_minMatch = 105, ZSTD_c_targetLength = 106, ZSTD_c_strategy = 107,
@@ -94,6 +116,7 @@ ZSTDB200_API size_t ZSTD_CCtx_setPledgedSrcSize(ZSTD_CCtx* cctx, unsigned long l
 ZSTDB200_API size_t ZSTD_CCtx_reset(ZSTD_CCtx* cctx, ZSTD_ResetDirective reset);
 ZSTDB200_API size_t ZSTD_CCtx_loadDictionary(ZSTD_CCtx* cctx, const void* dict, size_t dictSize);
 ZSTDB200_API size_t ZSTD_CCtx_refCDict(ZSTD_CCtx* cctx, const ZSTD_CDict* cdict);
+ZSTDB200_API size_t ZSTD_CCtx_refPrefix(ZSTD_CCtx* cctx, const void* prefix, size_t prefixSize);
 ZSTDB200_API size_t ZSTD_compress2(ZSTD_CCtx* cctx, void* dst, size_t dstCapacity, const void* src, size_t srcSize);
 
 /* lib/zstd.h:681-862 — streaming.  The GPU works on whole frames, so the stream front end collects input in the context
@@ -257,6 +280,13 @@ ZSTDB200_API void ZSTDB200_getLastDStats(const ZSTD_DCtx* dctx, ZSTDB200_dstats*
  * several waves on several streams.  d_src needs no padding: no byte outside [d_src, d_src + srcSize) is read. */
 ZSTDB200_API size_t ZSTDB200_compressDevice(ZSTD_CCtx* cctx, void* d_dst, size_t dstCapacity,
                                             const void* d_src, size_t srcSize, int compressionLevel, void* stream);
+
+/* ZSTD_CCtx_refPrefix with the prefix in device memory, for ZSTDB200_compressDevice: nothing of it crosses PCIe and no copy
+ * is made (the kernels read it where it lies; it need not be adjacent to the input).  With a NULL stream the producer of
+ * d_prefix must have completed before the compression call, as for d_src.  A host-buffer call (ZSTD_compress2,
+ * ZSTD_compressStream2) that finds a device prefix pending returns 40 and forgets it.  A host prefix (ZSTD_CCtx_refPrefix)
+ * followed by ZSTDB200_compressDevice is fine: the call uploads it. */
+ZSTDB200_API size_t ZSTDB200_CCtx_refPrefixDevice(ZSTD_CCtx* cctx, const void* d_prefix, size_t prefixSize);
 
 /* ZSTD_compressSequences with sequences, input and output in device memory (a match finder on the GPU hands its sequences
  * over without a round trip through the host).  d_seqs: nbSeqs ZSTD_Sequence.  `stream`: as for ZSTDB200_compressDevice.

@@ -105,6 +105,11 @@ def lib() -> ctypes.CDLL:
     L.ZSTD_CCtx_loadDictionary.argtypes = [_vp, _vp, _sz]
     L.ZSTD_CCtx_refCDict.restype = _sz
     L.ZSTD_CCtx_refCDict.argtypes = [_vp, _vp]
+    if hasattr(L, "ZSTD_CCtx_refPrefix"):                                               # absent from older development builds
+        L.ZSTD_CCtx_refPrefix.restype = _sz
+        L.ZSTD_CCtx_refPrefix.argtypes = [_vp, _vp, _sz]
+        L.ZSTDB200_CCtx_refPrefixDevice.restype = _sz
+        L.ZSTDB200_CCtx_refPrefixDevice.argtypes = [_vp, _vp, _sz]
     L.ZSTD_compress2.restype = _sz
     L.ZSTD_compress2.argtypes = [_vp, _vp, _sz, _vp, _sz]
     L.ZSTD_compressStream2.restype = _sz
@@ -274,6 +279,20 @@ class ZSTD_CCtx:
 
     def ref_cdict(self, cdict: Optional["ZSTD_CDict"]) -> None:
         _check(lib().ZSTD_CCtx_refCDict(self._h, cdict._h if cdict is not None else None))
+
+    def ref_prefix(self, prefix) -> None:
+        """ZSTD_CCtx_refPrefix: raw content for the next frame only (compress2, compress_device, the first frame of a
+        stream); it replaces any dictionary, None or b"" clears it.  The context reads the bytes in place, so this object
+        keeps them until the next call of this method."""
+        p, n, keep = (None, 0, None) if not prefix else _buf(prefix)
+        _check(lib().ZSTD_CCtx_refPrefix(self._h, p, n))
+        self._prefix = keep
+
+    def ref_prefix_device(self, d_prefix: int, size: int) -> None:
+        """ZSTDB200_CCtx_refPrefixDevice: the same with the prefix in device memory (an int, e.g. torch.Tensor.data_ptr()),
+        for compress_device.  The caller keeps that memory alive until the frame is made."""
+        _check(lib().ZSTDB200_CCtx_refPrefixDevice(self._h, d_prefix if size else None, size))
+        self._prefix = None
 
     def compress2(self, src) -> bytes:
         """ZSTD_compress2 with the context's sticky parameters / dictionary."""

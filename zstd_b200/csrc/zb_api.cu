@@ -118,6 +118,7 @@ struct ZSTD_CDict_s {
     int level;
     std::unique_ptr<u8[]> copy;    /* ZSTD_createCDict's copy of the bytes (ZSTD_dlm_byCopy) */
     const u8* content;             /* the whole dictionary: that copy, or the caller's buffer */
+    bool contentOnDevice;          /* a prefix given with ZSTDB200_CCtx_refPrefixDevice: content is a device pointer */
     size_t size;
     size_t contentOff, tail;       /* entropy header size, bytes of content that blocks can see */
     ZbDictEntropy entropy;         /* parsed on the host by zb_digestDict */
@@ -158,7 +159,7 @@ template <typename T> struct ZbVec {
     T& operator[](size_t i) { return p[i]; }
     const T& operator[](size_t i) const { return p[i]; }
 };
-struct ZbLdmFrame { u32 frame; ZbLdmParams prm; u64 matchBase; };
+struct ZbLdmFrame { u32 frame; ZbLdmParams prm; u64 matchBase; u64 prefix; };   /* prefix: indexed prefix bytes in front of the frame */
 struct ZbPlan { ZbVec<ZbBlock> blocks; ZbVec<ZbChunk> chunks; ZbVec<ZbFrame> frames; std::vector<ZbGroup> groups; ZbStrides sd; bool unsupported;
                 std::vector<ZbLdmFrame> ldm; u64 ldmMatches;      /* frames with long-distance matching, their share of the match list */
                 u64 frameBytes, frameBlocks; u32 frameMaxBlock;   /* the whole frames, other ranks' blocks included: what decides the waves */
@@ -201,6 +202,10 @@ struct ZSTD_CCtx_s {
     ZbDevBuf<u64> d_ldmMatch, d_ldmFirst; ZbDevBuf<u32> d_ldmCnt; ZbDevBuf<u8> d_ldmScratch;
     std::unique_ptr<ZSTD_CDict, ZbCDictFree> advLocalDict;   /* ZSTD_CCtx_loadDictionary: owned copy, digested at its first use */
     const ZSTD_CDict* advRefCDict; /* ZSTD_CCtx_refCDict: borrowed */
+    /* ZSTD_CCtx_refPrefix / ZSTDB200_CCtx_refPrefixDevice: borrowed, for the next frame only; digested into callDict by the
+     * call that consumes it */
+    const u8* advPrefix; size_t advPrefixSize; bool advPrefixOnDevice;
+    ZbDevBuf<u8> d_prefix;         /* host prefix with LDM on: the indexed part, uploaded ahead of the LDM pass */
     ZbPlan plan;                   /* the call's plan; its vectors are reused (a million records are 100 MB of descriptors: fresh pages cost more than filling them) */
     /* streaming front end (ZSTD_compressStream2 with ZSTD_e_continue / ZSTD_e_flush): input collected on the host, compressed
      * output waiting to be handed out */
@@ -323,6 +328,9 @@ struct ZbCall {
     bool checksum, noDictID;                                      /* frame header options */
     u64 partBegin = 0, partEnd = ~0ull;                           /* ZSTDB200_compressFramePart: this rank's share of the one frame */
     const u32* ldm = nullptr;                                     /* long-distance matching: the 4 ldm parameters (0 = derived), or NULL */
+    /* the part of a prefix that the LDM pass indexes (its last min(size, 2^27) bytes; the whole prefix is the call's cdict),
+     * in host or device memory; one frame per call */
+    const u8* prefix = nullptr; u64 prefixSize = 0; bool prefixOnDevice = false;
 };
 
 static int g_strictLevels = 0;
@@ -377,13 +385,14 @@ static void zb_plan(ZbPlan& P, const ZbCall& a, size_t dictSize, size_t dictTail
             P.groups.back().c1 = (u32)P.chunks.size();
             continue;
         }
-        bool const ldm = a.ldm && fsz > ZB_LDM_MIN_FRAME;        /* a frame of one chunk is parsed whole: compressed as without LDM */
+        /* a frame of one chunk is parsed whole: compressed as without LDM, unless an indexed prefix lies in front of it */
+        bool const ldm = a.ldm && fsz && fsz + a.prefixSize > ZB_LDM_MIN_FRAME;
         ZbCParams cp = zb_getCParams(level, fsz, dictSize, ldm);
         ZbParams prm = zb_makeParams(cp);
         if (ldm) {
-            ZbLdmFrame lf; lf.frame = (u32)f; lf.prm = zb_ldmResolve(a.ldm, cp.windowLog); lf.matchBase = P.ldmMatches;
+            ZbLdmFrame lf; lf.frame = (u32)f; lf.prm = zb_ldmResolve(a.ldm, cp.windowLog); lf.matchBase = P.ldmMatches; lf.prefix = a.prefixSize;
             P.ldm.push_back(lf);
-            P.ldmMatches += zb_ldm_survivor_cap(fsz, lf.prm.minMatch);
+            P.ldmMatches += zb_ldm_survivor_cap(fsz + a.prefixSize, lf.prm.minMatch);
         }
         if (dictRep) {                                           /* a zstd-format dictionary's repcodes (zstd_compress.c:5054-5056) */
             prm.codeRep[0] = dictRep[0]; prm.codeRep[1] = dictRep[1]; prm.codeRep[2] = dictRep[2];
@@ -436,14 +445,15 @@ static void zb_plan(ZbPlan& P, const ZbCall& a, size_t dictSize, size_t dictTail
 }
 
 /* Parses dictionary bytes into cd: the entropy tables of a zstd-format dictionary, where its content starts and the content
- * tail that blocks can see.  A new digest has nothing on the device yet: no tail, no images. */
-static size_t zb_digestDict(ZSTD_CDict* cd, const u8* dict, size_t dictSize)
+ * tail that blocks can see.  A new digest has nothing on the device yet: no tail, no images.  rawContent: the bytes are
+ * content whatever they begin with (a prefix, ZSTD_dct_rawContent) and are not read here; onDevice: they lie in device memory. */
+static size_t zb_digestDict(ZSTD_CDict* cd, const u8* dict, size_t dictSize, bool rawContent = false, bool onDevice = false)
 {
-    cd->content = dict; cd->size = dict ? dictSize : 0;
+    cd->content = dict; cd->size = dict ? dictSize : 0; cd->contentOnDevice = onDevice;
     cd->contentOff = 0; cd->tail = 0; cd->resident = false; cd->nbImages = 0;
     memset(&cd->entropy, 0, sizeof(cd->entropy));
     if (cd->size < 8) return 0;                                          /* ignored by zb_compress */
-    size_t const off = zb_loadDictionary(&cd->entropy, dict, cd->size);
+    size_t const off = rawContent ? 0 : zb_loadDictionary(&cd->entropy, dict, cd->size);
     if (zb_isErr(off)) return off;
     cd->contentOff = off;
     size_t const contentSize = cd->size - off;
@@ -464,7 +474,8 @@ static size_t zb_residentDict(ZSTD_CDict* cd, int device, bool shared, cudaStrea
         cd->device = device;
     }
     CK(cudaMemsetAsync(cd->d_dict, 0, ZB_PRIME_BYTES + 64, stream));
-    if (cd->tail) CK(cudaMemcpyAsync(cd->d_dict + 32, cd->content + (cd->size - cd->tail), cd->tail, cudaMemcpyHostToDevice, stream));
+    if (cd->tail) CK(cudaMemcpyAsync(cd->d_dict + 32, cd->content + (cd->size - cd->tail), cd->tail,
+                                     cd->contentOnDevice ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, stream));
     if (cd->entropy.present) CK(cudaMemcpyAsync(cd->d_de, &cd->entropy, sizeof(ZbDictEntropy), cudaMemcpyHostToDevice, stream));
     if (shared) CK(cudaStreamSynchronize(stream));
     cd->resident = true;
@@ -504,11 +515,13 @@ static size_t zb_buildDictImages(ZSTD_CDict* cd, ZbPlan& P, bool shared, cudaStr
 /* Long-distance matching (zb_ldm.cu): every LDM frame's matches, by block index in the call, before the first wave (a block
  * may copy from anywhere in its 2^27-byte window, i.e. from any earlier wave).  The frames run one after another on
  * `stream` through one scratch area. */
-static size_t zb_runLdm(ZSTD_CCtx* c, const ZbPlan& P, const u8* d_src, cudaStream_t stream, unsigned* launches)
+static size_t zb_runLdm(ZSTD_CCtx* c, const ZbPlan& P, const u8* d_src, const u8* d_prefix, cudaStream_t stream, unsigned* launches)
 {
     size_t scratch = 0;
     for (size_t i = 0; i < P.ldm.size(); i++) {
-        size_t const b = zb_ldm_scratch_bytes(P.frames[P.ldm[i].frame].srcSize, &P.ldm[i].prm);
+        u64 const n = P.frames[P.ldm[i].frame].srcSize;
+        if (zb_ldm_survivor_cap(P.ldm[i].prefix + n, P.ldm[i].prm.minMatch) >> 32) return ZB_ERR(ZB_error_memory_allocation);   /* a survivor's index is a u32 */
+        size_t const b = zb_ldm_scratch_bytes(P.ldm[i].prefix, n, &P.ldm[i].prm);
         if (b > scratch) scratch = b;
     }
     size_t const nbBlocks = P.blocks.size();
@@ -519,9 +532,10 @@ static size_t zb_runLdm(ZSTD_CCtx* c, const ZbPlan& P, const u8* d_src, cudaStre
     for (size_t i = 0; i < P.ldm.size(); i++) {
         ZbLdmFrame const& lf = P.ldm[i];
         ZbFrame const& fr = P.frames[lf.frame];
-        CK(zb_launch_ldm(d_src + fr.srcOff, fr.srcSize, &lf.prm, c->d_ldmScratch, fr.nbBlocks, lf.matchBase, c->d_ldmMatch,
+        CK(zb_launch_ldm(d_prefix, lf.prefix, d_src + fr.srcOff, fr.srcSize, &lf.prm, c->d_ldmScratch, fr.nbBlocks, lf.matchBase, c->d_ldmMatch,
                          c->d_ldmFirst + fr.firstBlock, c->d_ldmCnt + fr.firstBlock, stream));
         *launches += 4u + 3u * ((lf.prm.hashLog - lf.prm.bucketSizeLog + 7u) / 8u);   /* split, scan, compact, radix passes, select */
+        if (lf.prefix >= lf.prm.minMatch && fr.srcSize >= lf.prm.minMatch) *launches += 1u;   /* a split launch per segment */
     }
     return 0;
 }
@@ -676,7 +690,7 @@ static size_t zb_compress(ZSTD_CCtx* c, const ZbCall& a)
     std::vector<double> hostDone(nbWaves, 0.0);
     double const hostT0 = zb_now();
     unsigned launches = 0;
-    size_t err = 0;
+    size_t err = 0, prefixUp = 0;
     if (!single) CK(cudaEventRecord(c->ev[EV_START], sCopy));
     CK(cudaMemcpyAsync(c->d_blocks, P.blocks.data(), nbBlocks * sizeof(ZbBlock), cudaMemcpyHostToDevice, sCopy));
     CK(cudaMemcpyAsync(c->d_frames, P.frames.data(), nbFrames * sizeof(ZbFrame), cudaMemcpyHostToDevice, sCopy));
@@ -689,7 +703,13 @@ static size_t zb_compress(ZSTD_CCtx* c, const ZbCall& a)
         /* host buffers: the whole input goes up first (a block may copy from any earlier wave), so this upload does not
          * overlap the kernels as the per-wave uploads do */
         if (!deviceMemory) CK(cudaMemcpyAsync(d_in, src, inEnd, cudaMemcpyHostToDevice, sCopy));
-        err = zb_runLdm(c, P, d_in, sCopy, &launches);
+        const u8* d_prefix = a.prefix;                            /* the indexed prefix: in place on the device, or uploaded like the input */
+        if (a.prefixSize && !a.prefixOnDevice) {
+            TRY(c->d_prefix.ensure(a.prefixSize));
+            CK(cudaMemcpyAsync(c->d_prefix, a.prefix, a.prefixSize, cudaMemcpyHostToDevice, sCopy));
+            d_prefix = c->d_prefix; prefixUp = a.prefixSize;
+        }
+        err = zb_runLdm(c, P, d_in, d_prefix, sCopy, &launches);
     }
     for (u32 w = 0; w < nbWaves && !err; w++) {
         u32 const b0 = wb[w], b1 = wb[w + 1];
@@ -801,7 +821,7 @@ static size_t zb_compress(ZSTD_CCtx* c, const ZbCall& a)
     } else { cudaEventElapsedTime(&ms, c->ev[EV_START], c->ev[EV_END]); c->stats.kernel_ms = ms; }
     c->stats.total_ms = c->stats.kernel_ms;
     c->stats.launches = launches; c->stats.nbBlocks = nbBlocks;
-    if (!deviceMemory) { c->stats.h2d_bytes = inEnd; c->stats.d2h_bytes = (size_t)total; }
+    if (!deviceMemory) { c->stats.h2d_bytes = inEnd + prefixUp; c->stats.d2h_bytes = (size_t)total; }
     if (total > dstCapacity) return ZB_ERR(ZB_error_dstSize_tooSmall);
     return (size_t)total;
 }
@@ -821,12 +841,39 @@ static size_t zb_digestCallDict(ZSTD_CCtx* c, const void* dict, size_t dictSize,
 /* the sticky long-distance-matching parameters of a call that honours them, or NULL when LDM is off */
 static const u32* zb_ldmArg(const ZSTD_CCtx* c) { return c->advLdm ? c->advLdmPrm : nullptr; }
 
+/* One frame against the pending prefix (ZSTD_CCtx_refPrefix, zstd_compress.c:6272-6275): the prefix is this frame's only,
+ * so it is forgotten first, whatever becomes of the call.  It is a raw-content dictionary, digested into the context's
+ * callDict (a prefix of less than 8 bytes is ignored, as any dictionary that short); with LDM on its last 2^27 bytes, all
+ * that a block can reach, are indexed along with the frame. */
+static size_t zb_compressWithPrefix(ZSTD_CCtx* c, void* dst, size_t dstCapacity, const void* src, size_t srcSize, int level,
+                                    bool deviceMemory, cudaStream_t stream)
+{
+    const u8* const prefix = c->advPrefix; size_t const size = c->advPrefixSize; bool const onDevice = c->advPrefixOnDevice;
+    c->advPrefix = NULL; c->advPrefixSize = 0;
+    if (onDevice && !deviceMemory) return ZB_ERR(ZB_error_parameter_unsupported);    /* a host-buffer call uploads what it reads */
+    if (!deviceMemory && dstCapacity && !dst) return ZB_ERR(ZB_error_dstBuffer_null);
+    if (!deviceMemory && dstCapacity < 18) return ZB_ERR(ZB_error_dstSize_tooSmall);
+    if (!c->callDict) c->callDict.reset(ZSTD_createCDict(NULL, 0, 0));
+    if (!c->callDict) return ZB_ERR(ZB_error_memory_allocation);
+    TRY(zb_digestDict(c->callDict.get(), prefix, size, true, onDevice));
+    size_t const off = 0;
+    ZbCall a = { dst, dstCapacity, src, &off, &srcSize, 1, c->callDict.get(), level, NULL, deviceMemory, stream,
+                 c->advChecksum != 0, c->advNoDictID != 0 };
+    a.ldm = zb_ldmArg(c);
+    if (a.ldm && size >= 8) {
+        u64 const reach = 1ull << ZB_LDM_WINDOW_LOG;
+        a.prefixSize = size < reach ? size : reach; a.prefix = prefix + (size - a.prefixSize); a.prefixOnDevice = onDevice;
+    }
+    return zb_compress(c, a);
+}
+
 extern "C" size_t ZSTDB200_compressFrames(ZSTD_CCtx* c, void* dst, size_t dstCapacity,
                                           const void* src, const size_t* frameOffsets, const size_t* frameSizes,
                                           size_t nbFrames, const void* dict, size_t dictSize,
                                           size_t* cSizes, int level, int deviceMemory, void* streamv)
 {
     if (!c) return ZB_ERR(ZB_error_GENERIC);
+    if (c->advPrefix) return ZB_ERR(ZB_error_parameter_unsupported);            /* "the next frame only" has no meaning for a batch */
     const ZSTD_CDict* cd;
     TRY(zb_digestCallDict(c, dict, dictSize, &cd));
     ZbCall a = { dst, dstCapacity, src, frameOffsets, frameSizes, nbFrames, cd, level, cSizes, deviceMemory != 0,
@@ -842,6 +889,7 @@ extern "C" size_t ZSTDB200_compressFrames_usingCDict(ZSTD_CCtx* c, void* dst, si
 {
     if (!cdict) return ZB_ERR(ZB_error_dictionary_wrong);                        /* zstd_compress.c:5753 */
     if (!c) return ZB_ERR(ZB_error_GENERIC);
+    if (c->advPrefix) return ZB_ERR(ZB_error_parameter_unsupported);
     ZbCall a = { dst, dstCapacity, src, frameOffsets, frameSizes, nbFrames, cdict, cdict->level, cSizes, deviceMemory != 0,
                  (cudaStream_t)streamv, c->advChecksum != 0, c->advNoDictID != 0 };
     a.ldm = zb_ldmArg(c);
@@ -911,7 +959,7 @@ extern "C" size_t ZSTDB200_compressFramePart(ZSTD_CCtx* c, void* d_dst, size_t d
     if (!c) return ZB_ERR(ZB_error_GENERIC);
     if (partBegin % ZSTDB200_framePartAlignment() || partBegin + partSize > frameSize || (partSize == 0 && frameSize != 0)) return ZB_ERR(ZB_error_srcSize_wrong);
     if (c->advChecksum) return ZB_ERR(ZB_error_parameter_unsupported);          /* a content checksum needs the whole content in one place */
-    if (c->advLdm) return ZB_ERR(ZB_error_parameter_unsupported);               /* a rank holds a halo of 128 KiB, not the LDM window */
+    if (c->advLdm || c->advPrefix) return ZB_ERR(ZB_error_parameter_unsupported);   /* a rank holds a halo of 128 KiB, not the LDM window or a prefix */
     size_t const halo = partBegin < ZB_PRIME_BYTES ? partBegin : ZB_PRIME_BYTES;
     const u8* const frameBase = (const u8*)d_part + halo - partBegin;          /* address frame offset 0 would have; only offsets >= partBegin - halo are touched */
     size_t const off = 0;
@@ -924,6 +972,7 @@ extern "C" size_t ZSTDB200_compressDevice(ZSTD_CCtx* c, void* d_dst, size_t dstC
                                           const void* d_src, size_t srcSize, int level, void* stream)
 {
     size_t const off = 0;
+    if (c && c->advPrefix) return zb_compressWithPrefix(c, d_dst, dstCapacity, d_src, srcSize, level, true, (cudaStream_t)stream);
     return ZSTDB200_compressFrames(c, d_dst, dstCapacity, d_src, &off, &srcSize, 1, NULL, 0, NULL, level, 1, stream);
 }
 
@@ -1026,7 +1075,7 @@ extern "C" size_t ZSTD_CCtx_reset(ZSTD_CCtx* c, ZSTD_ResetDirective reset)      
     if (reset == 1 || reset == 3) { c->stInSize = 0; c->stOutSize = 0; c->stOutPos = 0; c->stFrames = 0; }   /* an unfinished stream is dropped */
     if (reset == 2 || reset == 3) {
         c->advLevel = 3; c->advChecksum = 0; c->advNoDictID = 0; c->advDelims = 0; c->advLdm = 0; memset(c->advLdmPrm, 0, sizeof(c->advLdmPrm));
-        c->advLocalDict.reset(); c->advRefCDict = NULL;
+        c->advLocalDict.reset(); c->advRefCDict = NULL; c->advPrefix = NULL; c->advPrefixSize = 0;   /* ZSTD_clearAllDicts, zstd_compress.c:1360 */
     }
     return 0;
 }
@@ -1034,7 +1083,7 @@ extern "C" size_t ZSTD_CCtx_reset(ZSTD_CCtx* c, ZSTD_ResetDirective reset)      
 extern "C" size_t ZSTD_CCtx_loadDictionary(ZSTD_CCtx* c, const void* dict, size_t dictSize)  /* zstd_compress.c:1260: copied, sticky */
 {
     if (!c) return ZB_ERR(ZB_error_GENERIC);
-    c->advLocalDict.reset(); c->advRefCDict = NULL;
+    c->advLocalDict.reset(); c->advRefCDict = NULL; c->advPrefix = NULL; c->advPrefixSize = 0;
     if (!dict || dictSize == 0) return 0;                                                    /* NULL / 0: back to no dictionary */
     c->advLocalDict.reset(ZSTD_createCDict(dict, dictSize, c->advLevel));
     return c->advLocalDict ? 0 : ZB_ERR(ZB_error_dictionary_corrupted);
@@ -1043,14 +1092,29 @@ extern "C" size_t ZSTD_CCtx_loadDictionary(ZSTD_CCtx* c, const void* dict, size_
 extern "C" size_t ZSTD_CCtx_refCDict(ZSTD_CCtx* c, const ZSTD_CDict* cdict)                  /* zstd_compress.c:1330: borrowed, sticky */
 {
     if (!c) return ZB_ERR(ZB_error_GENERIC);
-    c->advLocalDict.reset();
+    c->advLocalDict.reset(); c->advPrefix = NULL; c->advPrefixSize = 0;
     c->advRefCDict = cdict;
     return 0;
 }
 
+/* zstd_compress.c:1339-1356: borrowed raw content for the next frame only; it takes the place of any dictionary, and NULL / 0
+ * leaves the context without either.  Refused inside an unfinished stream. */
+static size_t zb_refPrefix(ZSTD_CCtx* c, const void* prefix, size_t prefixSize, bool onDevice)
+{
+    if (!c) return ZB_ERR(ZB_error_GENERIC);
+    if (c->stInSize || c->stOutSize || c->stFrames) return ZB_ERR(ZB_error_stage_wrong);
+    c->advLocalDict.reset(); c->advRefCDict = NULL;
+    bool const some = prefix && prefixSize;
+    c->advPrefix = some ? (const u8*)prefix : NULL; c->advPrefixSize = some ? prefixSize : 0; c->advPrefixOnDevice = onDevice;
+    return 0;
+}
+extern "C" size_t ZSTD_CCtx_refPrefix(ZSTD_CCtx* c, const void* prefix, size_t prefixSize) { return zb_refPrefix(c, prefix, prefixSize, false); }
+extern "C" size_t ZSTDB200_CCtx_refPrefixDevice(ZSTD_CCtx* c, const void* d_prefix, size_t prefixSize) { return zb_refPrefix(c, d_prefix, prefixSize, true); }
+
 extern "C" size_t ZSTD_compress2(ZSTD_CCtx* c, void* dst, size_t dstCapacity, const void* src, size_t srcSize)     /* zstd_compress.c:6365 */
 {
     if (!c) return ZB_ERR(ZB_error_GENERIC);
+    if (c->advPrefix) return zb_compressWithPrefix(c, dst, dstCapacity, src, srcSize, c->advLevel, false, NULL);
     const ZSTD_CDict* const cd = c->advRefCDict ? c->advRefCDict : c->advLocalDict.get();
     int const level = c->advRefCDict ? c->advRefCDict->level : c->advLevel;                  /* a referenced CDict brings its own level (:5836) */
     return zb_compressOne(c, dst, dstCapacity, src, srcSize, cd, level, c->advChecksum != 0, c->advNoDictID != 0, zb_ldmArg(c));
@@ -1079,6 +1143,7 @@ static size_t zb_compressSeqs(ZSTD_CCtx* c, void* dst, size_t dstCapacity, const
                               const void* src, size_t srcSize, bool deviceMemory, cudaStream_t userStream)
 {
     if (!c) return ZB_ERR(ZB_error_GENERIC);
+    if (c->advPrefix) return ZB_ERR(ZB_error_parameter_unsupported);           /* the caller's sequences cannot reach into a prefix */
     if (dstCapacity && !dst) return ZB_ERR(ZB_error_dstBuffer_null);
     if (n && !seqs) return ZB_ERR(ZB_error_externalSequences_invalid);
     if (n > 0xFFFFFFF0u) return ZB_ERR(ZB_error_srcSize_wrong);

@@ -24,11 +24,12 @@ cudaError_t zb_launch_match(const u8* d_src, const u8* d_dictEnd, const u32* d_i
                             cudaEvent_t evMid, cudaStream_t stream, const ZbLdmView* ldm = nullptr);
 /* ldm (K1c): the launch's blocks' long-distance matches (zb_launch_ldm), laid over the parse output; NULL = none */
 
-/* Long-distance matching of one frame of n bytes at d_frame (zb_ldm.cu): nbBlocks blocks of ZB_BLOCK_MAX bytes; block k's
- * matches go to d_match[d_ldmFirst[k] .. + d_ldmCnt[k]), inside d_match[matchBase, matchBase + zb_ldm_survivor_cap(n, minMatch)).
- * d_scratch: zb_ldm_scratch_bytes(n, prm) bytes, free again when the stream reaches the end of the launch. */
-size_t zb_ldm_scratch_bytes(u64 n, const ZbLdmParams* prm);
-cudaError_t zb_launch_ldm(const u8* d_frame, u64 n, const ZbLdmParams* prm, void* d_scratch, u32 nbBlocks,
+/* Long-distance matching of one frame of n bytes at d_frame behind P indexed prefix bytes at d_prefix (P = 0: none; the two
+ * need not be adjacent) (zb_ldm.cu): nbBlocks blocks of ZB_BLOCK_MAX bytes, the frame's; block k's matches go to
+ * d_match[d_ldmFirst[k] .. + d_ldmCnt[k]), inside d_match[matchBase, matchBase + zb_ldm_survivor_cap(P + n, minMatch)).
+ * d_scratch: zb_ldm_scratch_bytes(P, n, prm) bytes, free again when the stream reaches the end of the launch. */
+size_t zb_ldm_scratch_bytes(u64 P, u64 n, const ZbLdmParams* prm);
+cudaError_t zb_launch_ldm(const u8* d_prefix, u64 P, const u8* d_frame, u64 n, const ZbLdmParams* prm, void* d_scratch, u32 nbBlocks,
                           u64 matchBase, u64* d_match, u64* d_ldmFirst, u32* d_ldmCnt, cudaStream_t stream);
 
 /* K1s: caller-supplied sequences (ZSTD_Sequence[n], 16-byte aligned, device memory) in place of K1 (zb_seqimport.cu).

@@ -1,6 +1,10 @@
 /* zb_ldm.cu — long-distance match finder (ZSTD_c_enableLongDistanceMatching): the pass that runs in front of the parse of
  * every frame of more than one chunk, so that a block can copy from anywhere in its window (up to 2^27 bytes back), not
- * only from the 128 KiB primed in front of its chunk.
+ * only from the 128 KiB primed in front of its chunk.  A frame compressed against a prefix (ZSTD_CCtx_refPrefix) has two
+ * segments: the prefix's last P bytes at positions [0, P) and the frame at [P, P + n), each in its own buffer.  L1 runs
+ * over each segment by itself (no hash or thinning across the seam) into one set of slots, the scan, compaction and sort
+ * run once over both, and L3 selects for the frame's blocks only, picking a candidate's buffer by q < P (the rule with a
+ * prefix, in plain C: oracle/zb_prefix.c).
  *
  * The rule is stated once, in plain C, in oracle/zb_ldm.c; these kernels produce the same matches bit for bit:
  *   L1  (one CTA per tile of LDM_TILE split points) gear rolling hash, split test, XXH64 of the minMatch bytes of every
@@ -14,7 +18,7 @@
  *       preceding keys of their bucket as candidates, warp-cooperative forward (32 x 8 bytes) and backward (32 bytes)
  *       counts.  The block's matches go to the match array at its first survivor's index (a block has at most one
  *       match per survivor), with their number in ldmCnt.
- * Workspace of a frame of n bytes (zb_ldm_scratch_bytes): 36 bytes per survivor for n / minMatch + 1 survivors, 16 bytes per L1
+ * Workspace of P + n bytes (zb_ldm_scratch_bytes): 36 bytes per survivor for (P + n) / minMatch + 1 survivors, 16 bytes per L1
  * slot (about as many) and the radix counts; 8 bytes per survivor for the match list (the executor's, kept for the call). */
 #include "zb_device.cuh"
 #include "zb_kernels.h"
@@ -56,10 +60,11 @@ __device__ __forceinline__ u64 zbl_xxh64(const u8* p, u32 len)
     return h;
 }
 
-/* ---- L1: splits, hashes, thinning.  Shared: v[LDM_TILE + 2H] then flags[LDM_TILE + 2H], H = minMatch - 1 ---- */
+/* ---- L1: splits, hashes, thinning of one segment src[0, n), whose first byte is position posBase and whose tiles own the
+ * slots from tileBase on.  Shared: v[LDM_TILE + 2H] then flags[LDM_TILE + 2H], H = minMatch - 1 ---- */
 __global__ void __launch_bounds__(LDM_THREADS)
-zb_ldm_split_kernel(const u8* __restrict__ src, u64 n, ZbLdmParams prm, u64* __restrict__ slotPos, u64* __restrict__ slotV, u32 slotCap,
-                    u32* __restrict__ tileCnt)
+zb_ldm_split_kernel(const u8* __restrict__ src, u64 n, u64 posBase, u32 tileBase, ZbLdmParams prm, u64* __restrict__ slotPos, u64* __restrict__ slotV,
+                    u32 slotCap, u32* __restrict__ tileCnt)
 {
     extern __shared__ u64 sV[];
     __shared__ u64 gear[256];
@@ -111,12 +116,13 @@ zb_ldm_split_kernel(const u8* __restrict__ src, u64 n, ZbLdmParams prm, u64* __r
     __syncthreads();
     u32 base = inc - c, total = 0;
     for (u32 w = 0; w < LDM_THREADS / 32u; w++) { if (w < warp) base += wsum[w]; total += wsum[w]; }
-    u64* const op = slotPos + (size_t)blockIdx.x * slotCap; u64* const ov = slotV + (size_t)blockIdx.x * slotCap;
+    u32 const tile = tileBase + blockIdx.x;
+    u64* const op = slotPos + (size_t)tile * slotCap; u64* const ov = slotV + (size_t)tile * slotCap;
     for (u32 k = 0; k < PER; k++) if (keep & (1u << k)) {
         u32 const j = H + tid * PER + k;
-        op[base] = (u64)(w0 + j); ov[base] = sV[j]; base++;
+        op[base] = posBase + (u64)(w0 + j); ov[base] = sV[j]; base++;
     }
-    if (tid == 0) tileCnt[blockIdx.x] = total;
+    if (tid == 0) tileCnt[tile] = total;
 }
 
 /* exclusive scan of in[0, m) into out[0, m], out[m] = total (one CTA; in and out may be the same array) */
@@ -234,15 +240,17 @@ __device__ __forceinline__ u32 zbl_count_back(const u8* a, const u8* b, u32 limi
     }
 }
 
+/* Positions: prefix [0, P), frame [P, P + n); block k of the frame spans [P + k * ZB_BLOCK_MAX, ...).  All lanes of a warp
+ * work on one candidate, so the choice of its buffer does not diverge. */
 __global__ void __launch_bounds__(32 * L3_WARPS)
-zb_ldm_select_kernel(const u8* __restrict__ src, u64 n, ZbLdmParams prm, const u64* __restrict__ pos, const u64* __restrict__ v,
+zb_ldm_select_kernel(const u8* __restrict__ pfx, u64 P, const u8* __restrict__ src, u64 n, ZbLdmParams prm, const u64* __restrict__ pos, const u64* __restrict__ v,
                      const u64* __restrict__ sorted, const u32* __restrict__ rank, const u32* __restrict__ nPtr, u32 nbBlocks,
                      u64 matchBase, u64* __restrict__ match, u64* __restrict__ ldmFirst, u32* __restrict__ ldmCnt)
 {
     u32 const lane = threadIdx.x & 31u, k = blockIdx.x * L3_WARPS + (threadIdx.x >> 5);
     if (k >= nbBlocks) return;
     u32 const N = *nPtr;
-    u64 const bs = (u64)k * ZB_BLOCK_MAX, be = bs + ZB_BLOCK_MAX < n ? bs + ZB_BLOCK_MAX : n;
+    u64 const bs = P + (u64)k * ZB_BLOCK_MAX, be = bs + ZB_BLOCK_MAX < P + n ? bs + ZB_BLOCK_MAX : P + n;
     u64 const W = 1ull << prm.windowLog, lowQ = be > W ? be - W : 0;
     u32 lo = 0, hi = N;                                            /* first survivor at or after bs */
     while (lo < hi) { u32 const mid = (lo + hi) >> 1; if (pos[mid] < bs) lo = mid + 1u; else hi = mid; }
@@ -262,10 +270,14 @@ zb_ldm_select_kernel(const u8* __restrict__ src, u64 n, ZbLdmParams prm, const u
             u32 const ci = (u32)c;
             u64 const q = pos[ci];
             if ((u32)(v[ci] >> 32) != ck || q < lowQ) continue;
-            u32 const f = zbl_count_fwd(src + p, src + q, (u32)(be - p), lane);
+            bool const inPfx = q < P;                                /* a prefix candidate: no match runs over the seam */
+            const u8* const pp = src + (p - P); const u8* const qq = inPfx ? pfx + q : src + (q - P);
+            u64 const fmax = (inPfx && P - q < be - p) ? P - q : be - p;
+            u32 const f = zbl_count_fwd(pp, qq, (u32)fmax, lane);
             if (f < prm.minMatch) continue;
-            u64 const bmax = (p - anchor) < q ? (p - anchor) : q;
-            u32 const b = zbl_count_back(src + p, src + q, (u32)bmax, lane);
+            u64 const qroom = inPfx ? q : q - P;
+            u64 const bmax = (p - anchor) < qroom ? (p - anchor) : qroom;
+            u32 const b = zbl_count_back(pp, qq, (u32)bmax, lane);
             if (f + b > bestLen || (f + b == bestLen && q > bestQ)) { bestLen = f + b; bestQ = q; bestF = f; bestB = b; }
         }
         if (!bestLen) continue;
@@ -278,13 +290,13 @@ zb_ldm_select_kernel(const u8* __restrict__ src, u64 n, ZbLdmParams prm, const u
 
 /* ------------------------------------------------------------------------------------------------ host */
 struct ZbLdmScratch { u64 nbTiles, slotCap, cap, nbRadixTiles; };
-static ZbLdmScratch zbl_geometry(u64 n, const ZbLdmParams* p)
+static u64 zbl_tiles(u64 n, u32 minMatch) { return n >= minMatch ? (n - minMatch + 1u + LDM_TILE - 1u) / LDM_TILE : 0u; }   /* L1 CTAs of a segment */
+static ZbLdmScratch zbl_geometry(u64 P, u64 n, const ZbLdmParams* p)
 {
     ZbLdmScratch g;
-    u64 const nbP = n >= p->minMatch ? n - p->minMatch + 1u : 0u;
-    g.nbTiles = (nbP + LDM_TILE - 1u) / LDM_TILE;
+    g.nbTiles = zbl_tiles(P, p->minMatch) + zbl_tiles(n, p->minMatch);
     g.slotCap = LDM_TILE / p->minMatch + 1u;
-    g.cap = zb_ldm_survivor_cap(n, p->minMatch);
+    g.cap = zb_ldm_survivor_cap(P + n, p->minMatch);               /* a segment of m bytes has at most m / minMatch survivors */
     g.nbRadixTiles = (g.cap + RADIX_TILE - 1u) / RADIX_TILE;
     return g;
 }
@@ -292,16 +304,16 @@ static size_t zbl_align(size_t x) { return (x + 255u) & ~(size_t)255u; }
 
 /* slots (2 x u64 per slot), tile counts / offsets (the last one is the survivor count), pos / v / keys x 2 (4 x u64 per survivor),
  * rank (u32 per survivor), radix counts */
-extern "C" size_t zb_ldm_scratch_bytes(u64 n, const ZbLdmParams* p)
+extern "C" size_t zb_ldm_scratch_bytes(u64 P, u64 n, const ZbLdmParams* p)
 {
-    ZbLdmScratch const g = zbl_geometry(n, p);
+    ZbLdmScratch const g = zbl_geometry(P, n, p);
     return zbl_align(g.nbTiles * g.slotCap * 16u) + zbl_align((g.nbTiles + 1u) * 4u) + zbl_align(g.cap * 32u) + zbl_align(g.cap * 4u) + zbl_align((256u * g.nbRadixTiles + 1u) * 4u);
 }
 
-extern "C" cudaError_t zb_launch_ldm(const u8* d_frame, u64 n, const ZbLdmParams* prm, void* d_scratch, u32 nbBlocks,
+extern "C" cudaError_t zb_launch_ldm(const u8* d_prefix, u64 P, const u8* d_frame, u64 n, const ZbLdmParams* prm, void* d_scratch, u32 nbBlocks,
                                      u64 matchBase, u64* d_match, u64* d_ldmFirst, u32* d_ldmCnt, cudaStream_t stream)
 {
-    ZbLdmScratch const g = zbl_geometry(n, prm);
+    ZbLdmScratch const g = zbl_geometry(P, n, prm);
     if (g.nbTiles == 0) return cudaMemsetAsync(d_ldmCnt, 0, nbBlocks * sizeof(u32), stream);
     u8* s = (u8*)d_scratch;
     auto take = [&](size_t bytes) { u8* const r = s; s += zbl_align(bytes); return (void*)r; };
@@ -314,7 +326,9 @@ extern "C" cudaError_t zb_launch_ldm(const u8* d_frame, u64 n, const ZbLdmParams
     size_t const smem = (size_t)span * 9u;
     cudaError_t e = cudaFuncSetAttribute(zb_ldm_split_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    zb_ldm_split_kernel<<<(u32)g.nbTiles, LDM_THREADS, smem, stream>>>(d_frame, n, *prm, slotPos, slotV, (u32)g.slotCap, tileOff);
+    u32 const tilesP = (u32)zbl_tiles(P, prm->minMatch), tilesF = (u32)g.nbTiles - tilesP;
+    if (tilesP) zb_ldm_split_kernel<<<tilesP, LDM_THREADS, smem, stream>>>(d_prefix, P, 0, 0, *prm, slotPos, slotV, (u32)g.slotCap, tileOff);
+    if (tilesF) zb_ldm_split_kernel<<<tilesF, LDM_THREADS, smem, stream>>>(d_frame, n, P, tilesP, *prm, slotPos, slotV, (u32)g.slotCap, tileOff);
     zb_ldm_scan_kernel<<<1, SCAN_THREADS_L, 0, stream>>>(tileOff, tileOff, (u32)g.nbTiles);
     u32 const* const nPtr = tileOff + g.nbTiles;
     u32 const bucketBits = prm->hashLog - prm->bucketSizeLog;
@@ -329,7 +343,7 @@ extern "C" cudaError_t zb_launch_ldm(const u8* d_frame, u64 n, const ZbLdmParams
         zb_ldm_radix_scatter_kernel<<<rgrid, 32 * RADIX_WARPS, 0, stream>>>(in, out, nPtr, shift, (u32)g.nbRadixTiles, count, ps + 1u == passes ? rank : (u32*)0);
         u64* const t = in; in = out; out = t;
     }
-    zb_ldm_select_kernel<<<(nbBlocks + L3_WARPS - 1u) / L3_WARPS, 32 * L3_WARPS, 0, stream>>>(d_frame, n, *prm, pos, v, in, rank, nPtr, nbBlocks,
+    zb_ldm_select_kernel<<<(nbBlocks + L3_WARPS - 1u) / L3_WARPS, 32 * L3_WARPS, 0, stream>>>(d_prefix, P, d_frame, n, *prm, pos, v, in, rank, nPtr, nbBlocks,
                                                                                            matchBase, d_match, d_ldmFirst, d_ldmCnt);
     return cudaGetLastError();
 }
