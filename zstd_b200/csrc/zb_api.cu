@@ -172,19 +172,14 @@ struct ZSTD_CCtx_s {
     int device;                    /* -1 until the first call created the stream and events on bindDevice */
     int bindDevice;                /* device captured by ZSTD_createCCtx */
     ZbStream stream;
-    /* per-block workspace */
     ZbDevBuf<ZbChunk> d_chunks;
-    ZbDevBuf<ZbSegMeta> d_segmeta; /* K1b -> K1c: per parse segment counts */
+    ZbDevBuf<u8> d_work;           /* per-block workspace: the rows of every slot (zb_workLayout) */
     u32 devWaveBlocks;             /* device-memory calls: blocks per wave (0 = always one wave) */
     ZbStream waveStream[ZB_WAVE_SLOTS_MAX + 1];       /* one per workspace slot, then the host path's download stream */
     u32 waveSlots;                 /* waves in flight, device-memory calls */
     u32 hostWaveSlots;             /* waves in flight, host-memory calls */
     u32 hostWaveBlocks;            /* host-memory calls: blocks per wave */
-    ZbDevBuf<ZbBlock> d_blocks; ZbDevBuf<ZbFrame> d_frames; ZbDevBuf<ZbBlockMeta> d_meta;
-    ZbDevBuf<u64> d_seqs; ZbDevBuf<u8> d_lits; ZbDevBuf<u8> d_body;
-    ZbDevBuf<u16> d_dist;          /* K1a->K1b candidate distances, then K3's FSE state records */
-    ZbDevBuf<u16> d_dist2;         /* dfast only: short-hash candidate distances */
-    ZbDevBuf<u32> d_far, d_far2;   /* candidate distances >= 0xFFFF (dist16 = ZB_FAR) */
+    ZbDevBuf<ZbBlock> d_blocks; ZbDevBuf<ZbFrame> d_frames;
     ZbDevBuf<u64> d_outOffsets, d_frameSizes;
     ZbDevBuf<u64> d_totals;        /* d_totals[w]: bytes produced up to and including wave w */
     ZbHostBuf<u64> h_totals;       /* mirror of d_totals */
@@ -283,7 +278,7 @@ extern "C" size_t ZSTD_freeCCtx(ZSTD_CCtx* c)
     return zb_deleteOnDevice(c);                                /* its dictionaries, streams, events and buffers free themselves */
 }
 
-/* descriptors (per block / per frame, small) and the heavy per-block workspace are sized separately:
+/* descriptors (per block / per frame, small) and the per-block workspace (d_work) are sized separately:
  * the host-pointer path runs the blocks in waves that share a few workspace slots */
 static size_t zb_ensureDesc(ZSTD_CCtx* c, size_t nbBlocks, size_t nbFrames, size_t nbWaves, size_t nbChunks)
 {
@@ -291,23 +286,6 @@ static size_t zb_ensureDesc(ZSTD_CCtx* c, size_t nbBlocks, size_t nbFrames, size
     TRY(c->d_blocks.ensure(nbBlocks)); TRY(c->d_outOffsets.ensure(nbBlocks + 1));
     TRY(c->d_frames.ensure(nbFrames)); TRY(c->d_frameSizes.ensure(nbFrames));
     TRY(c->d_totals.ensure(nbWaves)); TRY(c->h_totals.ensure(nbWaves));
-    return 0;
-}
-/* workspace for nbSlotBlocks blocks laid out with the strides `sd`, 256 bytes of padding behind each array */
-/* (sequence calls, needMatch = false: no candidate or segment arrays beyond the dist area that K3 uses) */
-static size_t zb_ensureHeavy(ZSTD_CCtx* c, size_t nbSlotBlocks, const ZbStrides& sd, bool needDist2, bool needMatch = true)
-{
-    size_t const nb = nbSlotBlocks, dist = nb * sd.dist;
-    auto padded = [](auto& buf, size_t n) { return buf.ensure(n + 256 / sizeof(*buf.p)); };
-    TRY(padded(c->d_meta, nb));
-    TRY(padded(c->d_seqs, nb * sd.seq));
-    TRY(padded(c->d_lits, nb * sd.lit));
-    TRY(padded(c->d_body, nb * sd.body));
-    TRY(padded(c->d_dist, dist));
-    if (needDist2) TRY(padded(c->d_dist2, dist));
-    if (needMatch) TRY(padded(c->d_segmeta, nb * ((sd.dist + ZB_PARSE_SEG - 1u) / ZB_PARSE_SEG)));
-    if (needMatch) TRY(padded(c->d_far, dist));
-    if (needDist2) TRY(padded(c->d_far2, dist));
     return 0;
 }
 
@@ -540,10 +518,10 @@ static size_t zb_runLdm(ZSTD_CCtx* c, const ZbPlan& P, const u8* d_src, const u8
     return 0;
 }
 
-/* K1..K3 for blocks [b0, b1) = chunks [c0, c1) using workspace slot positions [slot0, slot0 + (b1-b0)); d_de: the
- * dictionary's entropy tables when it is zstd-format, else NULL */
-static size_t zb_runBlocks(ZSTD_CCtx* c, const ZbPlan& P, const u8* d_src, const u8* d_dictEnd, const ZbDictEntropy* d_de, u32 b0, u32 b1, u32 c0, u32 c1, size_t slot0,
-                           cudaStream_t stream, bool timed, unsigned* launches)
+/* K1..K3 for blocks [b0, b1) = chunks [c0, c1), block b0 in the first of `rows`; d_de: the dictionary's entropy tables
+ * when it is zstd-format, else NULL */
+static size_t zb_runBlocks(ZSTD_CCtx* c, const ZbPlan& P, const u8* d_src, const u8* d_dictEnd, const ZbDictEntropy* d_de, u32 b0, u32 b1, u32 c0, u32 c1,
+                           const ZbWorkRows& rows, cudaStream_t stream, bool timed, unsigned* launches)
 {
     for (int phase = 0; phase < 3; phase++) {
         for (size_t g = 0; g < P.groups.size(); g++) {
@@ -551,21 +529,17 @@ static size_t zb_runBlocks(ZSTD_CCtx* c, const ZbPlan& P, const u8* d_src, const
             u32 const lo = G.b0 > b0 ? G.b0 : b0, hi = G.b1 < b1 ? G.b1 : b1;
             u32 const clo = G.c0 > c0 ? G.c0 : c0, chi = G.c1 < c1 ? G.c1 : c1;
             if (lo >= hi) continue;
-            size_t const s = slot0 + (lo - b0);
+            ZbWorkRows const R = rows.at(lo - b0);
             if (phase == 0) {
-                bool const df = G.prm.strategy == 2;
                 ZbLdmView lv; lv.match = c->d_ldmMatch; lv.first = c->d_ldmFirst + lo; lv.cnt = c->d_ldmCnt + lo;
-                CK(zb_launch_match(d_src, d_dictEnd, d_dictEnd ? G.image : (const u32*)0, c->d_blocks + lo, hi - lo, c->d_chunks + clo, chi - clo, lo, &G.prm, &P.sd,
-                                   c->d_dist + s * P.sd.dist, c->d_far + s * P.sd.dist, df ? c->d_dist2 + s * P.sd.dist : (u16*)0, df ? c->d_far2 + s * P.sd.dist : (u32*)0,
-                                   c->d_seqs + s * P.sd.seq, c->d_lits + s * P.sd.lit, c->d_meta + s, c->d_segmeta + s * ((P.sd.dist + ZB_PARSE_SEG - 1u) / ZB_PARSE_SEG),
+                CK(zb_launch_match(d_src, d_dictEnd, d_dictEnd ? G.image : (const u32*)0, c->d_blocks + lo, hi - lo, c->d_chunks + clo, chi - clo, lo, &G.prm, &R,
                                    (timed && P.groups.size() == 1) ? c->ev[EV_MID] : (cudaEvent_t)0, stream, G.ldm ? &lv : nullptr));
-                *launches += df ? 4 : 3;       /* walk(s), parse, merge */
+                *launches += G.prm.strategy == 2 ? 4 : 3;       /* walk(s), parse, merge */
             } else if (phase == 1) {
-                CK(zb_launch_literals(c->d_blocks + lo, hi - lo, &G.prm, &P.sd, d_de, c->d_lits + s * P.sd.lit, c->d_body + s * P.sd.body, c->d_meta + s, stream));
+                CK(zb_launch_literals(c->d_blocks + lo, hi - lo, &G.prm, &R.sd, d_de, R.lits, R.body, R.meta, stream));
                 *launches += 1;
             } else {
-                CK(zb_launch_sequences(d_src, c->d_blocks + lo, hi - lo, &G.prm, &P.sd, d_de, c->d_seqs + s * P.sd.seq, c->d_dist + s * P.sd.dist,
-                                       c->d_body + s * P.sd.body, c->d_meta + s, stream));
+                CK(zb_launch_sequences(d_src, c->d_blocks + lo, hi - lo, &G.prm, &R.sd, d_de, R.seqs, R.dist, R.body, R.meta, stream));
                 *launches += 1;
             }
         }
@@ -632,8 +606,10 @@ static size_t zb_compress(ZSTD_CCtx* c, const ZbCall& a)
     /* device-resident input: large calls are cut into waves on several streams, so that the shared-memory bound candidate
      * walk of one wave overlaps the register-only parse / entropy kernels of another.  The rule counts whole frames: a rank's
      * share of a frame (ZSTDB200_compressFramePart) goes the way the whole frame would. */
-    ZbStrides const fsd = zb_strides(P.frameMaxBlock);
-    u64 const wsBytes = P.frameBlocks * ((u64)fsd.dist * 6u + (u64)fsd.seq * 8u + fsd.lit + fsd.body);        /* one-wave workspace */
+    bool dfast = false;
+    for (size_t g = 0; g < P.groups.size(); g++) dfast |= P.groups[g].prm.strategy == 2;
+    ZbWorkKind const kind = dfast ? ZB_WORK_DFAST : ZB_WORK_FAST;
+    u64 const wsBytes = zb_workLayout(NULL, P.frameBlocks, kind, zb_strides(P.frameMaxBlock), NULL);   /* one-wave workspace */
     bool const single = deviceMemory && (a.stream || !c->devWaveBlocks ||
                                          (P.frameBytes < 2ull * c->devWaveBlocks * ZB_BLOCK_MAX && wsBytes <= (12ull << 30)));
     u32 const waveBlocks128 = deviceMemory ? c->devWaveBlocks : c->hostWaveBlocks;       /* wave size in 128 KiB blocks */
@@ -671,8 +647,10 @@ static size_t zb_compress(ZSTD_CCtx* c, const ZbCall& a)
     bool const download = !deviceMemory;
     bool const timeline = !single && getenv("ZSTDB200_TIMELINE") != NULL;      /* development: print each wave's milestones */
     TRY(zb_ensureDesc(c, nbBlocks, nbFrames, nbWaves, P.chunks.size()));
-    {   bool d2 = false; for (size_t g = 0; g < P.groups.size(); g++) d2 |= (P.groups[g].prm.strategy == 2);
-        TRY(zb_ensureHeavy(c, (size_t)slots * maxWaveBlocks, P.sd, d2)); }
+    ZbWorkRows work;                                              /* slot s = rows [s * maxWaveBlocks, (s + 1) * maxWaveBlocks) */
+    {   size_t const bytes = zb_workLayout(NULL, (size_t)slots * maxWaveBlocks, kind, P.sd, NULL);
+        TRY(bytes); TRY(c->d_work.ensure(bytes));
+        zb_workLayout(c->d_work, (size_t)slots * maxWaveBlocks, kind, P.sd, &work); }
     /* the wave events are created once and kept: a call creates none unless it has more waves than any call before it (or
      * ZSTDB200_TIMELINE changed, which wants timed events) */
     TRY(c->evH2D.ensure(nbWaves, timeline)); TRY(c->evStitch.ensure(nbWaves, timeline));
@@ -713,7 +691,7 @@ static size_t zb_compress(ZSTD_CCtx* c, const ZbCall& a)
     }
     for (u32 w = 0; w < nbWaves && !err; w++) {
         u32 const b0 = wb[w], b1 = wb[w + 1];
-        size_t const s0 = (size_t)(w % slots) * maxWaveBlocks;
+        ZbWorkRows const rows = work.at((size_t)(w % slots) * maxWaveBlocks);
         if (!deviceMemory && !ldm) {
             /* input bytes of the wave (frames are laid out in offset order; history was uploaded by earlier waves) */
             u64 lo = ~0ull, hi = 0;
@@ -728,10 +706,10 @@ static size_t zb_compress(ZSTD_CCtx* c, const ZbCall& a)
             CK(cudaStreamWaitEvent(st, c->evH2D[w], 0));
         }
         lastStream = st;
-        err = zb_runBlocks(c, P, d_in, d_dictEnd, de ? cd->d_de.p : NULL, b0, b1, wc[w], wc[w + 1], s0, st, single, &launches);
+        err = zb_runBlocks(c, P, d_in, d_dictEnd, de ? cd->d_de.p : NULL, b0, b1, wc[w], wc[w + 1], rows, st, single, &launches);
         if (err) break;
         if (w > 0) CK(cudaStreamWaitEvent(st, c->evStitch[w - 1], 0));
-        CK(zb_launch_stitch(d_in, c->d_blocks + b0, b1 - b0, c->d_frames, c->d_body + s0 * P.sd.body, P.sd.body, c->d_meta + s0,
+        CK(zb_launch_stitch(d_in, c->d_blocks + b0, b1 - b0, c->d_frames, &rows,
                             c->d_outOffsets + b0, w > 0 ? c->d_totals + (w - 1) : NULL, c->d_totals + w, d_out, outCap, st));
         launches += 2;
         if (!single) CK(cudaEventRecord(c->evStitch[w], st));
@@ -1228,7 +1206,10 @@ static size_t zb_compressSeqs(ZSTD_CCtx* c, void* dst, size_t dstCapacity, const
     u32 const waveBlocks = (c->devWaveBlocks && nbBlocks > c->devWaveBlocks) ? c->devWaveBlocks : nbBlocks;
     u32 const nbWaves = (nbBlocks + waveBlocks - 1) / waveBlocks;
     TRY(zb_ensureDesc(c, nbBlocks, 1, nbWaves, 0));
-    TRY(zb_ensureHeavy(c, waveBlocks, sd, false, false));
+    ZbWorkRows work;
+    {   size_t const bytes = zb_workLayout(NULL, waveBlocks, ZB_WORK_SEQUENCES, sd, NULL);
+        TRY(bytes); TRY(c->d_work.ensure(bytes));
+        zb_workLayout(c->d_work, waveBlocks, ZB_WORK_SEQUENCES, sd, &work); }
     u8* d_out = (u8*)dst; size_t outCap = dstCapacity;
     if (!deviceMemory) {
         size_t const bound = srcSize + 3 * (size_t)nbBlocks + 64;      /* every block at most raw: 3 header bytes each, blocks may be tiny */
@@ -1240,13 +1221,13 @@ static size_t zb_compressSeqs(ZSTD_CCtx* c, void* dst, size_t dstCapacity, const
     unsigned launches = 2 + (n ? 2u : 0u) + (expl && srcSize ? 1u : 0u);
     for (u32 w = 0; w < nbWaves; w++) {
         u32 const b0 = w * waveBlocks, nb = (b0 + waveBlocks <= nbBlocks) ? waveBlocks : nbBlocks - b0;
-        CK(zb_launch_seq_convert(d_src, c->d_blocks + b0, nb, d_first + b0, d_firstPos + b0, d_seqs, (u32)n, &prm, &sd, c->d_seqs, c->d_lits, c->d_meta, st));
+        CK(zb_launch_seq_convert(d_src, c->d_blocks + b0, nb, d_first + b0, d_firstPos + b0, d_seqs, (u32)n, &prm, &work, st));
         if (w == 0) CK(cudaEventRecord(c->ev[EV_K1], st));
-        CK(zb_launch_literals(c->d_blocks + b0, nb, &prm, &sd, de ? cd->d_de.p : NULL, c->d_lits, c->d_body, c->d_meta, st));
+        CK(zb_launch_literals(c->d_blocks + b0, nb, &prm, &sd, de ? cd->d_de.p : NULL, work.lits, work.body, work.meta, st));
         if (timed) CK(cudaEventRecord(c->ev[EV_K2], st));
-        CK(zb_launch_sequences(d_src, c->d_blocks + b0, nb, &prm, &sd, de ? cd->d_de.p : NULL, c->d_seqs, c->d_dist, c->d_body, c->d_meta, st));
+        CK(zb_launch_sequences(d_src, c->d_blocks + b0, nb, &prm, &sd, de ? cd->d_de.p : NULL, work.seqs, work.dist, work.body, work.meta, st));
         if (timed) CK(cudaEventRecord(c->ev[EV_K3], st));
-        CK(zb_launch_stitch(d_src, c->d_blocks + b0, nb, c->d_frames, c->d_body, sd.body, c->d_meta, c->d_outOffsets + b0,
+        CK(zb_launch_stitch(d_src, c->d_blocks + b0, nb, c->d_frames, &work, c->d_outOffsets + b0,
                             w > 0 ? c->d_totals + (w - 1) : NULL, c->d_totals + w, d_out, outCap, st));
         launches += 5;
     }

@@ -29,11 +29,6 @@ typedef uint64_t u64;
 #define ZB_DFAST_LONGLOG_MAX  14u            /* 64 KiB */
 #endif
 #define ZB_FAR           0xFFFFu             /* dist16 value: the distance is in the far array */
-#define ZB_MAX_SEQ       (ZB_BLOCK_MAX / 4)  /* every sequence carries a match of >= 4 bytes */
-#define ZB_SEQ_STRIDE    (ZB_MAX_SEQ + 8)    /* u64 per block */
-#define ZB_LIT_STRIDE    (ZB_BLOCK_MAX + 256)/* bytes per block */
-#define ZB_BODY_STRIDE   (ZB_BLOCK_MAX + 1024)/* staging for one compressed block body */
-#define ZB_STATE_STRIDE  (ZB_MAX_SEQ)        /* u16 per FSE stream per block (aliases the dist area: 3*32768 <= 131072) */
 
 /* block types, lib/common/zstd_internal.h:90 */
 #define ZB_BT_RAW 0
@@ -141,8 +136,8 @@ typedef struct {
     u32 codeRep[3];    /* repcode history the decoder holds at a frame's first block: {1,4,8} or the dictionary's */
 } ZbParams;
 
-/* Per-block strides of the workspace arrays of one call, derived from its largest block (M = that size
- * rounded up to 64): 128 KiB blocks use the ZB_*_STRIDE values above, a call of 1 KiB records 1/128 of them. */
+/* Per-block strides of the workspace arrays of one call, derived from its largest block (M = that size rounded up to 64):
+ * a call of 128 KiB blocks has 128 Ki dist, 32776 seq, 128 KiB + 256 lit and 128 KiB + 1 KiB body per block. */
 /* fast strategy: a block is parsed in segments of ZB_PARSE_SEG bytes, one warp each (a segment behaves like a block
  * for the parse; candidates, literals and sequences stay the block's).  Per segment, for the merge kernel: */
 #define ZB_PARSE_SEG   (16u << 10)
@@ -180,6 +175,8 @@ static inline ZB_HD ZbStrides zb_seq_strides(u32 maxBlock)
     sd.seq = M / 3u + 8u; sd.state = ((M + 2u) / 3u + 7u) & ~7u; sd.dist = 3u * sd.state;
     return sd;
 }
+/* parse segments per block row: ZbSegMeta records per block in the segmeta array (1 for calls of blocks <= 16 KiB) */
+static inline ZB_HD u32 zb_segsPerRow(const ZbStrides& sd) { return (sd.dist + ZB_PARSE_SEG - 1u) / ZB_PARSE_SEG; }
 #define ZB_SEQ_OFF_MAX ((1u << 24) - 4u)   /* largest offset of a sequence call (the packed sequence holds 28 bits of offBase; sequence calls keep this bound) */
 /* a final sequence as the sequences kernel reads it: offBase (28 bits: long-distance offsets reach 2^27), literal length
  * (18 bits), match length (18 bits, >= 3); both lengths are <= ZB_BLOCK_MAX */
@@ -214,6 +211,7 @@ typedef struct { const u64* match; const u64* first; const u32* cnt; } ZbLdmView
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdlib.h>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -248,6 +246,56 @@ template <typename T, bool Pinned> struct ZbBuf {
 };
 template <typename T> using ZbDevBuf = ZbBuf<T, false>;
 template <typename T> using ZbHostBuf = ZbBuf<T, true>;
+
+/* The compression workspace: one row per block in flight, holding what the block carries from stage to stage.
+ *   meta (K1 -> K4), seqs (K1 -> K3), lits (K1 -> K2), body (K2, K3 -> K4);
+ *   dist / far: candidate distances (K1a -> K1b), u16 per position, and u32 per position for those that need it (ZB_FAR);
+ *   dist2 / far2: the same for doubleFast's short-hash table;
+ *   segmeta: zb_segsPerRow records (K1b -> K1c).
+ * Array X's row r starts r * sd.X elements in (dist, far, dist2 and far2 use sd.dist; meta 1 and segmeta
+ * zb_segsPerRow(sd)).  Once K1b is done the candidate rows are free and later stages reuse them:
+ *   K3: a block's FSE state records, 3 x sd.state u16, in its dist row (a sequence call's dist area exists for them);
+ *   K1c with long-distance matches: the block's surviving raw sequences (at most sd.seq u64) in its far row and one u32
+ *   per survivor plus one in its dist row.
+ * Which arrays a call has depends on its kind. */
+enum ZbWorkKind { ZB_WORK_FAST, ZB_WORK_DFAST, ZB_WORK_SEQUENCES };   /* sequences: no far or segmeta; dist2 / far2: doubleFast only */
+struct ZbWorkRows {
+    ZbStrides sd;
+    ZbBlockMeta* meta; u64* seqs; u8* lits; u8* body; u16* dist; u32* far; u16* dist2; u32* far2; ZbSegMeta* segmeta;
+    /* the view moved down by `row` rows (an array the kind does not have stays NULL) */
+    ZbWorkRows at(size_t row) const {
+        ZbWorkRows r = *this;
+        auto down = [row](auto*& p, size_t stride) { if (p) p += row * stride; };
+        down(r.meta, 1); down(r.seqs, sd.seq); down(r.lits, sd.lit); down(r.body, sd.body);
+        down(r.dist, sd.dist); down(r.far, sd.dist); down(r.dist2, sd.dist); down(r.far2, sd.dist); down(r.segmeta, zb_segsPerRow(sd));
+        return r;
+    }
+};
+/* Places the arrays of `rows` rows of `kind` at the strides `sd` one behind the other from `base`, *out = the view of row 0,
+ * and returns the bytes they take (base NULL: only that size).  Every array has at least 256 bytes of padding behind it and
+ * starts 2 MiB into the buffer or a multiple of that, where an allocation of its own would start: with the arrays merely
+ * 256-byte aligned, K3 took 2 % longer (H100 80GB HBM3 at 700 W, level 3, 2 GiB in one wave).  Strides whose candidate
+ * rows cannot hold the reuse above are an error. */
+static inline size_t zb_workLayout(u8* base, size_t rows, ZbWorkKind kind, const ZbStrides& sd, ZbWorkRows* out)
+{
+    bool const match = kind != ZB_WORK_SEQUENCES;
+    if (3ull * sd.state > sd.dist) return ZB_ERR(ZB_error_GENERIC);
+    if (match && ((u64)sd.seq * 8u > (u64)sd.dist * 4u || ((u64)sd.seq + 1u) * 4u > (u64)sd.dist * 2u)) return ZB_ERR(ZB_error_GENERIC);
+    ZbWorkRows w = {};
+    w.sd = sd;
+    size_t const align = (size_t)2 << 20;
+    size_t bytes = 0;
+    auto place = [&](auto*& p, size_t n) {
+        if (base) p = reinterpret_cast<std::remove_reference_t<decltype(p)>>(base + bytes);
+        bytes = (bytes + n * sizeof(*p) + 256u + align - 1u) & ~(align - 1u);
+    };
+    place(w.meta, rows); place(w.seqs, rows * sd.seq); place(w.lits, rows * sd.lit); place(w.body, rows * sd.body);
+    place(w.dist, rows * sd.dist);
+    if (match) { place(w.far, rows * sd.dist); place(w.segmeta, rows * zb_segsPerRow(sd)); }
+    if (kind == ZB_WORK_DFAST) { place(w.dist2, rows * sd.dist); place(w.far2, rows * sd.dist); }
+    if (base) *out = w;
+    return bytes;
+}
 
 /* A non-blocking stream that a context owns, created by ensure() and destroyed with its owner.  Move-assignable, so that a
  * context can take over a stream that was created together with its events, all or nothing. */

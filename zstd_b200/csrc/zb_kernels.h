@@ -8,19 +8,18 @@
 extern "C" {
 #endif
 
-/* K1: match-finder = K1a candidate walk (one CTA per chunk) + K1b greedy parse (one warp per 16 KiB segment) + K1c merge
- * (d_segmeta: ZB_PARSE_SEGS records per block).  d_blocks / d_chunks point at the first block / chunk of the launch;
- * the launch's blocks use the workspace rows [0, nbBlocks) of the arrays passed in, slotFirstBlock = index (in the
- * call's block array) of the block that owns row 0.  Per-block workspace strides come in `sd` (ZbStrides).
- * d_dist / d_far: sd->dist u16 + u32 per block (dead after this call; K3 reuses d_dist for the FSE state records);
- * d_dist2 / d_far2: same, only used by the doubleFast strategy (short-hash candidates).
+/* Every launch of K1..K4 works on the workspace rows [0, nbBlocks) (zb_workLayout, zb_common.h), one per block of the
+ * launch: K1, K1s-b and K4 take them as `rows`.
+ * K1: match-finder = K1a candidate walk (one CTA per chunk) + K1b greedy parse (one warp per 16 KiB segment) + K1c merge.
+ * d_blocks / d_chunks point at the first block / chunk of the launch; slotFirstBlock = index (in the call's block array)
+ * of the block that owns row 0.  Writes meta, seqs and lits; dist, far, segmeta (and doubleFast's dist2, far2) are its
+ * own scratch.
  * d_dictEnd: one past the dictionary content in device memory (NULL = no dictionary); chunks / blocks with dictLen > 0
  * take the oldest dictLen bytes of their history from in front of it.  d_image (may be NULL): table already walked
  * over that dictionary tail by zb_launch_dict_image (same ZbParams), prm->tableN u32. */
 cudaError_t zb_launch_dict_image(const u8* d_dictEnd, const ZbChunk* d_dictChunk, const ZbParams* prm, u32* d_image, cudaStream_t stream);
 cudaError_t zb_launch_match(const u8* d_src, const u8* d_dictEnd, const u32* d_image, const ZbBlock* d_blocks, u32 nbBlocks,
-                            const ZbChunk* d_chunks, u32 nbChunks, u32 slotFirstBlock, const ZbParams* prm, const ZbStrides* sd,
-                            u16* d_dist, u32* d_far, u16* d_dist2, u32* d_far2, u64* d_seqs, u8* d_lits, ZbBlockMeta* d_meta, ZbSegMeta* d_segmeta,
+                            const ZbChunk* d_chunks, u32 nbChunks, u32 slotFirstBlock, const ZbParams* prm, const ZbWorkRows* rows,
                             cudaEvent_t evMid, cudaStream_t stream, const ZbLdmView* ldm = nullptr);
 /* ldm (K1c): the launch's blocks' long-distance matches (zb_launch_ldm), laid over the parse output; NULL = none */
 
@@ -38,7 +37,7 @@ cudaError_t zb_launch_ldm(const u8* d_prefix, u64 P, const u8* d_frame, u64 n, c
  * to be preset to ~0) and the block starts: explicit delimiters -> d_blockEnd / d_blockSeq per closing delimiter, else
  * d_blockFirst / d_blockFirstPos of the nbBlocks blocks of blockMax bytes (preset d_blockFirst to ~0).  blocks (explicit
  * only): the ZbBlock table, d_blockFirst / d_blockFirstPos, d_ctrl[3] = end of the last block.  convert (K1s-b): the
- * blocks' triples, literals and meta into the workspace rows [0, nbBlocks) with strides sd (zb_seq_strides). */
+ * blocks' triples, literals and meta into the workspace rows (ZB_WORK_SEQUENCES, strides zb_seq_strides). */
 cudaError_t zb_launch_seq_partition(const void* d_seqs, u32 n, int expl, u64* d_tileLen, u32* d_tileEnds, u64* d_ctrl, cudaStream_t stream);
 cudaError_t zb_launch_seq_place(const void* d_seqs, u32 n, int expl, const u64* d_tileLen, const u32* d_tileEnds,
                                 u64 srcSize, u64 window, u64 dictContent, u32 blockMax, u32 nbBlocks,
@@ -46,8 +45,7 @@ cudaError_t zb_launch_seq_place(const void* d_seqs, u32 n, int expl, const u64* 
 cudaError_t zb_launch_seq_blocks(const u64* d_blockEnd, const u32* d_blockSeq, u32 nbBlocks, u32 blockMax, u32 dictFlag,
                                  ZbBlock* d_blocks, u32* d_blockFirst, u64* d_blockFirstPos, u64* d_ctrl, cudaStream_t stream);
 cudaError_t zb_launch_seq_convert(const u8* d_src, const ZbBlock* d_blocks, u32 nbBlocks, const u32* d_blockFirst, const u64* d_blockFirstPos,
-                                  const void* d_seqs, u32 n, const ZbParams* prm, const ZbStrides* sd,
-                                  u64* d_seqOut, u8* d_lits, ZbBlockMeta* d_meta, cudaStream_t stream);
+                                  const void* d_seqs, u32 n, const ZbParams* prm, const ZbWorkRows* rows, cudaStream_t stream);
 
 /* host: the format's predefined FSE tables (zb_dict.cu), and their upload to the current device (zb_sequences.cu) */
 void zb_buildDefaultTables(ZbdFseCTable* out3);
@@ -56,6 +54,8 @@ cudaError_t zb_upload_default_tables(const ZbdFseCTable* host3, cudaStream_t str
 /* host: parse a dictionary (zb_dict.cu).  Returns the content offset, 0 for raw content, or an error code */
 size_t zb_loadDictionary(ZbDictEntropy* de, const u8* dict, size_t dictSize);
 
+/* K2 and K3 take their arrays one by one: the entropy test harness (tests/entropy_harness.cu) runs them over allocations
+ * of its own.  The driver passes the workspace rows of the launch (K3's d_stateBits: the dist rows, see zb_workLayout). */
 /* K2: literals section (histogram, Huffman table, 1/4-stream encode).  One CTA per block.
  * d_de (may be NULL): dictionary entropy state used by ZB_FLAG_DICT blocks. */
 cudaError_t zb_launch_literals(const ZbBlock* d_blocks, u32 nbBlocks, const ZbParams* prm, const ZbStrides* sd, const ZbDictEntropy* d_de,
@@ -66,11 +66,10 @@ cudaError_t zb_launch_sequences(const u8* d_src, const ZbBlock* d_blocks, u32 nb
                                 const u64* d_seqs, u16* d_stateBits, u8* d_body, ZbBlockMeta* d_meta, cudaStream_t stream);
 
 /* K4: stitch — per-block output sizes -> exclusive scan -> frame/block headers + payload copy, for
- * one wave of blocks.  d_blocks/d_meta/d_body/d_outOffsets point at the wave's first block;
+ * one wave of blocks, from the body and meta rows.  d_blocks/d_outOffsets point at the wave's first block;
  * d_outOffsets gets nbBlocks+1 absolute offsets, starting at *d_base (NULL = 0); *d_total receives
  * the running total after this wave (even past dstCapacity: nothing is written past dst+dstCapacity). */
-cudaError_t zb_launch_stitch(const u8* d_src, const ZbBlock* d_blocks, u32 nbBlocks, const ZbFrame* d_frames,
-                             const u8* d_body, u32 bodyStride, const ZbBlockMeta* d_meta,
+cudaError_t zb_launch_stitch(const u8* d_src, const ZbBlock* d_blocks, u32 nbBlocks, const ZbFrame* d_frames, const ZbWorkRows* rows,
                              u64* d_outOffsets, const u64* d_base, u64* d_total,
                              u8* d_dst, u64 dstCapacity, cudaStream_t stream);
 cudaError_t zb_launch_checksums(const u8* d_src, const ZbFrame* d_frames, u32 nbFrames, const u64* d_outOffsets, u8* d_dst, u64 dstCapacity, cudaStream_t stream);

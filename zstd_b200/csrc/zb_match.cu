@@ -383,7 +383,7 @@ zb_parse_kernel(const u8* __restrict__ src, const u8* __restrict__ dictEnd, cons
 {
     u32 const lane = threadIdx.x & 31u;
     u32 const g = blockIdx.x * PARSE_WARPS + (threadIdx.x >> 5);  /* one warp per segment: the warps of a CTA share a block's history in L1/L2 */
-    u32 const segs = (sd.dist + ZB_PARSE_SEG - 1u) / ZB_PARSE_SEG;   /* segments of the call's largest block (1 for calls of short frames) */
+    u32 const segs = zb_segsPerRow(sd);                            /* segments of the call's largest block (1 for calls of short frames) */
     u32 const b = g / segs, k = g % segs;
     if (b >= nbBlocks) return;
     ZbBlock const bd = blocks[b];
@@ -507,7 +507,7 @@ zb_parse_dfast_kernel(const u8* __restrict__ src, const u8* __restrict__ dictEnd
 {
     u32 const lane = threadIdx.x & 31u;
     u32 const g = blockIdx.x * PARSE_WARPS + (threadIdx.x >> 5);  /* one warp per segment, as in zb_parse_kernel */
-    u32 const segs = (sd.dist + ZB_PARSE_SEG - 1u) / ZB_PARSE_SEG;
+    u32 const segs = zb_segsPerRow(sd);
     u32 const b = g / segs, k = g % segs;
     if (b >= nbBlocks) return;
     ZbBlock const bd = blocks[b];
@@ -729,7 +729,7 @@ zb_merge_segments_kernel(const u8* __restrict__ src, const ZbBlock* __restrict__
     u8*  const mylit = lits + (size_t)b * sd.lit;
     const u8* const in = src + bd.srcOff;                        /* literals always lie inside the block itself */
     u32 const segs = (bd.size + ZB_PARSE_SEG - 1u) / ZB_PARSE_SEG;
-    u32 const segStride = (sd.dist + ZB_PARSE_SEG - 1u) / ZB_PARSE_SEG;
+    u32 const segStride = zb_segsPerRow(sd);
     /* ---- 1. which raw sequences survive (warp 0; positions are relative to the block) ---- */
     if (warp == 0u) {
         u32 nb = 0; u64 r0 = 0, rl = 0;
@@ -898,7 +898,7 @@ static cudaError_t zb_launch_walk(const u8* d_src, const u8* d_dictEnd, const Zb
  * followed for doubleFast by prm->tableNLong u32 of the 8-byte-hash table */
 extern "C" cudaError_t zb_launch_dict_image(const u8* d_dictEnd, const ZbChunk* d_dictChunk, const ZbParams* prm, u32* d_image, cudaStream_t stream)
 {
-    ZbStrides sd; sd.dist = ZB_BLOCK_MAX; sd.seq = ZB_SEQ_STRIDE; sd.lit = ZB_LIT_STRIDE; sd.body = ZB_BODY_STRIDE; sd.state = ZB_STATE_STRIDE;   /* unused: no block is walked */
+    ZbStrides const sd = zb_strides(ZB_BLOCK_MAX);               /* unused: no block row is written */
     cudaError_t e = zb_launch_walk(nullptr, d_dictEnd, d_dictChunk, 1, prm->mls, prm->tableN, prm->insStep, sd, 0, nullptr, nullptr, nullptr, d_image, stream);
     if (e == cudaSuccess && prm->strategy == 2)
         e = zb_launch_walk(nullptr, d_dictEnd, d_dictChunk, 1, 8, prm->tableNLong, prm->insStep, sd, 0, nullptr, nullptr, nullptr, d_image + prm->tableN, stream);
@@ -906,14 +906,15 @@ extern "C" cudaError_t zb_launch_dict_image(const u8* d_dictEnd, const ZbChunk* 
 }
 
 extern "C" cudaError_t zb_launch_match(const u8* d_src, const u8* d_dictEnd, const u32* d_image, const ZbBlock* d_blocks, u32 nbBlocks,
-                                       const ZbChunk* d_chunks, u32 nbChunks, u32 slotFirstBlock, const ZbParams* prm, const ZbStrides* sdp,
-                                       u16* d_dist, u32* d_far, u16* d_dist2, u32* d_far2, u64* d_seqs, u8* d_lits, ZbBlockMeta* d_meta, ZbSegMeta* d_segmeta,
+                                       const ZbChunk* d_chunks, u32 nbChunks, u32 slotFirstBlock, const ZbParams* prm, const ZbWorkRows* rows,
                                        cudaEvent_t evMid, cudaStream_t stream, const ZbLdmView* ldm)
 {
     if (nbBlocks == 0) return cudaSuccess;
-    ZbStrides const sd = *sdp;
+    ZbStrides const sd = rows->sd;
+    u16* const d_dist = rows->dist; u32* const d_far = rows->far; u16* const d_dist2 = rows->dist2; u32* const d_far2 = rows->far2;
+    u64* const d_seqs = rows->seqs; u8* const d_lits = rows->lits; ZbBlockMeta* const d_meta = rows->meta; ZbSegMeta* const d_segmeta = rows->segmeta;
     cudaError_t e;
-    u32 const segs = (sd.dist + ZB_PARSE_SEG - 1u) / ZB_PARSE_SEG;
+    u32 const segs = zb_segsPerRow(sd);
     u32 const sgrid = (u32)(((u64)nbBlocks * segs + PARSE_WARPS - 1) / PARSE_WARPS);                       /* one warp per segment */
     if (prm->strategy == 2) {
         /* doubleFast: one candidate walk per table */
@@ -930,7 +931,7 @@ extern "C" cudaError_t zb_launch_match(const u8* d_src, const u8* d_dictEnd, con
     }
     if (segs == 1u && sd.dist <= 8192u)
         zb_merge_small_kernel<<<(nbBlocks + MERGE_THREADS / 32u - 1u) / (MERGE_THREADS / 32u), MERGE_THREADS, 0, stream>>>(d_src, d_blocks, nbBlocks, *prm, sd, d_segmeta, d_seqs, d_lits, d_meta);
-    else if (ldm)
+    else if (ldm)                                                /* scratch in the dead candidate rows: far, then dist (zb_workLayout) */
         zb_merge_segments_kernel<true><<<nbBlocks, MERGE_THREADS, 0, stream>>>(d_src, d_blocks, *prm, sd, d_segmeta, d_seqs, d_lits, d_meta, *ldm, d_far, d_dist);
     else
         zb_merge_segments_kernel<false><<<nbBlocks, MERGE_THREADS, 0, stream>>>(d_src, d_blocks, *prm, sd, d_segmeta, d_seqs, d_lits, d_meta, ZbLdmView(), nullptr, nullptr);

@@ -245,11 +245,10 @@ extern "C" cudaError_t zb_launch_seq_blocks(const u64* d_blockEnd, const u32* d_
 }
 
 extern "C" cudaError_t zb_launch_seq_convert(const u8* d_src, const ZbBlock* d_blocks, u32 nbBlocks, const u32* d_blockFirst, const u64* d_blockFirstPos,
-                                             const void* d_seqs, u32 n, const ZbParams* prm, const ZbStrides* sd,
-                                             u64* d_seqOut, u8* d_lits, ZbBlockMeta* d_meta, cudaStream_t stream)
+                                             const void* d_seqs, u32 n, const ZbParams* prm, const ZbWorkRows* rows, cudaStream_t stream)
 {
     if (nbBlocks == 0) return cudaSuccess;
-    zb_seq_convert_kernel<<<nbBlocks, MERGE_THREADS, 0, stream>>>(d_src, d_blocks, d_blockFirst, d_blockFirstPos, (const uint4*)d_seqs, n, *prm, *sd,
-                                                                 d_seqOut, d_lits, d_meta);
+    zb_seq_convert_kernel<<<nbBlocks, MERGE_THREADS, 0, stream>>>(d_src, d_blocks, d_blockFirst, d_blockFirstPos, (const uint4*)d_seqs, n, *prm, rows->sd,
+                                                                 rows->seqs, rows->lits, rows->meta);
     return cudaGetLastError();
 }

@@ -168,12 +168,12 @@ zb_copy_small_kernel(const u8* __restrict__ src, const ZbBlock* __restrict__ blo
     for (u32 i = lane; i < m.bodySize; i += 32u) out[i] = from[i];
 }
 
-extern "C" cudaError_t zb_launch_stitch(const u8* d_src, const ZbBlock* d_blocks, u32 nbBlocks, const ZbFrame* d_frames,
-                                        const u8* d_body, u32 bodyStride, const ZbBlockMeta* d_meta,
+extern "C" cudaError_t zb_launch_stitch(const u8* d_src, const ZbBlock* d_blocks, u32 nbBlocks, const ZbFrame* d_frames, const ZbWorkRows* rows,
                                         u64* d_outOffsets, const u64* d_base, u64* d_total,
                                         u8* d_dst, u64 dstCapacity, cudaStream_t stream)
 {
     if (nbBlocks == 0) return cudaSuccess;
+    const u8* const d_body = rows->body; u32 const bodyStride = rows->sd.body; const ZbBlockMeta* const d_meta = rows->meta;
     zb_sizes_scan_kernel<<<1, SCAN_THREADS, 0, stream>>>(d_blocks, nbBlocks, d_frames, d_meta, d_outOffsets, d_base, d_total);
     if (bodyStride <= 8192u + 1024u)
         zb_copy_small_kernel<<<(nbBlocks + COPY_THREADS / 32u - 1u) / (COPY_THREADS / 32u), COPY_THREADS, 0, stream>>>(d_src, d_blocks, nbBlocks, d_frames, d_body, bodyStride, d_meta, d_outOffsets, d_dst, dstCapacity);
