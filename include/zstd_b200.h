@@ -281,6 +281,48 @@ ZSTDB200_API void ZSTDB200_getLastDStats(const ZSTD_DCtx* dctx, ZSTDB200_dstats*
 ZSTDB200_API size_t ZSTDB200_compressDevice(ZSTD_CCtx* cctx, void* d_dst, size_t dstCapacity,
                                             const void* d_src, size_t srcSize, int compressionLevel, void* stream);
 
+/* Stream-ordered compression: the call enqueues the whole compression on `stream` and returns without waiting for the GPU;
+ * the verdict lands in device memory, so the consumer of the compressed bytes (a copy, a send, the next kernel) can be
+ * queued behind it, and the call can be captured into a CUDA graph.
+ * Output: byte for byte what ZSTDB200_compressDevice produces (single frame), or ZSTDB200_compressFrames with deviceMemory = 1
+ * (ZSTDB200_compressFrames_usingCDict when cdict is not NULL) for the same inputs and context state.
+ * `stream` is the caller's cudaStream_t; NULL is the legacy default stream (PyTorch's default stream) — unlike
+ * ZSTDB200_compressDevice, where NULL selects the context's own streams.  Inputs of 256 MiB or more run as the same waves as
+ * a NULL-stream ZSTDB200_compressDevice call, on the context's wave streams, forked from and joined back into `stream`.
+ * Return value: 0 once the work is enqueued, or an error code decided before anything is enqueued: ZSTD_error_GENERIC (1)
+ * without a device or with d_result NULL, parameter_unsupported (40) for strict levels (ZSTDB200_setStrictLevels) or a
+ * pending prefix as below, memory_allocation (64), stage_wrong (60) under capture (below).
+ * *d_result (8 bytes of device, managed or mapped page-locked memory) is written by the call's last kernel, in stream order:
+ * the total compressed size, or an error code as size_t (ZSTD_isError is true for it): dstSize_tooSmall (70) when the frames
+ * do not fit, in which case nothing is written past d_dst + dstCapacity.  d_cSizes (batch call, may be NULL; same kinds of
+ * memory): the size of each frame.  frameOffsets / frameSizes are host arrays, read before the call returns.
+ * Parameters.  ZSTDB200_compressDeviceAsync honours the sticky checksum flag, dictID flag, long-distance matching and its
+ * parameters, the dictionary of ZSTD_CCtx_loadDictionary (at compressionLevel) or ZSTD_CCtx_refCDict (at the CDict's level,
+ * as ZSTD_compress2), and a device prefix (ZSTDB200_CCtx_refPrefixDevice); a pending host prefix returns 40 and is
+ * forgotten.  ZSTDB200_compressFramesAsync applies compressionLevel without a CDict and the CDict's level with one, and
+ * returns 40 while a prefix is pending.  The input, the dictionary's bytes and a CDict must stay valid until the work ran.
+ * No host wait: once an earlier call of the same or a larger shape has sized the context's buffers, made the dictionary
+ * resident and built its table images, a call neither synchronises, nor copies synchronously or from pageable memory, nor
+ * allocates or frees.  A call that has to do one of those may synchronise with the context's earlier calls.  The
+ * descriptors of a call are staged in a ring of ZSTDB200_ASYNC_SLOTS page-locked slots; the host waits when the next slot's
+ * call has not yet uploaded them (more than that many calls queued behind unfinished work).
+ * Ordering: the calls made on one context run on the GPU in the order they are made, whatever stream they name and whether
+ * they are stream-ordered or not (they share the context's workspace); ZSTD_freeCCtx waits for them.
+ * CUDA graphs: a call made while `stream` is capturing (cudaStreamCaptureModeGlobal or weaker, e.g. torch.cuda.graph) becomes
+ * part of the graph, and every replay compresses whatever bytes lie at d_src then.  Precondition: a call of the same shape
+ * (sizes, level, parameters, dictionary) on the same context before the capture, completed when the capture starts.  A call
+ * that would have to allocate, upload a dictionary or build a table image returns stage_wrong (60) before enqueuing
+ * anything.  While such a graph lives, its context must make no other call and must not be freed: replays use its workspace
+ * and descriptor slot.
+ * ZSTDB200_getLastStats after a stream-ordered call fills launches and nbBlocks only (reading the times would synchronise). */
+#define ZSTDB200_ASYNC_SLOTS 4
+ZSTDB200_API size_t ZSTDB200_compressDeviceAsync(ZSTD_CCtx* cctx, void* d_dst, size_t dstCapacity, const void* d_src, size_t srcSize,
+                                                 int compressionLevel, unsigned long long* d_result, void* stream);
+ZSTDB200_API size_t ZSTDB200_compressFramesAsync(ZSTD_CCtx* cctx, void* d_dst, size_t dstCapacity, const void* d_src,
+                                                 const size_t* frameOffsets, const size_t* frameSizes, size_t nbFrames,
+                                                 const ZSTD_CDict* cdict, int compressionLevel,
+                                                 unsigned long long* d_cSizes, unsigned long long* d_result, void* stream);
+
 /* ZSTD_CCtx_refPrefix with the prefix in device memory, for ZSTDB200_compressDevice: nothing of it crosses PCIe and no copy
  * is made (the kernels read it where it lies; it need not be adjacent to the input).  With a NULL stream the producer of
  * d_prefix must have completed before the compression call, as for d_src.  A host-buffer call (ZSTD_compress2,

@@ -124,6 +124,10 @@ def lib() -> ctypes.CDLL:
     L.ZSTD_mergeBlockDelimiters.argtypes = [_vp, _sz]
     L.ZSTDB200_compressFrames_usingCDict.restype = _sz
     L.ZSTDB200_compressFrames_usingCDict.argtypes = [_vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, ctypes.c_int, _vp]
+    L.ZSTDB200_compressDeviceAsync.restype = _sz
+    L.ZSTDB200_compressDeviceAsync.argtypes = [_vp, _vp, _sz, _vp, _sz, ctypes.c_int, _vp, _vp]
+    L.ZSTDB200_compressFramesAsync.restype = _sz
+    L.ZSTDB200_compressFramesAsync.argtypes = [_vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, ctypes.c_int, _vp, _vp, _vp]
     if hasattr(L, "ZSTD_createDCtx"):
         L.ZSTD_createDCtx.restype = _vp
         L.ZSTD_createDCtx.argtypes = []
@@ -164,6 +168,12 @@ def lib() -> ctypes.CDLL:
         L.ZSTD_DCtx_refPrefix.argtypes = [_vp, _vp, _sz]
     _lib = L
     return L
+
+
+def result_error(value: int) -> Optional[int]:
+    """The ZSTD error code a stream-ordered call left in its result word (e.g. 70, dstSize_tooSmall), or None for a size."""
+    L = lib()
+    return L.ZSTD_getErrorCode(value) if L.ZSTD_isError(value) else None
 
 
 def _check(code: int) -> int:
@@ -306,6 +316,23 @@ class ZSTD_CCtx:
     def compress_device(self, d_dst: int, dst_capacity: int, d_src: int, src_size: int, level: int = 3, stream: int = 0) -> int:
         """One frame, device pointers (ints, e.g. torch.Tensor.data_ptr()).  Returns compressed size."""
         return _check(lib().ZSTDB200_compressDevice(self._h, d_dst, dst_capacity, d_src, src_size, level, stream))
+
+    def compress_device_async(self, d_dst: int, dst_capacity: int, d_src: int, src_size: int, d_result: int, level: int = 3,
+                              stream: int = 0) -> None:
+        """ZSTDB200_compressDeviceAsync: one frame, enqueued on `stream` (a cudaStream_t as int, e.g.
+        torch.cuda.current_stream().cuda_stream; 0 = the legacy default stream).  Returns once the work is enqueued; the
+        size, or an error code, lands in the 8 bytes at d_result in stream order (see result_error)."""
+        _check(lib().ZSTDB200_compressDeviceAsync(self._h, d_dst, dst_capacity, d_src, src_size, level, d_result, stream))
+
+    def compress_frames_async(self, d_dst: int, dst_capacity: int, d_src: int, offsets: Sequence[int], sizes: Sequence[int],
+                              d_result: int, level: int = 3, cdict: Optional["ZSTD_CDict"] = None, d_c_sizes: int = 0,
+                              stream: int = 0) -> None:
+        """ZSTDB200_compressFramesAsync: many frames, enqueued on `stream`; d_c_sizes (0 = none): one u64 per frame."""
+        n = len(sizes)
+        offs = (_sz * n)(*offsets)
+        szs = (_sz * n)(*sizes)
+        _check(lib().ZSTDB200_compressFramesAsync(self._h, d_dst, dst_capacity, d_src, offs, szs, n, cdict._h if cdict else None,
+                                                  level, d_c_sizes or None, d_result, stream))
 
     def compress_frame_part(self, d_dst: int, dst_capacity: int, d_part: int, frame_size: int, part_begin: int, part_size: int,
                             level: int = 3, stream: int = 0) -> int:

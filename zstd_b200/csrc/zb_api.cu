@@ -136,15 +136,17 @@ struct ZbGroup { ZbParams prm; u32 b0, b1, c0, c1; const u32* image; bool ldm; }
  * ordinary memory is used. */
 template <typename T> struct ZbVec {
     T* p; size_t n, cap; bool pinned;
-    ZbVec() : p(NULL), n(0), cap(0), pinned(false) {}
+    bool pageable;                 /* never page-locked: growing it makes no CUDA call */
+    ZbVec() : p(NULL), n(0), cap(0), pinned(false), pageable(false) {}
     ~ZbVec() { release(); }
     ZbVec(const ZbVec&) = delete; ZbVec& operator=(const ZbVec&) = delete;
     void release() { if (p) { if (pinned) cudaFreeHost(p); else free(p); } p = NULL; n = cap = 0; }
     void reserve(size_t want) {
         if (want <= cap) return;
         size_t const c = want < 2 * cap ? 2 * cap : want;
-        T* q = NULL; bool pin = true;
-        if (cudaMallocHost((void**)&q, c * sizeof(T)) != cudaSuccess) { cudaGetLastError(); pin = false; q = (T*)malloc(c * sizeof(T)); }
+        T* q = NULL; bool pin = !pageable;
+        if (pin && cudaMallocHost((void**)&q, c * sizeof(T)) != cudaSuccess) { cudaGetLastError(); pin = false; }
+        if (!pin) q = (T*)malloc(c * sizeof(T));
         if (n) memcpy(q, p, n * sizeof(T));
         size_t const keep = n;
         release(); p = q; n = keep; cap = c; pinned = pin;
@@ -211,6 +213,13 @@ struct ZSTD_CCtx_s {
     int advDelims;
     ZbDevBuf<ZSTD_Sequence> d_seqIn;
     ZbDevBuf<u8> d_seqTile, d_seqBlk; ZbDevBuf<u64> d_seqCtrl;
+    /* stream-ordered calls (ZSTDB200_compressDeviceAsync / ZSTDB200_compressFramesAsync).  order: every call's first work
+     * waits for it, a stream-ordered call records it behind its last.  Such a call plans into asyncPlan (ordinary memory,
+     * so that planning makes no CUDA call) and stages its descriptors in a page-locked slot of a ring: slot s is free again
+     * once evStage[s], recorded behind its upload, has completed.  evJoin: one per wave stream, a wave call's join. */
+    ZbEvents order, evStage, evJoin;
+    ZbPlan asyncPlan;
+    ZbHostBuf<u8> stage[ZSTDB200_ASYNC_SLOTS]; bool stageBusy[ZSTDB200_ASYNC_SLOTS]; u32 stageNext;
 };
 
 static double zb_now(void) { struct timespec ts; clock_gettime(CLOCK_MONOTONIC, &ts); return (double)ts.tv_sec + 1e-9 * (double)ts.tv_nsec; }
@@ -236,6 +245,7 @@ extern "C" ZSTD_CCtx* ZSTD_createCCtx(void)
     c->device = -1;
     c->bindDevice = zb_contextDevice();
     c->advLevel = 3;                                                         /* ZSTD_CLEVEL_DEFAULT */
+    c->asyncPlan.blocks.pageable = c->asyncPlan.chunks.pageable = c->asyncPlan.frames.pageable = true;
     {   const char* s = getenv("ZSTDB200_SERIAL"); const char* w = getenv("ZSTDB200_WAVE_BLOCKS");
         c->devWaveBlocks = (s && atoi(s)) ? 0u : (w ? (u32)atoi(w) : 1024u);     /* 128 MiB waves x 4 slots: among the best on the H100, tests/wave_sweep.py (DESIGN.md section 11) */
         const char* n = getenv("ZSTDB200_WAVE_SLOTS"); const char* h = getenv("ZSTDB200_HOST_WAVE_BLOCKS");
@@ -259,15 +269,17 @@ static size_t zb_ctxInit(ZSTD_CCtx* c)
     CK(cudaSetDevice(dev));
     /* everything or nothing: the stream and events are the context's only once every step succeeded (device stays -1
      * until then); after a failure they are destroyed here */
-    ZbStream st; ZbEvents ev;
+    ZbStream st; ZbEvents ev, order, evStage, evJoin;
     TRY(st.ensure());
     TRY(ev.ensure(EV_PHASES, true));
+    TRY(order.ensure(1, false)); TRY(evStage.ensure(ZSTDB200_ASYNC_SLOTS, false)); TRY(evJoin.ensure(ZB_WAVE_SLOTS_MAX, false));
     /* the predefined FSE tables live in device memory (one copy per device; re-uploading the same bytes is harmless) */
     static ZbdFseCTable defaults[3]; static std::once_flag once;
     std::call_once(once, [] { zb_buildDefaultTables(defaults); });
     CK(zb_upload_default_tables(defaults, st));
     CK(cudaStreamSynchronize(st));
     c->stream = std::move(st); c->ev = std::move(ev);
+    c->order = std::move(order); c->evStage = std::move(evStage); c->evJoin = std::move(evJoin);
     c->device = dev;
     return 0;
 }
@@ -275,6 +287,11 @@ static size_t zb_ctxInit(ZSTD_CCtx* c)
 extern "C" size_t ZSTD_freeCCtx(ZSTD_CCtx* c)
 {
     if (c) { free(c->stIn); free(c->stOut); }
+    if (c && c->device >= 0) {                                  /* stream-ordered calls still queued read what is freed below */
+        ZbDeviceGuard guard;
+        cudaSetDevice(c->device);
+        cudaEventSynchronize(c->order[0]);
+    }
     return zb_deleteOnDevice(c);                                /* its dictionaries, streams, events and buffers free themselves */
 }
 
@@ -309,6 +326,9 @@ struct ZbCall {
     /* the part of a prefix that the LDM pass indexes (its last min(size, 2^27) bytes; the whole prefix is the call's cdict),
      * in host or device memory; one frame per call */
     const u8* prefix = nullptr; u64 prefixSize = 0; bool prefixOnDevice = false;
+    /* a stream-ordered call: its total (or error code) and per-frame sizes (may be NULL) go to device-writable memory, in
+     * the order of `stream`, which is then the caller's also when NULL (the legacy default stream) */
+    unsigned long long* result = nullptr; unsigned long long* d_cSizes = nullptr;
 };
 
 static int g_strictLevels = 0;
@@ -492,8 +512,8 @@ static size_t zb_buildDictImages(ZSTD_CDict* cd, ZbPlan& P, bool shared, cudaStr
 
 /* Long-distance matching (zb_ldm.cu): every LDM frame's matches, by block index in the call, before the first wave (a block
  * may copy from anywhere in its 2^27-byte window, i.e. from any earlier wave).  The frames run one after another on
- * `stream` through one scratch area. */
-static size_t zb_runLdm(ZSTD_CCtx* c, const ZbPlan& P, const u8* d_src, const u8* d_prefix, cudaStream_t stream, unsigned* launches)
+ * `stream` through one scratch area.  zb_ldmBuffers sizes the match list and that area, zb_runLdm launches. */
+static size_t zb_ldmBuffers(ZSTD_CCtx* c, const ZbPlan& P)
 {
     size_t scratch = 0;
     for (size_t i = 0; i < P.ldm.size(); i++) {
@@ -507,6 +527,10 @@ static size_t zb_runLdm(ZSTD_CCtx* c, const ZbPlan& P, const u8* d_src, const u8
     TRY(c->d_ldmFirst.ensure(nbBlocks));
     TRY(c->d_ldmCnt.ensure(nbBlocks));
     TRY(c->d_ldmScratch.ensure(scratch));
+    return 0;
+}
+static size_t zb_runLdm(ZSTD_CCtx* c, const ZbPlan& P, const u8* d_src, const u8* d_prefix, cudaStream_t stream, unsigned* launches)
+{
     for (size_t i = 0; i < P.ldm.size(); i++) {
         ZbLdmFrame const& lf = P.ldm[i];
         ZbFrame const& fr = P.frames[lf.frame];
@@ -576,32 +600,108 @@ static u64 zb_xxh64(const u8* p, size_t len)
     return h;
 }
 
+/* ------------------------------------------------------------------ stream-ordered calls
+ * zb_noAlloc for the scope of one object: set while a call sizes its buffers without growing them, and for the whole of a call
+ * that is being captured into a graph */
+struct ZbNoAlloc {
+    bool prev;
+    explicit ZbNoAlloc(bool on) : prev(zb_noAlloc) { zb_noAlloc = on; }
+    ~ZbNoAlloc() { zb_noAlloc = prev; }
+};
+
+/* whether a call under capture can use cd as it stands: no first upload, no upload that synchronises, and a table image for
+ * every parameter group that would get one (images: the call builds images) */
+static bool zb_dictWarm(ZSTD_CDict* cd, int device, bool shared, const ZbPlan& P, bool images)
+{
+    std::lock_guard<std::mutex> g(cd->lock);
+    if (cd->device != device) return false;
+    if (!cd->resident && (shared || !cd->contentOnDevice)) return false;
+    if (!images || cd->tail < 8) return true;
+    for (size_t gi = 0; gi < P.groups.size(); gi++) {
+        bool found = false;
+        for (u32 i = 0; i < cd->nbImages; i++) found |= memcmp(&cd->imagePrm[i], &P.groups[gi].prm, sizeof(ZbParams)) == 0;
+        if (!found && cd->nbImages < ZB_MAX_IMAGES) return false;
+    }
+    return true;
+}
+
+/* Copies a stream-ordered call's descriptors into the next staging slot, which its queued upload then reads: the slot is
+ * taken once the upload that last read it has run (the host waits only when the ring is full of calls still queued).  Every
+ * slot has room for them: the call's sizing grew the ring.  Under capture the wait needs the relaxed capture mode (the event
+ * was recorded outside the graph). */
+static size_t zb_stageDescriptors(ZSTD_CCtx* c, const ZbPlan& P, u32* slot, const ZbBlock** blocks, const ZbFrame** frames, const ZbChunk** chunks)
+{
+    u32 const s = c->stageNext;
+    c->stageNext = (s + 1u) % ZSTDB200_ASYNC_SLOTS;
+    if (c->stageBusy[s]) {
+        cudaStreamCaptureMode m = cudaStreamCaptureModeRelaxed;
+        CK(cudaThreadExchangeStreamCaptureMode(&m));
+        cudaError_t const e = cudaEventSynchronize(c->evStage[s]);
+        cudaThreadExchangeStreamCaptureMode(&m);
+        CK(e);
+        c->stageBusy[s] = false;
+    }
+    size_t const nb = P.blocks.size() * sizeof(ZbBlock), nf = P.frames.size() * sizeof(ZbFrame), nc = P.chunks.size() * sizeof(ZbChunk);
+    u8* const base = c->stage[s];
+    size_t const offF = (nb + 15u) & ~(size_t)15u, offC = offF + ((nf + 15u) & ~(size_t)15u);
+    memcpy(base, P.blocks.data(), nb); memcpy(base + offF, P.frames.data(), nf); memcpy(base + offC, P.chunks.data(), nc);
+    *slot = s; *blocks = (const ZbBlock*)base; *frames = (const ZbFrame*)(base + offF); *chunks = (const ZbChunk*)(base + offC);
+    return 0;
+}
+static size_t zb_stageBytes(const ZbPlan& P)
+{
+    return ((P.blocks.size() * sizeof(ZbBlock) + 15u) & ~(size_t)15u) + ((P.frames.size() * sizeof(ZbFrame) + 15u) & ~(size_t)15u)
+         + P.chunks.size() * sizeof(ZbChunk);
+}
+
 /* ------------------------------------------------------------------ the executor: every compression call, in waves
  * H2D copy of wave w+1 | kernels of waves w, w-1, ... (one stream + workspace slot each) | D2H of finished waves.
  * A block needs ~ms of latency end to end (one warp walks it), so several waves are kept in flight.
  * A device-memory call on a stream of the caller's, under ZSTDB200_SERIAL=1 or below the wave thresholds is ONE wave on
- * one stream (`single`): the upload stream is the wave stream, and events around each phase time the kernels. */
+ * one stream (`single`): the upload stream is the wave stream, and events around each phase time the kernels.
+ * A stream-ordered call (a.result) has the caller's stream as its upload stream whatever the size, forks its waves from it
+ * and joins them back into it, and ends with a kernel that writes the verdict to a.result: the host never waits for the GPU
+ * unless a buffer has to grow, a dictionary has to be uploaded or every staging slot is in flight.  Calls on one context run
+ * in the order they are made: each waits for c->order before its first work, and a stream-ordered call records it behind
+ * its last (a synchronous call is complete when it returns). */
 static size_t zb_compress(ZSTD_CCtx* c, const ZbCall& a)
 {
-    if (a.nbFrames == 0) return 0;
+    bool const async = a.result != nullptr;
+    if (a.nbFrames == 0 && !async) return 0;
     ZbDeviceGuard guard;
+    /* a stream-ordered call into a stream that is capturing a graph becomes part of the graph.  It may not allocate, free,
+     * synchronise or upload a dictionary there: where it would have to, it returns stage_wrong before enqueuing anything */
+    bool capturing = false;
+    if (async) {
+        if (c->device >= 0) CK(cudaSetDevice(c->device));
+        cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+        CK(cudaStreamIsCapturing(a.stream, &cs));
+        capturing = cs != cudaStreamCaptureStatusNone;
+        if (capturing && c->device < 0) return ZB_ERR(ZB_error_stage_wrong);
+    }
     TRY(zb_ctxInit(c));
     memset(&c->stats, 0, sizeof(c->stats));
+    ZbNoAlloc const frozen(capturing);
+    if (a.nbFrames == 0) {                                        /* a batch without frames: its total, 0, in stream order */
+        CK(zb_launch_call_result(NULL, 0, NULL, NULL, a.dstCapacity, NULL, a.result, a.stream));
+        c->stats.launches = 1;
+        return 0;
+    }
     u8* const dst = (u8*)a.dst; const u8* const src = (const u8*)a.src;
     size_t const dstCapacity = a.dstCapacity, nbFrames = a.nbFrames;
     const size_t* const frameOffsets = a.frameOffsets; const size_t* const frameSizes = a.frameSizes;
     bool const deviceMemory = a.deviceMemory;
-    cudaStream_t const sCopy = (deviceMemory && a.stream) ? a.stream : c->stream;      /* descriptors, dictionary, input */
+    cudaStream_t const sCopy = (async || (deviceMemory && a.stream)) ? a.stream : c->stream;      /* descriptors, dictionary, input */
     /* the dictionary: a caller's ZSTD_CDict, which other contexts may share (its device state is guarded by cd->lock), or
      * the context's digest of this call's bytes */
     ZSTD_CDict* const cd = (a.cdict && a.cdict->size >= 8) ? const_cast<ZSTD_CDict*>(a.cdict) : NULL;   /* zstd_compress.c:5130 : tiny dictionaries are ignored */
     bool const shared = cd != c->callDict.get();
-    if (cd) TRY(zb_residentDict(cd, c->device, shared, sCopy));
     const ZbDictEntropy* const de = (cd && cd->entropy.present) ? &cd->entropy : NULL;
-    const u8* const d_dictEnd = cd ? cd->d_dict + 32 + cd->tail : NULL;
-    ZbPlan& P = c->plan;
+    ZbPlan& P = async ? c->asyncPlan : c->plan;
     zb_plan(P, a, cd ? cd->size : 0, cd ? cd->tail : 0, de ? de->dictID : 0u, de ? de->rep : NULL);
     if (P.unsupported) return ZB_ERR(ZB_error_parameter_unsupported);
+    bool const buildImages = cd && (nbFrames >= 8 || shared);   /* a per-call digest builds its images afresh on every call: only for 8 frames or more */
+    if (capturing && cd && !zb_dictWarm(cd, c->device, shared, P, buildImages)) return ZB_ERR(ZB_error_stage_wrong);
     u32 const nbBlocks = (u32)P.blocks.size();
     /* device-resident input: large calls are cut into waves on several streams, so that the shared-memory bound candidate
      * walk of one wave overlaps the register-only parse / entropy kernels of another.  The rule counts whole frames: a rank's
@@ -610,7 +710,7 @@ static size_t zb_compress(ZSTD_CCtx* c, const ZbCall& a)
     for (size_t g = 0; g < P.groups.size(); g++) dfast |= P.groups[g].prm.strategy == 2;
     ZbWorkKind const kind = dfast ? ZB_WORK_DFAST : ZB_WORK_FAST;
     u64 const wsBytes = zb_workLayout(NULL, P.frameBlocks, kind, zb_strides(P.frameMaxBlock), NULL);   /* one-wave workspace */
-    bool const single = deviceMemory && (a.stream || !c->devWaveBlocks ||
+    bool const single = deviceMemory && ((a.stream && !async) || !c->devWaveBlocks ||
                                          (P.frameBytes < 2ull * c->devWaveBlocks * ZB_BLOCK_MAX && wsBytes <= (12ull << 30)));
     u32 const waveBlocks128 = deviceMemory ? c->devWaveBlocks : c->hostWaveBlocks;       /* wave size in 128 KiB blocks */
     u32 const ZB_WAVE_SLOTS = deviceMemory ? c->waveSlots : c->hostWaveSlots;
@@ -645,38 +745,59 @@ static size_t zb_compress(ZSTD_CCtx* c, const ZbCall& a)
     }
     size_t const outCap = deviceMemory ? dstCapacity : (dstCapacity < bound ? dstCapacity : bound);
     bool const download = !deviceMemory;
-    bool const timeline = !single && getenv("ZSTDB200_TIMELINE") != NULL;      /* development: print each wave's milestones */
-    TRY(zb_ensureDesc(c, nbBlocks, nbFrames, nbWaves, P.chunks.size()));
+    bool const timeline = !single && !async && getenv("ZSTDB200_TIMELINE") != NULL;      /* development: print each wave's milestones */
+    bool const timed = single && !async;                          /* events around each phase: a stream-ordered call reads none */
+    bool const ldm = !P.ldm.empty();
+    /* every buffer the call needs, before its first work is enqueued.  A buffer that grows frees the old one, which calls
+     * still queued on this context may read: the sizing runs once without growing anything, and only when that fails does
+     * the host wait for the context's earlier calls and size again (never under capture, where growing is refused) */
     ZbWorkRows work;                                              /* slot s = rows [s * maxWaveBlocks, (s + 1) * maxWaveBlocks) */
-    {   size_t const bytes = zb_workLayout(NULL, (size_t)slots * maxWaveBlocks, kind, P.sd, NULL);
+    size_t const stageBytes = async ? zb_stageBytes(P) : 0;
+    auto sizing = [&]() -> size_t {
+        TRY(zb_ensureDesc(c, nbBlocks, nbFrames, nbWaves, P.chunks.size()));
+        size_t const bytes = zb_workLayout(NULL, (size_t)slots * maxWaveBlocks, kind, P.sd, NULL);
         TRY(bytes); TRY(c->d_work.ensure(bytes));
-        zb_workLayout(c->d_work, (size_t)slots * maxWaveBlocks, kind, P.sd, &work); }
-    /* the wave events are created once and kept: a call creates none unless it has more waves than any call before it (or
-     * ZSTDB200_TIMELINE changed, which wants timed events) */
-    TRY(c->evH2D.ensure(nbWaves, timeline)); TRY(c->evStitch.ensure(nbWaves, timeline));
-    TRY(c->evSize.ensure(nbWaves, timeline)); TRY(c->evD2H.ensure(nbWaves, timeline));
-    /* wave streams are created on first use: every stream beyond the hardware queue count (8 by default) shares a
-     * queue with another one, and a download queued behind another wave's kernels stalls the whole pipeline */
+        zb_workLayout(c->d_work, (size_t)slots * maxWaveBlocks, kind, P.sd, &work);
+        /* the wave events are created once and kept: a call creates none unless it has more waves than any call before it (or
+         * ZSTDB200_TIMELINE changed, which wants timed events) */
+        TRY(c->evH2D.ensure(nbWaves, timeline)); TRY(c->evStitch.ensure(nbWaves, timeline));
+        TRY(c->evSize.ensure(nbWaves, timeline)); TRY(c->evD2H.ensure(nbWaves, timeline));
+        /* wave streams are created on first use: every stream beyond the hardware queue count (8 by default) shares a
+         * queue with another one, and a download queued behind another wave's kernels stalls the whole pipeline */
+        if (!single) for (u32 s = 0; s < slots; s++) TRY(c->waveStream[s].ensure());
+        if (!deviceMemory) { TRY(c->d_in.ensure(inEnd + 16)); TRY(c->d_out.ensure(outCap + 16)); TRY(c->waveStream[ZB_WAVE_SLOTS_MAX].ensure()); }
+        if (ldm) TRY(zb_ldmBuffers(c, P));
+        for (u32 s = 0; s < ZSTDB200_ASYNC_SLOTS && stageBytes; s++)
+            if (c->stage[s].cap < stageBytes) { TRY(c->stage[s].ensure(stageBytes)); c->stageBusy[s] = false; }   /* every slot, so that any can serve a capture */
+        return 0;
+    };
+    size_t sized;
+    {   ZbNoAlloc const dry(true); sized = sizing(); }
+    if (sized == ZB_ERR(ZB_error_stage_wrong) && !capturing) { CK(cudaEventSynchronize(c->order[0])); sized = sizing(); }
+    TRY(sized);
     u8* d_in; u8* d_out; cudaStream_t sD2H = (cudaStream_t)0;
     if (deviceMemory) { d_in = (u8*)src; d_out = dst; }
-    else {
-        TRY(c->d_in.ensure(inEnd + 16)); TRY(c->d_out.ensure(outCap + 16));
-        d_in = c->d_in; d_out = c->d_out;
-        TRY(c->waveStream[ZB_WAVE_SLOTS_MAX].ensure());
-        sD2H = c->waveStream[ZB_WAVE_SLOTS_MAX];
-    }
+    else { d_in = c->d_in; d_out = c->d_out; sD2H = c->waveStream[ZB_WAVE_SLOTS_MAX]; }
+    const ZbBlock* hBlocks = P.blocks.data(); const ZbFrame* hFrames = P.frames.data(); const ZbChunk* hChunks = P.chunks.data();
+    u32 stageSlot = 0;
+    if (async) TRY(zb_stageDescriptors(c, P, &stageSlot, &hBlocks, &hFrames, &hChunks));
     std::vector<double> hostDone(nbWaves, 0.0);
     double const hostT0 = zb_now();
     unsigned launches = 0;
     size_t err = 0, prefixUp = 0;
-    if (!single) CK(cudaEventRecord(c->ev[EV_START], sCopy));
-    CK(cudaMemcpyAsync(c->d_blocks, P.blocks.data(), nbBlocks * sizeof(ZbBlock), cudaMemcpyHostToDevice, sCopy));
-    CK(cudaMemcpyAsync(c->d_frames, P.frames.data(), nbFrames * sizeof(ZbFrame), cudaMemcpyHostToDevice, sCopy));
-    CK(cudaMemcpyAsync(c->d_chunks, P.chunks.data(), P.chunks.size() * sizeof(ZbChunk), cudaMemcpyHostToDevice, sCopy));
-    if (single) CK(cudaEventRecord(c->ev[EV_K0], sCopy));
-    if (cd && (nbFrames >= 8 || shared)) TRY(zb_buildDictImages(cd, P, shared, sCopy));   /* a per-call digest builds its images afresh on every call: only for 8 frames or more */
+    /* the first work: behind the context's earlier calls (an event recorded outside a graph cannot be waited for inside it:
+     * a captured call relies on them having completed, as a capture's warm-up does) */
+    if (!capturing) CK(cudaStreamWaitEvent(sCopy, c->order[0], 0));
+    if (cd) TRY(zb_residentDict(cd, c->device, shared, sCopy));
+    const u8* const d_dictEnd = cd ? cd->d_dict + 32 + cd->tail : NULL;   /* the device buffers exist from here on */
+    if (!single && !async) CK(cudaEventRecord(c->ev[EV_START], sCopy));
+    CK(cudaMemcpyAsync(c->d_blocks, hBlocks, nbBlocks * sizeof(ZbBlock), cudaMemcpyHostToDevice, sCopy));
+    CK(cudaMemcpyAsync(c->d_frames, hFrames, nbFrames * sizeof(ZbFrame), cudaMemcpyHostToDevice, sCopy));
+    CK(cudaMemcpyAsync(c->d_chunks, hChunks, P.chunks.size() * sizeof(ZbChunk), cudaMemcpyHostToDevice, sCopy));
+    if (async && !capturing) { CK(cudaEventRecord(c->evStage[stageSlot], sCopy)); c->stageBusy[stageSlot] = true; }
+    if (timed) CK(cudaEventRecord(c->ev[EV_K0], sCopy));
+    if (buildImages) TRY(zb_buildDictImages(cd, P, shared, sCopy));
     cudaStream_t lastStream = sCopy;
-    bool const ldm = !P.ldm.empty();
     if (ldm) {
         /* host buffers: the whole input goes up first (a block may copy from any earlier wave), so this upload does not
          * overlap the kernels as the per-wave uploads do */
@@ -706,7 +827,7 @@ static size_t zb_compress(ZSTD_CCtx* c, const ZbCall& a)
             CK(cudaStreamWaitEvent(st, c->evH2D[w], 0));
         }
         lastStream = st;
-        err = zb_runBlocks(c, P, d_in, d_dictEnd, de ? cd->d_de.p : NULL, b0, b1, wc[w], wc[w + 1], rows, st, single, &launches);
+        err = zb_runBlocks(c, P, d_in, d_dictEnd, de ? cd->d_de.p : NULL, b0, b1, wc[w], wc[w + 1], rows, st, timed, &launches);
         if (err) break;
         if (w > 0) CK(cudaStreamWaitEvent(st, c->evStitch[w - 1], 0));
         CK(zb_launch_stitch(d_in, c->d_blocks + b0, b1 - b0, c->d_frames, &rows,
@@ -719,6 +840,21 @@ static size_t zb_compress(ZSTD_CCtx* c, const ZbCall& a)
             CK(cudaMemcpyAsync(c->h_totals + w, c->d_totals + w, sizeof(u64), cudaMemcpyDeviceToHost, st));
             CK(cudaEventRecord(c->evSize[w], st));
         }
+    }
+    if (async) {
+        /* the tail of a stream-ordered call: the waves join the caller's stream, which then writes the checksums and the verdict */
+        if (!err) {
+            if (!single) for (u32 s = 0; s < slots; s++) {
+                CK(cudaEventRecord(c->evJoin[s], c->waveStream[s]));
+                CK(cudaStreamWaitEvent(sCopy, c->evJoin[s], 0));
+            }
+            if (a.checksum) { CK(zb_launch_checksums(d_in, c->d_frames, (u32)nbFrames, c->d_outOffsets, d_out, outCap, sCopy)); launches++; }
+            CK(zb_launch_call_result(c->d_frames, (u32)nbFrames, c->d_outOffsets, c->d_totals + nbWaves - 1, dstCapacity, a.d_cSizes, a.result, sCopy));
+            launches++;
+        }
+        if (!capturing) CK(cudaEventRecord(c->order[0], sCopy));
+        c->stats.launches = launches; c->stats.nbBlocks = nbBlocks;
+        return err;
     }
     double const hostEnq = zb_now() - hostT0;
     /* content checksums.  Host buffers: XXH64 on host threads while the GPU works (a serial recurrence per frame, one
@@ -753,7 +889,7 @@ static size_t zb_compress(ZSTD_CCtx* c, const ZbCall& a)
         CK(zb_launch_frame_sizes(c->d_frames, (u32)nbFrames, c->d_outOffsets, c->d_frameSizes, lastStream));
         if (single) launches++;                                          /* a multi-wave call's count leaves this kernel out */
     }
-    if (single) CK(cudaEventRecord(c->ev[EV_KEND], lastStream));
+    if (timed) CK(cudaEventRecord(c->ev[EV_KEND], lastStream));
     if (!err && !download && !timeline) CK(cudaMemcpyAsync(c->h_totals + nbWaves - 1, c->d_totals + nbWaves - 1, sizeof(u64), cudaMemcpyDeviceToHost, lastStream));
     if (!err && wantSizes) {
         fsz.resize(nbFrames);
@@ -822,9 +958,9 @@ static const u32* zb_ldmArg(const ZSTD_CCtx* c) { return c->advLdm ? c->advLdmPr
 /* One frame against the pending prefix (ZSTD_CCtx_refPrefix, zstd_compress.c:6272-6275): the prefix is this frame's only,
  * so it is forgotten first, whatever becomes of the call.  It is a raw-content dictionary, digested into the context's
  * callDict (a prefix of less than 8 bytes is ignored, as any dictionary that short); with LDM on its last 2^27 bytes, all
- * that a block can reach, are indexed along with the frame. */
+ * that a block can reach, are indexed along with the frame.  d_result: a stream-ordered call's verdict (NULL: synchronous). */
 static size_t zb_compressWithPrefix(ZSTD_CCtx* c, void* dst, size_t dstCapacity, const void* src, size_t srcSize, int level,
-                                    bool deviceMemory, cudaStream_t stream)
+                                    bool deviceMemory, cudaStream_t stream, unsigned long long* d_result = nullptr)
 {
     const u8* const prefix = c->advPrefix; size_t const size = c->advPrefixSize; bool const onDevice = c->advPrefixOnDevice;
     c->advPrefix = NULL; c->advPrefixSize = 0;
@@ -837,7 +973,7 @@ static size_t zb_compressWithPrefix(ZSTD_CCtx* c, void* dst, size_t dstCapacity,
     size_t const off = 0;
     ZbCall a = { dst, dstCapacity, src, &off, &srcSize, 1, c->callDict.get(), level, NULL, deviceMemory, stream,
                  c->advChecksum != 0, c->advNoDictID != 0 };
-    a.ldm = zb_ldmArg(c);
+    a.ldm = zb_ldmArg(c); a.result = d_result;
     if (a.ldm && size >= 8) {
         u64 const reach = 1ull << ZB_LDM_WINDOW_LOG;
         a.prefixSize = size < reach ? size : reach; a.prefix = prefix + (size - a.prefixSize); a.prefixOnDevice = onDevice;
@@ -952,6 +1088,37 @@ extern "C" size_t ZSTDB200_compressDevice(ZSTD_CCtx* c, void* d_dst, size_t dstC
     size_t const off = 0;
     if (c && c->advPrefix) return zb_compressWithPrefix(c, d_dst, dstCapacity, d_src, srcSize, level, true, (cudaStream_t)stream);
     return ZSTDB200_compressFrames(c, d_dst, dstCapacity, d_src, &off, &srcSize, 1, NULL, 0, NULL, level, 1, stream);
+}
+
+/* Stream-ordered calls: the bytes of ZSTDB200_compressDevice / ZSTDB200_compressFrames[_usingCDict] on device buffers, with
+ * the verdict left in device memory.  The single-frame call honours the sticky dictionary as ZSTD_compress2 does (a
+ * referenced CDict brings its level) and a device prefix; a host prefix is forgotten and refused, as a host-buffer call
+ * refuses a device prefix. */
+extern "C" size_t ZSTDB200_compressDeviceAsync(ZSTD_CCtx* c, void* d_dst, size_t dstCapacity, const void* d_src, size_t srcSize,
+                                               int level, unsigned long long* d_result, void* stream)
+{
+    if (!c || !d_result) return ZB_ERR(ZB_error_GENERIC);
+    if (c->advPrefix && !c->advPrefixOnDevice) { c->advPrefix = NULL; c->advPrefixSize = 0; return ZB_ERR(ZB_error_parameter_unsupported); }
+    if (c->advPrefix) return zb_compressWithPrefix(c, d_dst, dstCapacity, d_src, srcSize, level, true, (cudaStream_t)stream, d_result);
+    const ZSTD_CDict* const cd = c->advRefCDict ? c->advRefCDict : c->advLocalDict.get();
+    size_t const off = 0;
+    ZbCall a = { d_dst, dstCapacity, d_src, &off, &srcSize, 1, cd, c->advRefCDict ? c->advRefCDict->level : level, NULL, true,
+                 (cudaStream_t)stream, c->advChecksum != 0, c->advNoDictID != 0 };
+    a.ldm = zb_ldmArg(c); a.result = d_result;
+    return zb_compress(c, a);
+}
+
+extern "C" size_t ZSTDB200_compressFramesAsync(ZSTD_CCtx* c, void* d_dst, size_t dstCapacity, const void* d_src,
+                                               const size_t* frameOffsets, const size_t* frameSizes, size_t nbFrames,
+                                               const ZSTD_CDict* cdict, int level, unsigned long long* d_cSizes,
+                                               unsigned long long* d_result, void* stream)
+{
+    if (!c || !d_result) return ZB_ERR(ZB_error_GENERIC);
+    if (c->advPrefix) return ZB_ERR(ZB_error_parameter_unsupported);
+    ZbCall a = { d_dst, dstCapacity, d_src, frameOffsets, frameSizes, nbFrames, cdict, cdict ? cdict->level : level, NULL, true,
+                 (cudaStream_t)stream, c->advChecksum != 0, c->advNoDictID != 0 };
+    a.ldm = zb_ldmArg(c); a.result = d_result; a.d_cSizes = d_cSizes;
+    return zb_compress(c, a);
 }
 
 /* Seek table of a run of frames, in the reference's seekable format (contrib/seekable_format/
@@ -1128,6 +1295,7 @@ static size_t zb_compressSeqs(ZSTD_CCtx* c, void* dst, size_t dstCapacity, const
     ZbDeviceGuard guard;
     TRY(zb_ctxInit(c));
     memset(&c->stats, 0, sizeof(c->stats));
+    CK(cudaEventSynchronize(c->order[0]));                        /* stream-ordered calls still queued use the buffers sized below */
     const ZSTD_CDict* const cdArg = c->advRefCDict ? c->advRefCDict : c->advLocalDict.get();
     int const level = c->advRefCDict ? c->advRefCDict->level : c->advLevel;
     ZSTD_CDict* const cd = (cdArg && cdArg->size >= 8) ? const_cast<ZSTD_CDict*>(cdArg) : NULL;

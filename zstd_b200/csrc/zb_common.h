@@ -225,6 +225,10 @@ static inline bool zb_isErr(size_t c) { return c > ZB_ERR(ZB_error_maxCode); }
 /* a call that returns an error code passes it on */
 #define TRY(x) do { size_t const e_ = (x); if (zb_isErr(e_)) return e_; } while (0)
 
+/* Set on a thread while it enqueues a call into a stream that is capturing a CUDA graph: allocating or freeing is not allowed
+ * there, so every owner below refuses to grow with ZSTD_error_stage_wrong instead (the call then enqueues nothing). */
+inline thread_local bool zb_noAlloc = false;
+
 /* An array of T in device memory (cudaMalloc) or page-locked host memory (cudaMallocHost) that a context owns: grown on
  * demand, freed with the context.  cap counts elements. */
 template <typename T, bool Pinned> struct ZbBuf {
@@ -236,6 +240,7 @@ template <typename T, bool Pinned> struct ZbBuf {
     /* room for `need` elements; a larger need frees the array (its contents are not kept), then allocates need + headroom */
     size_t ensure(size_t need, size_t headroom = 0) {
         if (need <= cap) return 0;
+        if (zb_noAlloc) return ZB_ERR(ZB_error_stage_wrong);
         release();
         size_t const bytes = (need + headroom) * sizeof(T);
         CK(Pinned ? cudaMallocHost((void**)&p, bytes) : cudaMalloc((void**)&p, bytes));
@@ -304,7 +309,12 @@ struct ZbStream {
     ZbStream() = default;
     ZbStream& operator=(ZbStream&& o) { std::swap(s, o.s); return *this; }
     ~ZbStream() { if (s) cudaStreamDestroy(s); }
-    size_t ensure() { if (!s) CK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking)); return 0; }
+    size_t ensure() {
+        if (s) return 0;
+        if (zb_noAlloc) return ZB_ERR(ZB_error_stage_wrong);
+        CK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+        return 0;
+    }
     operator cudaStream_t() const { return s; }
 };
 
@@ -318,6 +328,7 @@ struct ZbEvents {
     void release() { for (cudaEvent_t e : ev) cudaEventDestroy(e); ev.clear(); }
     size_t ensure(size_t n, bool timing) {
         if (n <= ev.size() && timing == timed) return 0;
+        if (zb_noAlloc) return ZB_ERR(ZB_error_stage_wrong);
         release();
         timed = timing;
         while (ev.size() < n) {

@@ -82,6 +82,23 @@ __global__ void zb_frame_sizes_kernel(const ZbFrame* __restrict__ frames, u32 nb
     frameSizes[f] = outOffsets[fr.firstBlock + fr.nbBlocks] - outOffsets[fr.firstBlock];
 }
 
+/* the verdict of a stream-ordered call (ZSTDB200_compressDeviceAsync / ZSTDB200_compressFramesAsync), left in device memory:
+ * each frame's size (cSizes may be NULL) and the call's total, or dstSize_tooSmall when the frames did not fit in dstCapacity
+ * (K4 wrote nothing past it).  total NULL: a call without frames, whose total is 0. */
+__global__ void zb_call_result_kernel(const ZbFrame* __restrict__ frames, u32 nbFrames, const u64* __restrict__ outOffsets,
+                                      const u64* __restrict__ total, u64 dstCapacity, unsigned long long* cSizes, unsigned long long* result)
+{
+    u32 const f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (cSizes && f < nbFrames) {
+        ZbFrame const fr = frames[f];
+        cSizes[f] = outOffsets[fr.firstBlock + fr.nbBlocks] - outOffsets[fr.firstBlock];
+    }
+    if (f == 0) {
+        u64 const t = total ? *total : 0u;
+        *result = t > dstCapacity ? (unsigned long long)ZB_ERR(ZB_error_dstSize_tooSmall) : t;
+    }
+}
+
 #define COPY_THREADS 256
 __global__ void __launch_bounds__(COPY_THREADS)
 zb_copy_kernel(const u8* __restrict__ src, const ZbBlock* __restrict__ blocks, const ZbFrame* __restrict__ frames,
@@ -245,5 +262,13 @@ extern "C" cudaError_t zb_launch_frame_sizes(const ZbFrame* d_frames, u32 nbFram
 {
     if (nbFrames == 0) return cudaSuccess;
     zb_frame_sizes_kernel<<<(nbFrames + 255) / 256, 256, 0, stream>>>(d_frames, nbFrames, d_outOffsets, d_frameSizes);
+    return cudaGetLastError();
+}
+
+extern "C" cudaError_t zb_launch_call_result(const ZbFrame* d_frames, u32 nbFrames, const u64* d_outOffsets, const u64* d_total,
+                                             u64 dstCapacity, unsigned long long* d_cSizes, unsigned long long* d_result, cudaStream_t stream)
+{
+    zb_call_result_kernel<<<nbFrames ? (nbFrames + 255) / 256 : 1, 256, 0, stream>>>(d_frames, nbFrames, d_outOffsets, d_total, dstCapacity,
+                                                                                    d_cSizes, d_result);
     return cudaGetLastError();
 }
