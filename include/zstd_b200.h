@@ -256,7 +256,7 @@ ZSTDB200_API size_t ZSTD_DStreamOutSize(void);
 
 /* Decompress frames whose bytes are in device memory into device memory.  The frame / block headers are a chain that has to
  * be followed in order: for inputs of up to 512 MiB the compressed bytes are copied to a page-locked host buffer and walked
- * there, beyond that one device thread follows them (about 1 us per block); everything else is block-parallel.  Content
+ * there, beyond that one device thread follows them (1.3-1.4 us per block on an H100 80GB HBM3 at 700 W); everything else is block-parallel.  Content
  * checksums are not verified on this path.  `stream`: as for ZSTDB200_compressDevice.  Returns the decompressed size. */
 ZSTDB200_API size_t ZSTDB200_decompressDevice(ZSTD_DCtx* dctx, void* d_dst, size_t dstCapacity, const void* d_src, size_t srcSize, void* stream);
 /* same with a dictionary (host memory; uploaded by the call) */
@@ -269,6 +269,43 @@ typedef struct {
     size_t h2d_bytes, d2h_bytes;
 } ZSTDB200_dstats;
 ZSTDB200_API void ZSTDB200_getLastDStats(const ZSTD_DCtx* dctx, ZSTDB200_dstats* out);
+
+/* Stream-ordered decompression: the call enqueues the whole decompression on `stream` and returns without waiting for the
+ * GPU; the verdict lands in device memory, so the consumer of the decompressed bytes can be queued behind it, and the call
+ * can be captured into a CUDA graph.  The header walk runs on the device (one thread, fed from L1 by the rest of its CTA),
+ * so no compressed byte crosses PCIe.
+ * `stream` is the caller's cudaStream_t; NULL is the legacy default stream — unlike ZSTDB200_decompressDevice.
+ * Return value: 0 once the work is enqueued, or an error code decided before anything is enqueued: ZSTD_error_GENERIC (1)
+ * without a device or with d_result NULL, parameter_unsupported (40) while a ZSTD_DCtx_refPrefix is pending (the prefix is
+ * forgotten), memory_allocation (64), stage_wrong (60) under capture (below).
+ * *d_result (8 bytes of device, managed or mapped page-locked memory) is written by the call's last kernel, in stream order:
+ * the decompressed size, or an error code as size_t (ZSTD_isError is true for it).  For the same bytes, capacity and sticky
+ * dictionary it is what ZSTDB200_decompressDevice returns (content checksums are not verified either), but for inputs of
+ * more blocks or frames than the workspace below holds: those get workSpace_tooSmall (66), and ZSTDB200_decompressDevice
+ * decodes them.  Nothing is written outside [d_dst, d_dst + dstCapacity); with an error found before the output is placed
+ * (a corrupt header or block, a content size that does not match, dstSize_tooSmall (70)) nothing is written to d_dst.
+ * Workspace.  The host reads no header, so the context's buffers are sized from srcSize and dstCapacity alone, for up to
+ *   B = srcSize / 16 + dstCapacity / 1024 + 1024
+ * blocks and as many frames: any input whose blocks hold, on average, 16 compressed bytes or 1 KiB of content (every frame
+ * this library or the reference encoder writes of 8 bytes of content or more, and up to 1024 blocks of anything).  That
+ * costs about 7 bytes per byte of dstCapacity (literals, sequences, match positions, tiles) plus about 16 bytes per byte
+ * of srcSize (block and frame descriptors), a few GiB for a call of 1 GiB.  Buffers only grow; a context keeps them.
+ * Dictionaries: the sticky one (ZSTD_DCtx_refDDict, ZSTD_DCtx_loadDictionary) is honoured.  Its first use on a device
+ * uploads it and synchronises with the context's own stream; from then on it costs a call nothing.
+ * No host wait: once an earlier call has sized the context for this (srcSize, dstCapacity) or larger, a call neither
+ * synchronises, nor allocates, nor copies synchronously or from pageable memory.  A call that has to grow a buffer waits for
+ * the context's earlier calls; it never waits for the producer of d_src.
+ * Ordering: the calls made on one context run on the GPU in the order they are made, whatever stream they name; synchronous
+ * calls wait for the stream-ordered ones queued before them, and ZSTD_freeDCtx waits for them.  d_src must stay valid
+ * until the work ran.
+ * CUDA graphs: a call made while `stream` is capturing becomes part of the graph, and every replay decodes whatever bytes
+ * lie at d_src then.  Precondition: a completed call with the same (srcSize, dstCapacity) or larger on the same context
+ * before the capture, and a resident dictionary; otherwise the call returns stage_wrong (60) before enqueuing anything.
+ * While such a graph lives, its context makes no other call and is not freed: replays use its workspace.
+ * ZSTDB200_getLastDStats after a stream-ordered call fills launches only (reading the times would synchronise). */
+ZSTDB200_API size_t ZSTDB200_decompressDeviceAsync(ZSTD_DCtx* dctx, void* d_dst, size_t dstCapacity,
+                                                   const void* d_src, size_t srcSize,
+                                                   unsigned long long* d_result, void* stream);
 
 
 /* Compress one frame whose input and output already live in device memory (HBM).  The call returns when the frame is

@@ -143,6 +143,9 @@ def lib() -> ctypes.CDLL:
         L.ZSTD_findFrameCompressedSize.argtypes = [_vp, _sz]
         L.ZSTDB200_decompressDevice.restype = _sz
         L.ZSTDB200_decompressDevice.argtypes = [_vp, _vp, _sz, _vp, _sz, _vp]
+        if hasattr(L, "ZSTDB200_decompressDeviceAsync"):                                # absent from older development builds
+            L.ZSTDB200_decompressDeviceAsync.restype = _sz
+            L.ZSTDB200_decompressDeviceAsync.argtypes = [_vp, _vp, _sz, _vp, _sz, _vp, _vp]
         L.ZSTDB200_getLastDStats.restype = None
         L.ZSTDB200_getLastDStats.argtypes = [_vp, ctypes.POINTER(DStats)]
     if hasattr(L, "ZSTD_createDDict"):                                                  # absent from older development builds
@@ -519,6 +522,13 @@ class ZSTD_DCtx:
     def decompress_device(self, d_dst: int, dst_capacity: int, d_src: int, src_size: int, stream: int = 0) -> int:
         """Frames in device memory -> device memory (ints, e.g. torch.Tensor.data_ptr()).  Returns the decompressed size."""
         return _check(lib().ZSTDB200_decompressDevice(self._h, d_dst, dst_capacity, d_src, src_size, stream))
+
+    def decompress_device_async(self, d_dst: int, dst_capacity: int, d_src: int, src_size: int, d_result: int,
+                                stream: int = 0) -> None:
+        """ZSTDB200_decompressDeviceAsync: frames in device memory, decoded on `stream` (a cudaStream_t as int, e.g.
+        torch.cuda.current_stream().cuda_stream; 0 = the legacy default stream).  Returns once the work is enqueued; the
+        decompressed size, or an error code, lands in the 8 bytes at d_result in stream order (see result_error)."""
+        _check(lib().ZSTDB200_decompressDeviceAsync(self._h, d_dst, dst_capacity, d_src, src_size, d_result, stream))
 
     def stats(self) -> DStats:
         s = DStats()

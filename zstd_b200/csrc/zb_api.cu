@@ -600,14 +600,7 @@ static u64 zb_xxh64(const u8* p, size_t len)
     return h;
 }
 
-/* ------------------------------------------------------------------ stream-ordered calls
- * zb_noAlloc for the scope of one object: set while a call sizes its buffers without growing them, and for the whole of a call
- * that is being captured into a graph */
-struct ZbNoAlloc {
-    bool prev;
-    explicit ZbNoAlloc(bool on) : prev(zb_noAlloc) { zb_noAlloc = on; }
-    ~ZbNoAlloc() { zb_noAlloc = prev; }
-};
+/* ------------------------------------------------------------------ stream-ordered calls */
 
 /* whether a call under capture can use cd as it stands: no first upload, no upload that synchronises, and a table image for
  * every parameter group that would get one (images: the call builds images) */

@@ -228,6 +228,13 @@ static inline bool zb_isErr(size_t c) { return c > ZB_ERR(ZB_error_maxCode); }
 /* Set on a thread while it enqueues a call into a stream that is capturing a CUDA graph: allocating or freeing is not allowed
  * there, so every owner below refuses to grow with ZSTD_error_stage_wrong instead (the call then enqueues nothing). */
 inline thread_local bool zb_noAlloc = false;
+/* zb_noAlloc for the scope of one object: set while a call sizes its buffers without growing them, and for the whole of a call
+ * that is being captured into a graph */
+struct ZbNoAlloc {
+    bool prev;
+    explicit ZbNoAlloc(bool on) : prev(zb_noAlloc) { zb_noAlloc = on; }
+    ~ZbNoAlloc() { zb_noAlloc = prev; }
+};
 
 /* An array of T in device memory (cudaMalloc) or page-locked host memory (cudaMallocHost) that a context owns: grown on
  * demand, freed with the context.  cap counts elements. */

@@ -565,13 +565,16 @@ ZBD_HDN u32 zbd_decodeSequences(u64* seqs, u32 nbSeq, const u8* p, u32 size, con
  * Skippable frames are stepped over.  Returns 0 or a ZSTD error code (10 prefix_unknown, 20 corruption_detected,
  * 72 srcSize_wrong, 14 / 16 frame parameter errors). ---- */
 /* dictEntropy: the call's dictionary is a zstd-format one — a frame's first blocks may reuse its Huffman / FSE tables
- * (format: "Dictionary Format"); dictID: its ID (0 = raw content or none): a frame that names another one is refused (32). */
+ * (format: "Dictionary Format"); dictID: its ID (0 = raw content or none): a frame that names another one is refused (32).
+ * cursor (NULL on the host): the walk's position in src, published at every frame and block header, for the threads that
+ * load the bytes ahead of it (zbd_walk_kernel). */
 ZBD_HDN u32 zbd_walk(const u8* src, u64 size, ZbdBlock* blocks, u32 capB, ZbdFrame* frames, u32 capF, u32* nbB, u32* nbF, u64* litBytes, u64* seqCount,
-                     bool dictEntropy = false, u32 dictID = 0)
+                     bool dictEntropy = false, u32 dictID = 0, volatile u64* cursor = NULL)
 {
     u64 pos = 0, litPos = 0, seqPos = 0;
     u32 nb = 0, nf = 0;
     while (pos < size) {
+        if (cursor) *cursor = pos;
         ZbdFrameHeader fh;
         u32 const e = zbd_readFrameHeader(&fh, src + pos, size - pos);
         if (e) return (nf > 0 && e == 10u) ? 72u : e;             /* garbage behind a valid frame: srcSize_wrong, as the reference reports it */
@@ -591,6 +594,7 @@ ZBD_HDN u32 zbd_walk(const u8* src, u64 size, ZbdBlock* blocks, u32 capB, ZbdFra
         if (dictEntropy) { lastHuf = ZBD_DICT; for (u32 s = 0; s < 3u; s++) { lastEff[s] = 2u; lastSrc[s] = ZBD_DICT; } }
         bool first = true;
         while (true) {
+            if (cursor) *cursor = p;
             if (p + 3u > size) return 72u;
             u32 const bh = zbd_le(src + p, 3);
             u32 const last = bh & 1u, type = (bh >> 1) & 3u, bsz = bh >> 3;
