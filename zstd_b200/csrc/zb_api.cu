@@ -213,11 +213,10 @@ struct ZSTD_CCtx_s {
     int advDelims;
     ZbDevBuf<ZSTD_Sequence> d_seqIn;
     ZbDevBuf<u8> d_seqTile, d_seqBlk; ZbDevBuf<u64> d_seqCtrl;
-    /* stream-ordered calls (ZSTDB200_compressDeviceAsync / ZSTDB200_compressFramesAsync).  order: every call's first work
-     * waits for it, a stream-ordered call records it behind its last.  Such a call plans into asyncPlan (ordinary memory,
-     * so that planning makes no CUDA call) and stages its descriptors in a page-locked slot of a ring: slot s is free again
+    /* stream-ordered calls (ZSTDB200_compressDeviceAsync / ZSTDB200_compressFramesAsync) plan into asyncPlan (ordinary memory,
+     * so that planning makes no CUDA call) and stage their descriptors in a page-locked slot of a ring: slot s is free again
      * once evStage[s], recorded behind its upload, has completed.  evJoin: one per wave stream, a wave call's join. */
-    ZbEvents order, evStage, evJoin;
+    ZbOrder order; ZbEvents evStage, evJoin;
     ZbPlan asyncPlan;
     ZbHostBuf<u8> stage[ZSTDB200_ASYNC_SLOTS]; bool stageBusy[ZSTDB200_ASYNC_SLOTS]; u32 stageNext;
 };
@@ -269,10 +268,10 @@ static size_t zb_ctxInit(ZSTD_CCtx* c)
     CK(cudaSetDevice(dev));
     /* everything or nothing: the stream and events are the context's only once every step succeeded (device stays -1
      * until then); after a failure they are destroyed here */
-    ZbStream st; ZbEvents ev, order, evStage, evJoin;
+    ZbStream st; ZbEvents ev, evStage, evJoin; ZbOrder order;
     TRY(st.ensure());
     TRY(ev.ensure(EV_PHASES, true));
-    TRY(order.ensure(1, false)); TRY(evStage.ensure(ZSTDB200_ASYNC_SLOTS, false)); TRY(evJoin.ensure(ZB_WAVE_SLOTS_MAX, false));
+    TRY(order.create()); TRY(evStage.ensure(ZSTDB200_ASYNC_SLOTS, false)); TRY(evJoin.ensure(ZB_WAVE_SLOTS_MAX, false));
     /* the predefined FSE tables live in device memory (one copy per device; re-uploading the same bytes is harmless) */
     static ZbdFseCTable defaults[3]; static std::once_flag once;
     std::call_once(once, [] { zb_buildDefaultTables(defaults); });
@@ -286,13 +285,9 @@ static size_t zb_ctxInit(ZSTD_CCtx* c)
 
 extern "C" size_t ZSTD_freeCCtx(ZSTD_CCtx* c)
 {
-    if (c) { free(c->stIn); free(c->stOut); }
-    if (c && c->device >= 0) {                                  /* stream-ordered calls still queued read what is freed below */
-        ZbDeviceGuard guard;
-        cudaSetDevice(c->device);
-        cudaEventSynchronize(c->order[0]);
-    }
-    return zb_deleteOnDevice(c);                                /* its dictionaries, streams, events and buffers free themselves */
+    if (!c) return 0;
+    free(c->stIn); free(c->stOut);
+    return zb_deleteOnDevice(c, &c->order);                     /* its dictionaries, streams, events and buffers free themselves */
 }
 
 /* descriptors (per block / per frame, small) and the per-block workspace (d_work) are sized separately:
@@ -649,288 +644,293 @@ static size_t zb_stageBytes(const ZbPlan& P)
 
 /* ------------------------------------------------------------------ the executor: every compression call, in waves
  * H2D copy of wave w+1 | kernels of waves w, w-1, ... (one stream + workspace slot each) | D2H of finished waves.
- * A block needs ~ms of latency end to end (one warp walks it), so several waves are kept in flight.
- * A device-memory call on a stream of the caller's, under ZSTDB200_SERIAL=1 or below the wave thresholds is ONE wave on
- * one stream (`single`): the upload stream is the wave stream, and events around each phase time the kernels.
- * A stream-ordered call (a.result) has the caller's stream as its upload stream whatever the size, forks its waves from it
- * and joins them back into it, and ends with a kernel that writes the verdict to a.result: the host never waits for the GPU
- * unless a buffer has to grow, a dictionary has to be uploaded or every staging slot is in flight.  Calls on one context run
- * in the order they are made: each waits for c->order before its first work, and a stream-ordered call records it behind
- * its last (a synchronous call is complete when it returns). */
-static size_t zb_compress(ZSTD_CCtx* c, const ZbCall& a)
+ * A block needs ~ms of latency end to end (one warp walks it), so several waves are kept in flight. */
+struct ZbWaves {                  /* the geometry of one call */
+    bool single; ZbWorkKind kind; /* single: one wave, on the upload stream */
+    std::vector<u32> wb, wc;      /* wave w = blocks [wb[w], wb[w + 1]) = chunks [wc[w], wc[w + 1]) */
+    u32 nbWaves, maxWaveBlocks, slots;   /* workspace slot s = rows [s * maxWaveBlocks, (s + 1) * maxWaveBlocks) */
+    size_t inEnd, outCap;         /* host buffers: input bytes to upload, room of the output staging (device: dstCapacity) */
+};
+
+/* Host code only.  Device-resident input: large calls are cut into waves on several streams, so that the shared-memory
+ * bound candidate walk of one wave overlaps the register-only parse / entropy kernels of another; the rule counts whole
+ * frames (a rank's share of a frame goes the way the whole frame would).  Host buffers: the call ends when the LAST wave has
+ * gone through every kernel, so the final waves shrink (1/2, 1/4, 1/8 of a wave): less work behind the last upload. */
+static ZbWaves zb_wavePlan(const ZSTD_CCtx* c, const ZbPlan& P, const ZbCall& a)
 {
-    bool const async = a.result != nullptr;
-    if (a.nbFrames == 0 && !async) return 0;
-    ZbDeviceGuard guard;
-    /* a stream-ordered call into a stream that is capturing a graph becomes part of the graph.  It may not allocate, free,
-     * synchronise or upload a dictionary there: where it would have to, it returns stage_wrong before enqueuing anything */
-    bool capturing = false;
-    if (async) {
-        if (c->device >= 0) CK(cudaSetDevice(c->device));
-        cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-        CK(cudaStreamIsCapturing(a.stream, &cs));
-        capturing = cs != cudaStreamCaptureStatusNone;
-        if (capturing && c->device < 0) return ZB_ERR(ZB_error_stage_wrong);
-    }
-    TRY(zb_ctxInit(c));
-    memset(&c->stats, 0, sizeof(c->stats));
-    ZbNoAlloc const frozen(capturing);
-    if (a.nbFrames == 0) {                                        /* a batch without frames: its total, 0, in stream order */
-        CK(zb_launch_call_result(NULL, 0, NULL, NULL, a.dstCapacity, NULL, a.result, a.stream));
-        c->stats.launches = 1;
-        return 0;
-    }
-    u8* const dst = (u8*)a.dst; const u8* const src = (const u8*)a.src;
-    size_t const dstCapacity = a.dstCapacity, nbFrames = a.nbFrames;
-    const size_t* const frameOffsets = a.frameOffsets; const size_t* const frameSizes = a.frameSizes;
-    bool const deviceMemory = a.deviceMemory;
-    cudaStream_t const sCopy = (async || (deviceMemory && a.stream)) ? a.stream : c->stream;      /* descriptors, dictionary, input */
-    /* the dictionary: a caller's ZSTD_CDict, which other contexts may share (its device state is guarded by cd->lock), or
-     * the context's digest of this call's bytes */
-    ZSTD_CDict* const cd = (a.cdict && a.cdict->size >= 8) ? const_cast<ZSTD_CDict*>(a.cdict) : NULL;   /* zstd_compress.c:5130 : tiny dictionaries are ignored */
-    bool const shared = cd != c->callDict.get();
-    const ZbDictEntropy* const de = (cd && cd->entropy.present) ? &cd->entropy : NULL;
-    ZbPlan& P = async ? c->asyncPlan : c->plan;
-    zb_plan(P, a, cd ? cd->size : 0, cd ? cd->tail : 0, de ? de->dictID : 0u, de ? de->rep : NULL);
-    if (P.unsupported) return ZB_ERR(ZB_error_parameter_unsupported);
-    bool const buildImages = cd && (nbFrames >= 8 || shared);   /* a per-call digest builds its images afresh on every call: only for 8 frames or more */
-    if (capturing && cd && !zb_dictWarm(cd, c->device, shared, P, buildImages)) return ZB_ERR(ZB_error_stage_wrong);
-    u32 const nbBlocks = (u32)P.blocks.size();
-    /* device-resident input: large calls are cut into waves on several streams, so that the shared-memory bound candidate
-     * walk of one wave overlaps the register-only parse / entropy kernels of another.  The rule counts whole frames: a rank's
-     * share of a frame (ZSTDB200_compressFramePart) goes the way the whole frame would. */
+    ZbWaves W{};
+    u32 const nbBlocks = (u32)P.blocks.size(), nbChunks = (u32)P.chunks.size();
     bool dfast = false;
     for (size_t g = 0; g < P.groups.size(); g++) dfast |= P.groups[g].prm.strategy == 2;
-    ZbWorkKind const kind = dfast ? ZB_WORK_DFAST : ZB_WORK_FAST;
-    u64 const wsBytes = zb_workLayout(NULL, P.frameBlocks, kind, zb_strides(P.frameMaxBlock), NULL);   /* one-wave workspace */
-    bool const single = deviceMemory && ((a.stream && !async) || !c->devWaveBlocks ||
-                                         (P.frameBytes < 2ull * c->devWaveBlocks * ZB_BLOCK_MAX && wsBytes <= (12ull << 30)));
-    u32 const waveBlocks128 = deviceMemory ? c->devWaveBlocks : c->hostWaveBlocks;       /* wave size in 128 KiB blocks */
-    u32 const ZB_WAVE_SLOTS = deviceMemory ? c->waveSlots : c->hostWaveSlots;
+    W.kind = dfast ? ZB_WORK_DFAST : ZB_WORK_FAST;
+    u64 const wsBytes = zb_workLayout(NULL, P.frameBlocks, W.kind, zb_strides(P.frameMaxBlock), NULL);   /* one-wave workspace */
+    W.single = a.deviceMemory && ((a.stream && !a.result) || !c->devWaveBlocks ||
+                                  (P.frameBytes < 2ull * c->devWaveBlocks * ZB_BLOCK_MAX && wsBytes <= (12ull << 30)));
+    u32 const waveBlocks128 = a.deviceMemory ? c->devWaveBlocks : c->hostWaveBlocks;       /* wave size in 128 KiB blocks */
+    u32 const waveSlots = a.deviceMemory ? c->waveSlots : c->hostWaveSlots;
     /* a wave is sized in bytes of input (and of workspace): calls made of small blocks get proportionally more blocks per wave */
-    u32 const ZB_WAVE_BLOCKS = single ? nbBlocks : (u32)((u64)waveBlocks128 * (ZB_BLOCK_MAX / P.sd.dist) > (1u << 22) ? (1u << 22) : waveBlocks128 * (ZB_BLOCK_MAX / P.sd.dist));
-    /* wave boundaries.  Host path: the call ends when the LAST wave has gone through every kernel, so the
-     * final waves shrink (1/2, 1/4, 1/8 of a wave): less work behind the last upload. */
-    std::vector<u32> wb, wc;                                      /* wave w = blocks [wb[w], wb[w+1]) = chunks [wc[w], wc[w+1]) */
-    {   std::vector<u32> tail, target;
-        u32 left = nbBlocks;
-        if (!deviceMemory) for (u32 sz = ZB_WAVE_BLOCKS / 8u; sz >= 32u && sz < ZB_WAVE_BLOCKS && left > 2u * sz; sz *= 2u) { tail.push_back(sz); left -= sz; }
-        for (u32 b = 0; b < left; ) { u32 const e = (left - b > ZB_WAVE_BLOCKS) ? b + ZB_WAVE_BLOCKS : left; target.push_back(e - b); b = e; }
-        for (size_t i = tail.size(); i-- > 0; ) target.push_back(tail[i]);
-        /* a chunk is never split between waves: waves are filled chunk by chunk up to their target size */
-        wb.push_back(0); wc.push_back(0);
-        u32 acc = 0; size_t ti = 0;
-        for (u32 ci = 0; ci < (u32)P.chunks.size(); ci++) {
-            u32 const nextFirst = ci + 1u < (u32)P.chunks.size() ? P.chunks[ci + 1u].firstBlock : nbBlocks;
-            acc += nextFirst - P.chunks[ci].firstBlock;
-            if (ti < target.size() && acc >= target[ti] && ci + 1u < (u32)P.chunks.size()) { wb.push_back(nextFirst); wc.push_back(ci + 1u); acc = 0; ti++; }
-        }
-        wb.push_back(nbBlocks); wc.push_back((u32)P.chunks.size());
+    u32 const waveBlocks = W.single ? nbBlocks : (u32)((u64)waveBlocks128 * (ZB_BLOCK_MAX / P.sd.dist) > (1u << 22) ? (1u << 22) : waveBlocks128 * (ZB_BLOCK_MAX / P.sd.dist));
+    std::vector<u32> tail, target;
+    u32 left = nbBlocks;
+    if (!a.deviceMemory) for (u32 sz = waveBlocks / 8u; sz >= 32u && sz < waveBlocks && left > 2u * sz; sz *= 2u) { tail.push_back(sz); left -= sz; }
+    for (u32 b = 0; b < left; ) { u32 const e = (left - b > waveBlocks) ? b + waveBlocks : left; target.push_back(e - b); b = e; }
+    for (size_t i = tail.size(); i-- > 0; ) target.push_back(tail[i]);
+    /* a chunk is never split between waves: waves are filled chunk by chunk up to their target size */
+    W.wb.push_back(0); W.wc.push_back(0);
+    u32 acc = 0; size_t ti = 0;
+    for (u32 ci = 0; ci < nbChunks; ci++) {
+        u32 const nextFirst = ci + 1u < nbChunks ? P.chunks[ci + 1u].firstBlock : nbBlocks;
+        acc += nextFirst - P.chunks[ci].firstBlock;
+        if (ti < target.size() && acc >= target[ti] && ci + 1u < nbChunks) { W.wb.push_back(nextFirst); W.wc.push_back(ci + 1u); acc = 0; ti++; }
     }
-    u32 maxWaveBlocks = 0;
-    for (size_t w = 0; w + 1 < wb.size(); w++) if (wb[w + 1] - wb[w] > maxWaveBlocks) maxWaveBlocks = wb[w + 1] - wb[w];
-    u32 const nbWaves = (u32)wb.size() - 1u;
-    u32 const slots = nbWaves < ZB_WAVE_SLOTS ? nbWaves : ZB_WAVE_SLOTS;
-    size_t inEnd = 0, bound = 0;
-    if (!deviceMemory) for (size_t f = 0; f < nbFrames; f++) {
-        if (frameOffsets[f] + frameSizes[f] > inEnd) inEnd = frameOffsets[f] + frameSizes[f];
-        bound += ZSTD_compressBound(frameSizes[f]) + 32;
+    W.wb.push_back(nbBlocks); W.wc.push_back(nbChunks);
+    W.nbWaves = (u32)W.wb.size() - 1u;
+    for (u32 w = 0; w < W.nbWaves; w++) if (W.wb[w + 1] - W.wb[w] > W.maxWaveBlocks) W.maxWaveBlocks = W.wb[w + 1] - W.wb[w];
+    W.slots = W.nbWaves < waveSlots ? W.nbWaves : waveSlots;
+    size_t bound = 0;
+    if (!a.deviceMemory) for (size_t f = 0; f < a.nbFrames; f++) {
+        if (a.frameOffsets[f] + a.frameSizes[f] > W.inEnd) W.inEnd = a.frameOffsets[f] + a.frameSizes[f];
+        bound += ZSTD_compressBound(a.frameSizes[f]) + 32;
     }
-    size_t const outCap = deviceMemory ? dstCapacity : (dstCapacity < bound ? dstCapacity : bound);
-    bool const download = !deviceMemory;
-    bool const timeline = !single && !async && getenv("ZSTDB200_TIMELINE") != NULL;      /* development: print each wave's milestones */
-    bool const timed = single && !async;                          /* events around each phase: a stream-ordered call reads none */
-    bool const ldm = !P.ldm.empty();
-    /* every buffer the call needs, before its first work is enqueued.  A buffer that grows frees the old one, which calls
-     * still queued on this context may read: the sizing runs once without growing anything, and only when that fails does
-     * the host wait for the context's earlier calls and size again (never under capture, where growing is refused) */
-    ZbWorkRows work;                                              /* slot s = rows [s * maxWaveBlocks, (s + 1) * maxWaveBlocks) */
-    size_t const stageBytes = async ? zb_stageBytes(P) : 0;
-    auto sizing = [&]() -> size_t {
-        TRY(zb_ensureDesc(c, nbBlocks, nbFrames, nbWaves, P.chunks.size()));
-        size_t const bytes = zb_workLayout(NULL, (size_t)slots * maxWaveBlocks, kind, P.sd, NULL);
+    W.outCap = a.deviceMemory ? a.dstCapacity : (a.dstCapacity < bound ? a.dstCapacity : bound);
+    return W;
+}
+
+/* One compression call as its stages see it: zb_compress plans it (zb_plan, zb_wavePlan), sizes its buffers, enqueues it and
+ * ends it in one of three ways (DESIGN.md section 2) */
+struct ZbRun {
+    ZSTD_CCtx* c; const ZbCall& a; ZbPlan& P; ZbWaves W;
+    ZSTD_CDict* cd; bool shared, buildImages;       /* the dictionary; shared: a caller's CDict, which other contexts may use */
+    cudaStream_t sCopy;                             /* descriptors, dictionary, input */
+    bool timeline;                                  /* ZSTDB200_TIMELINE: print each wave's milestones */
+    ZbWorkRows work;                                /* the rows of every slot */
+    u8* d_in; u8* d_out; cudaStream_t sD2H, last;   /* kernel input and output, download stream, the last wave's stream */
+    unsigned launches; size_t err, prefixUp;        /* err: a launch failed; the call still finishes what it queued */
+    double t0, hostEnq; std::vector<double> hostDone;   /* host clock: enqueue start and duration, each wave's size seen */
+    std::vector<u64> fsz;                           /* per-frame sizes, read back by synchronous calls */
+    /* every buffer the call needs, before its first work is enqueued (run through ZbOrder::Call::size) */
+    size_t sizeBuffers() {
+        TRY(zb_ensureDesc(c, P.blocks.size(), a.nbFrames, W.nbWaves, P.chunks.size()));
+        size_t const bytes = zb_workLayout(NULL, (size_t)W.slots * W.maxWaveBlocks, W.kind, P.sd, NULL);
         TRY(bytes); TRY(c->d_work.ensure(bytes));
-        zb_workLayout(c->d_work, (size_t)slots * maxWaveBlocks, kind, P.sd, &work);
+        zb_workLayout(c->d_work, (size_t)W.slots * W.maxWaveBlocks, W.kind, P.sd, &work);
         /* the wave events are created once and kept: a call creates none unless it has more waves than any call before it (or
          * ZSTDB200_TIMELINE changed, which wants timed events) */
-        TRY(c->evH2D.ensure(nbWaves, timeline)); TRY(c->evStitch.ensure(nbWaves, timeline));
-        TRY(c->evSize.ensure(nbWaves, timeline)); TRY(c->evD2H.ensure(nbWaves, timeline));
+        TRY(c->evH2D.ensure(W.nbWaves, timeline)); TRY(c->evStitch.ensure(W.nbWaves, timeline));
+        TRY(c->evSize.ensure(W.nbWaves, timeline)); TRY(c->evD2H.ensure(W.nbWaves, timeline));
         /* wave streams are created on first use: every stream beyond the hardware queue count (8 by default) shares a
          * queue with another one, and a download queued behind another wave's kernels stalls the whole pipeline */
-        if (!single) for (u32 s = 0; s < slots; s++) TRY(c->waveStream[s].ensure());
-        if (!deviceMemory) { TRY(c->d_in.ensure(inEnd + 16)); TRY(c->d_out.ensure(outCap + 16)); TRY(c->waveStream[ZB_WAVE_SLOTS_MAX].ensure()); }
-        if (ldm) TRY(zb_ldmBuffers(c, P));
+        if (!W.single) for (u32 s = 0; s < W.slots; s++) TRY(c->waveStream[s].ensure());
+        if (!a.deviceMemory) { TRY(c->d_in.ensure(W.inEnd + 16)); TRY(c->d_out.ensure(W.outCap + 16)); TRY(c->waveStream[ZB_WAVE_SLOTS_MAX].ensure()); }
+        if (!P.ldm.empty()) TRY(zb_ldmBuffers(c, P));
+        size_t const stageBytes = a.result ? zb_stageBytes(P) : 0;
         for (u32 s = 0; s < ZSTDB200_ASYNC_SLOTS && stageBytes; s++)
             if (c->stage[s].cap < stageBytes) { TRY(c->stage[s].ensure(stageBytes)); c->stageBusy[s] = false; }   /* every slot, so that any can serve a capture */
         return 0;
-    };
-    size_t sized;
-    {   ZbNoAlloc const dry(true); sized = sizing(); }
-    if (sized == ZB_ERR(ZB_error_stage_wrong) && !capturing) { CK(cudaEventSynchronize(c->order[0])); sized = sizing(); }
-    TRY(sized);
-    u8* d_in; u8* d_out; cudaStream_t sD2H = (cudaStream_t)0;
-    if (deviceMemory) { d_in = (u8*)src; d_out = dst; }
-    else { d_in = c->d_in; d_out = c->d_out; sD2H = c->waveStream[ZB_WAVE_SLOTS_MAX]; }
-    const ZbBlock* hBlocks = P.blocks.data(); const ZbFrame* hFrames = P.frames.data(); const ZbChunk* hChunks = P.chunks.data();
-    u32 stageSlot = 0;
-    if (async) TRY(zb_stageDescriptors(c, P, &stageSlot, &hBlocks, &hFrames, &hChunks));
-    std::vector<double> hostDone(nbWaves, 0.0);
-    double const hostT0 = zb_now();
-    unsigned launches = 0;
-    size_t err = 0, prefixUp = 0;
-    /* the first work: behind the context's earlier calls (an event recorded outside a graph cannot be waited for inside it:
-     * a captured call relies on them having completed, as a capture's warm-up does) */
-    if (!capturing) CK(cudaStreamWaitEvent(sCopy, c->order[0], 0));
-    if (cd) TRY(zb_residentDict(cd, c->device, shared, sCopy));
-    const u8* const d_dictEnd = cd ? cd->d_dict + 32 + cd->tail : NULL;   /* the device buffers exist from here on */
-    if (!single && !async) CK(cudaEventRecord(c->ev[EV_START], sCopy));
-    CK(cudaMemcpyAsync(c->d_blocks, hBlocks, nbBlocks * sizeof(ZbBlock), cudaMemcpyHostToDevice, sCopy));
-    CK(cudaMemcpyAsync(c->d_frames, hFrames, nbFrames * sizeof(ZbFrame), cudaMemcpyHostToDevice, sCopy));
-    CK(cudaMemcpyAsync(c->d_chunks, hChunks, P.chunks.size() * sizeof(ZbChunk), cudaMemcpyHostToDevice, sCopy));
-    if (async && !capturing) { CK(cudaEventRecord(c->evStage[stageSlot], sCopy)); c->stageBusy[stageSlot] = true; }
-    if (timed) CK(cudaEventRecord(c->ev[EV_K0], sCopy));
-    if (buildImages) TRY(zb_buildDictImages(cd, P, shared, sCopy));
-    cudaStream_t lastStream = sCopy;
-    if (ldm) {
-        /* host buffers: the whole input goes up first (a block may copy from any earlier wave), so this upload does not
-         * overlap the kernels as the per-wave uploads do */
-        if (!deviceMemory) CK(cudaMemcpyAsync(d_in, src, inEnd, cudaMemcpyHostToDevice, sCopy));
-        const u8* d_prefix = a.prefix;                            /* the indexed prefix: in place on the device, or uploaded like the input */
-        if (a.prefixSize && !a.prefixOnDevice) {
-            TRY(c->d_prefix.ensure(a.prefixSize));
-            CK(cudaMemcpyAsync(c->d_prefix, a.prefix, a.prefixSize, cudaMemcpyHostToDevice, sCopy));
-            d_prefix = c->d_prefix; prefixUp = a.prefixSize;
-        }
-        err = zb_runLdm(c, P, d_in, d_prefix, sCopy, &launches);
     }
-    for (u32 w = 0; w < nbWaves && !err; w++) {
-        u32 const b0 = wb[w], b1 = wb[w + 1];
-        ZbWorkRows const rows = work.at((size_t)(w % slots) * maxWaveBlocks);
-        if (!deviceMemory && !ldm) {
-            /* input bytes of the wave (frames are laid out in offset order; history was uploaded by earlier waves) */
-            u64 lo = ~0ull, hi = 0;
-            for (u32 b = b0; b < b1; b++) { u64 const s = P.blocks[b].srcOff, e = s + P.blocks[b].size; if (s < lo) lo = s; if (e > hi) hi = e; }
-            if (hi > lo) CK(cudaMemcpyAsync(d_in + lo, src + lo, hi - lo, cudaMemcpyHostToDevice, sCopy));
+    /* everything the call queues, behind the context's earlier calls, up to and including the last wave's stitch */
+    size_t enqueue(ZbOrder::Call& call) {
+        bool const async = a.result != nullptr, ldm = !P.ldm.empty();
+        d_in = a.deviceMemory ? (u8*)a.src : c->d_in.p; d_out = a.deviceMemory ? (u8*)a.dst : c->d_out.p;
+        sD2H = a.deviceMemory ? (cudaStream_t)0 : c->waveStream[ZB_WAVE_SLOTS_MAX].s;
+        const ZbBlock* hBlocks = P.blocks.data(); const ZbFrame* hFrames = P.frames.data(); const ZbChunk* hChunks = P.chunks.data();
+        u32 stageSlot = 0;
+        if (async) TRY(zb_stageDescriptors(c, P, &stageSlot, &hBlocks, &hFrames, &hChunks));
+        hostDone.assign(W.nbWaves, 0.0);
+        t0 = zb_now();
+        TRY(call.enter(sCopy));
+        if (cd) TRY(zb_residentDict(cd, c->device, shared, sCopy));
+        const u8* const d_dictEnd = cd ? cd->d_dict + 32 + cd->tail : NULL;   /* the device buffers exist from here on */
+        const ZbDictEntropy* const d_de = (cd && cd->entropy.present) ? cd->d_de.p : NULL;
+        if (!W.single && !async) CK(cudaEventRecord(c->ev[EV_START], sCopy));
+        CK(cudaMemcpyAsync(c->d_blocks, hBlocks, P.blocks.size() * sizeof(ZbBlock), cudaMemcpyHostToDevice, sCopy));
+        CK(cudaMemcpyAsync(c->d_frames, hFrames, a.nbFrames * sizeof(ZbFrame), cudaMemcpyHostToDevice, sCopy));
+        CK(cudaMemcpyAsync(c->d_chunks, hChunks, P.chunks.size() * sizeof(ZbChunk), cudaMemcpyHostToDevice, sCopy));
+        if (async && !call.capturing) { CK(cudaEventRecord(c->evStage[stageSlot], sCopy)); c->stageBusy[stageSlot] = true; }
+        if (W.single && !async) CK(cudaEventRecord(c->ev[EV_K0], sCopy));   /* events around each phase of a synchronous wave */
+        if (buildImages) TRY(zb_buildDictImages(cd, P, shared, sCopy));
+        last = sCopy;
+        if (ldm) {
+            /* host buffers: the whole input goes up first (a block may copy from any earlier wave), so this upload does not
+             * overlap the kernels as the per-wave uploads do */
+            if (!a.deviceMemory) CK(cudaMemcpyAsync(d_in, a.src, W.inEnd, cudaMemcpyHostToDevice, sCopy));
+            const u8* d_prefix = a.prefix;                        /* the indexed prefix: in place on the device, or uploaded like the input */
+            if (a.prefixSize && !a.prefixOnDevice) {
+                TRY(c->d_prefix.ensure(a.prefixSize));
+                CK(cudaMemcpyAsync(c->d_prefix, a.prefix, a.prefixSize, cudaMemcpyHostToDevice, sCopy));
+                d_prefix = c->d_prefix; prefixUp = a.prefixSize;
+            }
+            err = zb_runLdm(c, P, d_in, d_prefix, sCopy, &launches);
         }
-        cudaStream_t st = sCopy;
-        if (!single) {
-            CK(cudaEventRecord(c->evH2D[w], sCopy));
-            TRY(c->waveStream[w % slots].ensure());
-            st = c->waveStream[w % slots];
-            CK(cudaStreamWaitEvent(st, c->evH2D[w], 0));
+        for (u32 w = 0; w < W.nbWaves && !err; w++) {
+            u32 const b0 = W.wb[w], b1 = W.wb[w + 1];
+            ZbWorkRows const rows = work.at((size_t)(w % W.slots) * W.maxWaveBlocks);
+            if (!a.deviceMemory && !ldm) {
+                /* input bytes of the wave (frames are laid out in offset order; history was uploaded by earlier waves) */
+                u64 lo = ~0ull, hi = 0;
+                for (u32 b = b0; b < b1; b++) { u64 const s = P.blocks[b].srcOff, e = s + P.blocks[b].size; if (s < lo) lo = s; if (e > hi) hi = e; }
+                if (hi > lo) CK(cudaMemcpyAsync(d_in + lo, (const u8*)a.src + lo, hi - lo, cudaMemcpyHostToDevice, sCopy));
+            }
+            cudaStream_t st = sCopy;
+            if (!W.single) {
+                CK(cudaEventRecord(c->evH2D[w], sCopy));
+                TRY(c->waveStream[w % W.slots].ensure());
+                st = c->waveStream[w % W.slots];
+                CK(cudaStreamWaitEvent(st, c->evH2D[w], 0));
+            }
+            last = st;
+            err = zb_runBlocks(c, P, d_in, d_dictEnd, d_de, b0, b1, W.wc[w], W.wc[w + 1], rows, st, W.single && !async, &launches);
+            if (err) break;
+            if (w > 0) CK(cudaStreamWaitEvent(st, c->evStitch[w - 1], 0));
+            CK(zb_launch_stitch(d_in, c->d_blocks + b0, b1 - b0, c->d_frames, &rows,
+                                c->d_outOffsets + b0, w > 0 ? c->d_totals + (w - 1) : NULL, c->d_totals + w, d_out, W.outCap, st));
+            launches += 2;
+            if (!W.single) CK(cudaEventRecord(c->evStitch[w], st));
+            /* the wave's size goes to the host behind the event the next wave's stitch waits for: a store into mapped
+             * host memory from inside the scan kernel would add a PCIe round trip to every link of that chain */
+            if (!a.deviceMemory || timeline) {
+                CK(cudaMemcpyAsync(c->h_totals + w, c->d_totals + w, sizeof(u64), cudaMemcpyDeviceToHost, st));
+                CK(cudaEventRecord(c->evSize[w], st));
+            }
         }
-        lastStream = st;
-        err = zb_runBlocks(c, P, d_in, d_dictEnd, de ? cd->d_de.p : NULL, b0, b1, wc[w], wc[w + 1], rows, st, timed, &launches);
-        if (err) break;
-        if (w > 0) CK(cudaStreamWaitEvent(st, c->evStitch[w - 1], 0));
-        CK(zb_launch_stitch(d_in, c->d_blocks + b0, b1 - b0, c->d_frames, &rows,
-                            c->d_outOffsets + b0, w > 0 ? c->d_totals + (w - 1) : NULL, c->d_totals + w, d_out, outCap, st));
-        launches += 2;
-        if (!single) CK(cudaEventRecord(c->evStitch[w], st));
-        /* the wave's size goes to the host behind the event the next wave's stitch waits for: a store into mapped
-         * host memory from inside the scan kernel would add a PCIe round trip to every link of that chain */
-        if (download || timeline) {
-            CK(cudaMemcpyAsync(c->h_totals + w, c->d_totals + w, sizeof(u64), cudaMemcpyDeviceToHost, st));
-            CK(cudaEventRecord(c->evSize[w], st));
-        }
+        hostEnq = zb_now() - t0;
+        return 0;
     }
-    if (async) {
-        /* the tail of a stream-ordered call: the waves join the caller's stream, which then writes the checksums and the verdict */
+    /* a stream-ordered call's end: the waves join the caller's stream, which then runs the checksum and verdict kernels */
+    size_t finishOrdered(ZbOrder::Call& call) {
         if (!err) {
-            if (!single) for (u32 s = 0; s < slots; s++) {
+            if (!W.single) for (u32 s = 0; s < W.slots; s++) {
                 CK(cudaEventRecord(c->evJoin[s], c->waveStream[s]));
                 CK(cudaStreamWaitEvent(sCopy, c->evJoin[s], 0));
             }
-            if (a.checksum) { CK(zb_launch_checksums(d_in, c->d_frames, (u32)nbFrames, c->d_outOffsets, d_out, outCap, sCopy)); launches++; }
-            CK(zb_launch_call_result(c->d_frames, (u32)nbFrames, c->d_outOffsets, c->d_totals + nbWaves - 1, dstCapacity, a.d_cSizes, a.result, sCopy));
+            if (a.checksum) { CK(zb_launch_checksums(d_in, c->d_frames, (u32)a.nbFrames, c->d_outOffsets, d_out, W.outCap, sCopy)); launches++; }
+            CK(zb_launch_call_result(c->d_frames, (u32)a.nbFrames, c->d_outOffsets, c->d_totals + W.nbWaves - 1, a.dstCapacity, a.d_cSizes, a.result, sCopy));
             launches++;
         }
-        if (!capturing) CK(cudaEventRecord(c->order[0], sCopy));
-        c->stats.launches = launches; c->stats.nbBlocks = nbBlocks;
+        TRY(call.leave(sCopy));
+        c->stats.launches = launches; c->stats.nbBlocks = (u32)P.blocks.size();
         return err;
     }
-    double const hostEnq = zb_now() - hostT0;
-    /* content checksums.  Host buffers: XXH64 on host threads while the GPU works (a serial recurrence per frame, one
-     * thread each).  Device buffers: a warp per frame once the last wave is stitched. */
-    std::vector<u64> xxh;
-    if (a.checksum && !err && !deviceMemory) {
-        xxh.resize(nbFrames);
-        size_t const nt = nbFrames < 8 ? nbFrames : 8;
-        if (nt <= 1) xxh[0] = zb_xxh64(src + frameOffsets[0], frameSizes[0]);
-        else {
-            std::vector<std::thread> th;
-            for (size_t t = 0; t < nt; t++) th.emplace_back([&, t] { for (size_t f = t; f < nbFrames; f += nt) xxh[f] = zb_xxh64(src + frameOffsets[f], frameSizes[f]); });
-            for (size_t t = 0; t < nt; t++) th[t].join();
-        }
+    /* the per-frame sizes the frame-sizes kernel wrote on `last`, read back into fsz and the caller's cSizes */
+    size_t readSizes() {
+        fsz.resize(a.nbFrames);
+        CK(cudaMemcpyAsync(fsz.data(), c->d_frameSizes, a.nbFrames * sizeof(u64), cudaMemcpyDeviceToHost, last));
+        CK(cudaStreamSynchronize(last));
+        if (a.cSizes) for (size_t f = 0; f < a.nbFrames; f++) a.cSizes[f] = (size_t)fsz[f];
+        return 0;
     }
-    if (a.checksum && !err && deviceMemory) { CK(zb_launch_checksums(d_in, c->d_frames, (u32)nbFrames, c->d_outOffsets, d_out, outCap, lastStream)); launches++; }
-    bool const wantSizes = a.cSizes != NULL || (a.checksum && !deviceMemory);
-    std::vector<u64> fsz;
-    u64 prev = 0, total = 0;
-    if (download || timeline) {
-        /* drain: as each wave's size becomes known, ship its bytes */
-        for (u32 w = 0; w < nbWaves && !err; w++) {
+    /* what both synchronous ends share once their last work is queued: every stream drained, the timeline, the stats */
+    size_t endSync() {
+        if (!W.single) for (u32 s = 0; s < W.slots; s++) if (c->waveStream[s]) CK(cudaStreamSynchronize(c->waveStream[s]));
+        CK(cudaStreamSynchronize(sCopy));
+        u64 const total = err ? 0 : c->h_totals[W.nbWaves - 1];
+        if (timeline) {
+            fprintf(stderr, "zstd_b200 timeline (ms after the call's first enqueue; host enqueue loop took %.3f ms; %s)\n", 1e3 * hostEnq,
+                    a.deviceMemory ? "device buffers" : "per-wave downloads");
+            for (u32 w = 0; w < W.nbWaves; w++) {
+                float up = 0, st = 0, dn = 0;
+                cudaEventElapsedTime(&up, c->ev[EV_START], c->evH2D[w]); cudaEventElapsedTime(&st, c->ev[EV_START], c->evStitch[w]);
+                cudaEventElapsedTime(&dn, c->ev[EV_START], c->evD2H[w]);
+                fprintf(stderr, "  wave %2u blocks %5u..%5u : uploaded %7.3f  stitched %7.3f (host saw it %7.3f)  downloaded %7.3f\n",
+                        w, W.wb[w], W.wb[w + 1], up, st, 1e3 * hostDone[w], dn);
+            }
+        }
+        if (err) return err;
+        float ms = 0;
+        if (W.single) {
+            cudaEventElapsedTime(&ms, c->ev[EV_K0], c->ev[EV_KEND]); c->stats.kernel_ms = ms;
+            cudaEventElapsedTime(&ms, c->ev[EV_K0], c->ev[EV_K1]); c->stats.match_ms = ms;
+            if (P.groups.size() == 1) { cudaEventElapsedTime(&ms, c->ev[EV_K0], c->ev[EV_MID]); c->stats.cand_ms = ms; cudaEventElapsedTime(&ms, c->ev[EV_MID], c->ev[EV_K1]); c->stats.parse_ms = ms; }
+            cudaEventElapsedTime(&ms, c->ev[EV_K1], c->ev[EV_K2]); c->stats.literals_ms = ms;
+            cudaEventElapsedTime(&ms, c->ev[EV_K2], c->ev[EV_K3]); c->stats.sequences_ms = ms;
+            cudaEventElapsedTime(&ms, c->ev[EV_K3], c->ev[EV_KEND]); c->stats.stitch_ms = ms;
+        } else { cudaEventElapsedTime(&ms, c->ev[EV_START], c->ev[EV_END]); c->stats.kernel_ms = ms; }
+        c->stats.total_ms = c->stats.kernel_ms;
+        c->stats.launches = launches; c->stats.nbBlocks = (u32)P.blocks.size();
+        if (!a.deviceMemory) { c->stats.h2d_bytes = W.inEnd + prefixUp; c->stats.d2h_bytes = (size_t)total; }
+        if (total > a.dstCapacity) return ZB_ERR(ZB_error_dstSize_tooSmall);
+        return (size_t)total;
+    }
+    /* a synchronous call's end on device buffers: the checksum kernel (a warp per frame), the frame sizes, the read-back */
+    size_t finishDevice() {
+        if (a.checksum && !err) { CK(zb_launch_checksums(d_in, c->d_frames, (u32)a.nbFrames, c->d_outOffsets, d_out, W.outCap, last)); launches++; }
+        if (timeline) for (u32 w = 0; w < W.nbWaves && !err; w++) {   /* each wave's milestones, as for host buffers */
             CK(cudaEventSynchronize(c->evSize[w]));
-            hostDone[w] = zb_now() - hostT0;
-            total = c->h_totals[w];
-            if (download && total <= outCap && total > prev) CK(cudaMemcpyAsync(dst + prev, d_out + prev, total - prev, cudaMemcpyDeviceToHost, sD2H));
-            if (total <= outCap) prev = total;
-            if (timeline) CK(cudaEventRecord(c->evD2H[w], download ? sD2H : lastStream));
+            hostDone[w] = zb_now() - t0;
+            CK(cudaEventRecord(c->evD2H[w], last));
         }
+        if (!err && a.cSizes) { CK(zb_launch_frame_sizes(c->d_frames, (u32)a.nbFrames, c->d_outOffsets, c->d_frameSizes, last)); launches += W.single; }   /* a multi-wave call's count leaves it out */
+        if (W.single) CK(cudaEventRecord(c->ev[EV_KEND], last));
+        if (!err && !timeline) CK(cudaMemcpyAsync(c->h_totals + W.nbWaves - 1, c->d_totals + W.nbWaves - 1, sizeof(u64), cudaMemcpyDeviceToHost, last));
+        if (!err && a.cSizes) TRY(readSizes());
+        if (!W.single) CK(cudaEventRecord(c->ev[EV_END], last));      /* the last wave's stitch is ordered behind every earlier one */
+        return endSync();
     }
-    if (!err && wantSizes) {
-        CK(zb_launch_frame_sizes(c->d_frames, (u32)nbFrames, c->d_outOffsets, c->d_frameSizes, lastStream));
-        if (single) launches++;                                          /* a multi-wave call's count leaves this kernel out */
-    }
-    if (timed) CK(cudaEventRecord(c->ev[EV_KEND], lastStream));
-    if (!err && !download && !timeline) CK(cudaMemcpyAsync(c->h_totals + nbWaves - 1, c->d_totals + nbWaves - 1, sizeof(u64), cudaMemcpyDeviceToHost, lastStream));
-    if (!err && wantSizes) {
-        fsz.resize(nbFrames);
-        CK(cudaMemcpyAsync(fsz.data(), c->d_frameSizes, nbFrames * sizeof(u64), cudaMemcpyDeviceToHost, lastStream));
-        CK(cudaStreamSynchronize(lastStream));
-        if (a.cSizes) for (size_t f = 0; f < nbFrames; f++) a.cSizes[f] = (size_t)fsz[f];
-    }
-    /* the last wave's stitch is ordered behind every earlier one (evStitch chain) */
-    if (download) { CK(cudaEventRecord(c->ev[EV_END], sD2H)); CK(cudaStreamSynchronize(sD2H)); }
-    else if (!single) CK(cudaEventRecord(c->ev[EV_END], lastStream));
-    if (!single) for (u32 s = 0; s < slots; s++) if (c->waveStream[s]) CK(cudaStreamSynchronize(c->waveStream[s]));
-    CK(cudaStreamSynchronize(sCopy));
-    if (!err) total = c->h_totals[nbWaves - 1];
-    if (!err && a.checksum && !deviceMemory && total <= dstCapacity) {                               /* the 4 bytes the size scan left free behind every frame */
-        u64 end = 0;
-        for (size_t f = 0; f < nbFrames; f++) {
+    /* a synchronous call's end on host buffers: XXH64 on up to 8 host threads while the GPU works, each wave downloaded as its
+     * size arrives, the checksums written into the 4 bytes the size scan left free behind every frame */
+    size_t finishHost() {
+        const u8* const src = (const u8*)a.src; u8* const dst = (u8*)a.dst;
+        std::vector<u64> xxh;
+        if (a.checksum && !err) {
+            xxh.resize(a.nbFrames);
+            size_t const nt = a.nbFrames < 8 ? a.nbFrames : 8;
+            if (nt <= 1) xxh[0] = zb_xxh64(src + a.frameOffsets[0], a.frameSizes[0]);
+            else {
+                std::vector<std::thread> th;
+                for (size_t t = 0; t < nt; t++) th.emplace_back([&, t] { for (size_t f = t; f < a.nbFrames; f += nt) xxh[f] = zb_xxh64(src + a.frameOffsets[f], a.frameSizes[f]); });
+                for (size_t t = 0; t < nt; t++) th[t].join();
+            }
+        }
+        for (u64 w = 0, prev = 0; w < W.nbWaves && !err; w++) {
+            CK(cudaEventSynchronize(c->evSize[w]));
+            hostDone[w] = zb_now() - t0;
+            u64 const total = c->h_totals[w];
+            if (total <= W.outCap && total > prev) CK(cudaMemcpyAsync(dst + prev, d_out + prev, total - prev, cudaMemcpyDeviceToHost, sD2H));
+            if (total <= W.outCap) prev = total;
+            if (timeline) CK(cudaEventRecord(c->evD2H[w], sD2H));
+        }
+        if (!err && (a.cSizes || a.checksum)) { CK(zb_launch_frame_sizes(c->d_frames, (u32)a.nbFrames, c->d_outOffsets, c->d_frameSizes, last)); TRY(readSizes()); }   /* host calls are never single: not counted */
+        CK(cudaEventRecord(c->ev[EV_END], sD2H)); CK(cudaStreamSynchronize(sD2H));
+        size_t const total = endSync();
+        if (!zb_isErr(total) && a.checksum) for (size_t f = 0, end = 0; f < a.nbFrames; f++) {
             end += fsz[f];
             if (end < 4 || end > total) break;
             u32 const ck = (u32)xxh[f];
             dst[end - 4] = (u8)ck; dst[end - 3] = (u8)(ck >> 8); dst[end - 2] = (u8)(ck >> 16); dst[end - 1] = (u8)(ck >> 24);
         }
+        return total;
     }
-    if (timeline) {
-        fprintf(stderr, "zstd_b200 timeline (ms after the call's first enqueue; host enqueue loop took %.3f ms; %s)\n", 1e3 * hostEnq,
-                deviceMemory ? "device buffers" : "per-wave downloads");
-        for (u32 w = 0; w < nbWaves; w++) {
-            float up = 0, st = 0, dn = 0;
-            cudaEventElapsedTime(&up, c->ev[EV_START], c->evH2D[w]); cudaEventElapsedTime(&st, c->ev[EV_START], c->evStitch[w]);
-            cudaEventElapsedTime(&dn, c->ev[EV_START], c->evD2H[w]);
-            fprintf(stderr, "  wave %2u blocks %5u..%5u : uploaded %7.3f  stitched %7.3f (host saw it %7.3f)  downloaded %7.3f\n",
-                    w, wb[w], wb[w + 1], up, st, 1e3 * hostDone[w], dn);
-        }
+};
+
+static size_t zb_compress(ZSTD_CCtx* c, const ZbCall& a)
+{
+    bool const async = a.result != nullptr;
+    if (a.nbFrames == 0 && !async) return 0;
+    ZbDeviceGuard guard;
+    ZbOrder::Call call(c->order);
+    if (async) TRY(call.begin(c->device, a.stream));
+    TRY(zb_ctxInit(c));
+    memset(&c->stats, 0, sizeof(c->stats));
+    if (a.nbFrames == 0) {                                        /* a batch without frames: its total, 0, in stream order */
+        CK(zb_launch_call_result(NULL, 0, NULL, NULL, a.dstCapacity, NULL, a.result, a.stream));
+        c->stats.launches = 1;
+        return 0;
     }
-    if (err) return err;
-    float ms = 0;
-    if (single) {
-        cudaEventElapsedTime(&ms, c->ev[EV_K0], c->ev[EV_KEND]); c->stats.kernel_ms = ms;
-        cudaEventElapsedTime(&ms, c->ev[EV_K0], c->ev[EV_K1]); c->stats.match_ms = ms;
-        if (P.groups.size() == 1) { cudaEventElapsedTime(&ms, c->ev[EV_K0], c->ev[EV_MID]); c->stats.cand_ms = ms; cudaEventElapsedTime(&ms, c->ev[EV_MID], c->ev[EV_K1]); c->stats.parse_ms = ms; }
-        cudaEventElapsedTime(&ms, c->ev[EV_K1], c->ev[EV_K2]); c->stats.literals_ms = ms;
-        cudaEventElapsedTime(&ms, c->ev[EV_K2], c->ev[EV_K3]); c->stats.sequences_ms = ms;
-        cudaEventElapsedTime(&ms, c->ev[EV_K3], c->ev[EV_KEND]); c->stats.stitch_ms = ms;
-    } else { cudaEventElapsedTime(&ms, c->ev[EV_START], c->ev[EV_END]); c->stats.kernel_ms = ms; }
-    c->stats.total_ms = c->stats.kernel_ms;
-    c->stats.launches = launches; c->stats.nbBlocks = nbBlocks;
-    if (!deviceMemory) { c->stats.h2d_bytes = inEnd + prefixUp; c->stats.d2h_bytes = (size_t)total; }
-    if (total > dstCapacity) return ZB_ERR(ZB_error_dstSize_tooSmall);
-    return (size_t)total;
+    /* the dictionary: a caller's ZSTD_CDict, which other contexts may share (its device state is guarded by cd->lock), or
+     * the context's digest of this call's bytes */
+    ZSTD_CDict* const cd = (a.cdict && a.cdict->size >= 8) ? const_cast<ZSTD_CDict*>(a.cdict) : NULL;   /* zstd_compress.c:5130 : tiny dictionaries are ignored */
+    const ZbDictEntropy* const de = (cd && cd->entropy.present) ? &cd->entropy : NULL;
+    ZbPlan& P = async ? c->asyncPlan : c->plan;
+    zb_plan(P, a, cd ? cd->size : 0, cd ? cd->tail : 0, de ? de->dictID : 0u, de ? de->rep : NULL);
+    if (P.unsupported) return ZB_ERR(ZB_error_parameter_unsupported);
+    bool const shared = cd != c->callDict.get(), buildImages = cd && (a.nbFrames >= 8 || shared);   /* a per-call digest builds its images afresh on every call: only for 8 frames or more */
+    if (call.capturing && cd && !zb_dictWarm(cd, c->device, shared, P, buildImages)) return ZB_ERR(ZB_error_stage_wrong);
+    ZbRun r{c, a, P, zb_wavePlan(c, P, a), cd, shared, buildImages, (async || (a.deviceMemory && a.stream)) ? a.stream : c->stream};
+    r.timeline = !r.W.single && !async && getenv("ZSTDB200_TIMELINE") != NULL;
+    TRY(call.size([&] { return r.sizeBuffers(); }));
+    TRY(r.enqueue(call));
+    if (async) return r.finishOrdered(call);
+    return a.deviceMemory ? r.finishDevice() : r.finishHost();
 }
 
 /* dictionary bytes passed to a call, digested into the context's callDict (*out = NULL without a dictionary) */
@@ -1288,7 +1288,7 @@ static size_t zb_compressSeqs(ZSTD_CCtx* c, void* dst, size_t dstCapacity, const
     ZbDeviceGuard guard;
     TRY(zb_ctxInit(c));
     memset(&c->stats, 0, sizeof(c->stats));
-    CK(cudaEventSynchronize(c->order[0]));                        /* stream-ordered calls still queued use the buffers sized below */
+    CK(c->order.hostWait());                                      /* stream-ordered calls still queued use the buffers sized below */
     const ZSTD_CDict* const cdArg = c->advRefCDict ? c->advRefCDict : c->advLocalDict.get();
     int const level = c->advRefCDict ? c->advRefCDict->level : c->advLevel;
     ZSTD_CDict* const cd = (cdArg && cdArg->size >= 8) ? const_cast<ZSTD_CDict*>(cdArg) : NULL;

@@ -225,16 +225,9 @@ static inline bool zb_isErr(size_t c) { return c > ZB_ERR(ZB_error_maxCode); }
 /* a call that returns an error code passes it on */
 #define TRY(x) do { size_t const e_ = (x); if (zb_isErr(e_)) return e_; } while (0)
 
-/* Set on a thread while it enqueues a call into a stream that is capturing a CUDA graph: allocating or freeing is not allowed
- * there, so every owner below refuses to grow with ZSTD_error_stage_wrong instead (the call then enqueues nothing). */
+/* Set on a thread while a call sizes its buffers without growing them and while a call is captured into a CUDA graph
+ * (ZbOrder below): every owner below then refuses to grow with ZSTD_error_stage_wrong instead. */
 inline thread_local bool zb_noAlloc = false;
-/* zb_noAlloc for the scope of one object: set while a call sizes its buffers without growing them, and for the whole of a call
- * that is being captured into a graph */
-struct ZbNoAlloc {
-    bool prev;
-    explicit ZbNoAlloc(bool on) : prev(zb_noAlloc) { zb_noAlloc = on; }
-    ~ZbNoAlloc() { zb_noAlloc = prev; }
-};
 
 /* An array of T in device memory (cudaMalloc) or page-locked host memory (cudaMallocHost) that a context owns: grown on
  * demand, freed with the context.  cap counts elements. */
@@ -348,6 +341,33 @@ struct ZbEvents {
     cudaEvent_t operator[](size_t i) const { return ev[i]; }
 };
 
+/* The order of a context's calls, one rule for the compressor and the decoder (DESIGN.md section 2, "Stream-ordered calls"):
+ * the `order` event, sizing without growth first, and what a call being captured into a graph may not do. */
+struct ZbOrder {
+    ZbEvents ev;
+    size_t create() { return ev.ensure(1, false); }
+    cudaError_t hostWait() const { return cudaEventSynchronize(ev[0]); }   /* every call queued so far has completed */
+    struct Call {                                  /* one call's side of the rule, for the call's duration */
+        const ZbOrder& o; bool capturing = false; bool const prevNoAlloc = zb_noAlloc;
+        explicit Call(const ZbOrder& order) : o(order) { zb_noAlloc = false; }
+        ~Call() { zb_noAlloc = prevNoAlloc; }
+        size_t begin(int device, cudaStream_t st) {   /* a stream-ordered call on st; device: the context's, -1 if none yet */
+            if (device >= 0) CK(cudaSetDevice(device));
+            cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+            CK(cudaStreamIsCapturing(st, &cs));
+            zb_noAlloc = capturing = cs != cudaStreamCaptureStatusNone;
+            return capturing && device < 0 ? ZB_ERR(ZB_error_stage_wrong) : 0;
+        }
+        template <typename F> size_t size(F&& sizing) {
+            zb_noAlloc = true; size_t r = sizing(); zb_noAlloc = capturing;
+            if (r == ZB_ERR(ZB_error_stage_wrong) && !capturing) { CK(o.hostWait()); r = sizing(); }
+            return r;
+        }
+        size_t enter(cudaStream_t st) { if (!capturing) CK(cudaStreamWaitEvent(st, o.ev[0], 0)); return 0; }
+        size_t leave(cudaStream_t st) { if (!capturing) CK(cudaEventRecord(o.ev[0], st)); return 0; }
+    };
+};
+
 /* restores the calling thread's current device when a call returns (a context works on the device it was created for) */
 struct ZbDeviceGuard {
     int prev;
@@ -355,15 +375,16 @@ struct ZbDeviceGuard {
     ~ZbDeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
 };
 
-/* deletes a context or digested dictionary on its device, where its members free what they own.  One that never reached a
- * device (device < 0) is deleted without a device switch: it holds nothing there, so its deletion makes no CUDA call (but
- * for the arrays a CDict's failed first upload left, which free themselves) */
-template <typename T> static inline size_t zb_deleteOnDevice(T* x)
+/* deletes a context (once the calls still queued on it have completed) or a digested dictionary on its device, where its
+ * members free what they own.  One that never reached a device (device < 0) is deleted without a device switch: it holds
+ * nothing there, so its deletion makes no CUDA call (but for the arrays a CDict's failed first upload left) */
+template <typename T> static inline size_t zb_deleteOnDevice(T* x, const ZbOrder* order = nullptr)
 {
     if (!x) return 0;
     if (x->device < 0) { delete x; return 0; }
     ZbDeviceGuard guard;
     cudaSetDevice(x->device);
+    if (order) order->hostWait();
     delete x;
     return 0;
 }
