@@ -405,6 +405,32 @@ ZSTDB200_API size_t ZSTDB200_compressFrames_usingCDict(ZSTD_CCtx* cctx, void* ds
                                             size_t nbFrames, const ZSTD_CDict* cdict,
                                             size_t* cSizes, int deviceMemory, void* stream);
 
+/* Same with a dictionary per frame, as a record store with one dictionary per table, column, tenant or file uses them
+ * (contrib/largeNbDicts/largeNbDicts.c:627-633 walks one CDict per block).  cdicts is a host array of nbFrames pointers,
+ * read before the call returns; a CDict may appear any number of times.  Frame i is byte for byte what
+ * ZSTD_compress_usingCDict(cctx, ..., cdicts[i]) produces for that record, at that CDict's level, with the sticky
+ * checksum, dictID and long-distance-matching parameters as for ZSTDB200_compressFrames_usingCDict; a NULL entry (or
+ * cdicts NULL: every entry) compresses the frame without a dictionary at compressionLevel, as ZSTDB200_compressFrames
+ * does.  Output layout, cSizes, deviceMemory, stream and the return value are those of
+ * ZSTDB200_compressFrames_usingCDict.  The number of kernel launches does not depend on the number of dictionaries:
+ * consecutive frames whose parameters are equal share them, whichever dictionary each has.  A CDict's first use uploads
+ * it and builds its table images for the call's parameter groups, in bulk for all of the call's new CDicts.  Fails with
+ * parameter_unsupported (40) when a frame's level is above 4 under ZSTDB200_setStrictLevels(1), while a prefix is
+ * pending, or when a CDict belongs to another device; dstSize_tooSmall (70) when the output does not fit; GENERIC (1)
+ * without a device.  A refused call writes nothing. */
+ZSTDB200_API size_t ZSTDB200_compressFrames_usingCDicts(ZSTD_CCtx* cctx, void* dst, size_t dstCapacity,
+                                            const void* src, const size_t* frameOffsets, const size_t* frameSizes,
+                                            size_t nbFrames, const ZSTD_CDict* const* cdicts, int compressionLevel,
+                                            size_t* cSizes, int deviceMemory, void* stream);
+/* The stream-ordered form, with ZSTDB200_compressFramesAsync's contract (device buffers, verdict and sizes in device
+ * memory, ordered with the context's other calls, capturable in a CUDA graph).  Under capture every CDict of the call must
+ * already be resident on the device and hold the table images its frames need (a warm call made them so); otherwise the
+ * call returns stage_wrong (60) before it enqueues anything. */
+ZSTDB200_API size_t ZSTDB200_compressFramesAsync_usingCDicts(ZSTD_CCtx* cctx, void* d_dst, size_t dstCapacity,
+                                            const void* d_src, const size_t* frameOffsets, const size_t* frameSizes,
+                                            size_t nbFrames, const ZSTD_CDict* const* cdicts, int compressionLevel,
+                                            unsigned long long* d_cSizes, unsigned long long* d_result, void* stream);
+
 /* Timing / evidence of the last call on this context (CUDA events on the launching stream). */
 typedef struct {
     float  kernel_ms;        /* first kernel start -> last kernel end */

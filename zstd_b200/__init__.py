@@ -128,6 +128,11 @@ def lib() -> ctypes.CDLL:
     L.ZSTDB200_compressDeviceAsync.argtypes = [_vp, _vp, _sz, _vp, _sz, ctypes.c_int, _vp, _vp]
     L.ZSTDB200_compressFramesAsync.restype = _sz
     L.ZSTDB200_compressFramesAsync.argtypes = [_vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, ctypes.c_int, _vp, _vp, _vp]
+    if hasattr(L, "ZSTDB200_compressFrames_usingCDicts"):                              # absent from older development builds
+        L.ZSTDB200_compressFrames_usingCDicts.restype = _sz
+        L.ZSTDB200_compressFrames_usingCDicts.argtypes = [_vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, ctypes.c_int, _vp, ctypes.c_int, _vp]
+        L.ZSTDB200_compressFramesAsync_usingCDicts.restype = _sz
+        L.ZSTDB200_compressFramesAsync_usingCDicts.argtypes = [_vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, ctypes.c_int, _vp, _vp, _vp]
     if hasattr(L, "ZSTD_createDCtx"):
         L.ZSTD_createDCtx.restype = _vp
         L.ZSTD_createDCtx.argtypes = []
@@ -369,6 +374,32 @@ class ZSTD_CCtx:
                                                            1 if device_memory else 0, stream))
         return r, list(csz)
 
+    def compress_frames_using_cdicts(self, dst: int, dst_capacity: int, src: int, offsets: Sequence[int], sizes: Sequence[int],
+                                     cdicts: Optional[Sequence[Optional["ZSTD_CDict"]]], level: int = 3, device_memory: bool = True,
+                                     stream: int = 0):
+        """Many independent frames, frame i against cdicts[i] at its level (None: no dictionary, at `level`; cdicts None:
+        None for every frame).  Returns (total_bytes, [size per frame])."""
+        n = len(sizes)
+        offs = (_sz * n)(*offsets)
+        szs = (_sz * n)(*sizes)
+        csz = (_sz * n)()
+        cds = _cdict_array(cdicts, n)
+        r = _check(lib().ZSTDB200_compressFrames_usingCDicts(self._h, dst, dst_capacity, src, offs, szs, n, cds, level, csz,
+                                                            1 if device_memory else 0, stream))
+        return r, list(csz)
+
+    def compress_frames_async_using_cdicts(self, d_dst: int, dst_capacity: int, d_src: int, offsets: Sequence[int],
+                                           sizes: Sequence[int], cdicts: Optional[Sequence[Optional["ZSTD_CDict"]]], d_result: int,
+                                           level: int = 3, d_c_sizes: int = 0, stream: int = 0) -> None:
+        """ZSTDB200_compressFramesAsync_usingCDicts: compress_frames_using_cdicts enqueued on `stream`, its verdict at
+        d_result and (d_c_sizes, 0 = none) one u64 size per frame in device memory."""
+        n = len(sizes)
+        offs = (_sz * n)(*offsets)
+        szs = (_sz * n)(*sizes)
+        cds = _cdict_array(cdicts, n)
+        _check(lib().ZSTDB200_compressFramesAsync_usingCDicts(self._h, d_dst, dst_capacity, d_src, offs, szs, n, cds, level,
+                                                              d_c_sizes or None, d_result, stream))
+
     # -- sequence API (lib/zstd.h:1555-1644) --
     def compress_sequences(self, seqs, src, dst_capacity: Optional[int] = None) -> bytes:
         """ZSTD_compressSequences: one frame from the caller's sequences (host buffers).  seqs: an (n, 4) uint32 array of
@@ -392,6 +423,15 @@ class ZSTD_CCtx:
         s = Stats()
         lib().ZSTDB200_getLastStats(self._h, ctypes.byref(s))
         return s
+
+
+def _cdict_array(cdicts, n):
+    """the host array of n CDict handles a per-frame-dictionary call reads (None: a NULL array)"""
+    if cdicts is None:
+        return None
+    if len(cdicts) != n:
+        raise ValueError(f"{len(cdicts)} dictionaries for {n} frames")
+    return (_vp * n)(*[(cd._h if cd is not None else None) for cd in cdicts])
 
 
 def _sequences(seqs):

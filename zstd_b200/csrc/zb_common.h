@@ -37,7 +37,7 @@ typedef uint64_t u64;
 
 #define ZB_FLAG_FIRST 1u       /* first block of its frame */
 #define ZB_FLAG_LAST  2u       /* last block of its frame  */
-#define ZB_FLAG_DICT  4u       /* its history (histLen bytes) is the tail of the call's dictionary content */
+#define ZB_FLAG_DICT  4u       /* the oldest dictLen bytes of its history are the tail of its frame's dictionary content */
 
 /* error codes = lib/zstd_errors.h:64-101 */
 #define ZB_ERR(code) ((size_t)-(long)(code))
@@ -64,8 +64,8 @@ typedef struct {
     u32 histLen;       /* bytes of history a match of this block may reach back into (chunk history and window) */
     u32 frame;         /* index into ZbFrame[] */
     u32 flags;         /* ZB_FLAG_* */
-    u32 dictLen;       /* the oldest dictLen bytes of that history are the tail of the call's dictionary content (ZB_FLAG_DICT) */
-    u32 pad;
+    u32 dictLen;       /* the oldest dictLen bytes of that history are the tail of its frame's dictionary content (ZB_FLAG_DICT) */
+    u32 dictSlot;      /* its frame's entry in the call's dictionary table (ZbDictSlot) */
 } ZbBlock;
 
 /* one chunk = up to ZB_CHUNK_BLOCKS consecutive blocks of a frame: the unit of the candidate walk */
@@ -76,7 +76,7 @@ typedef struct {
     u32 dictLen;       /* the oldest dictLen of them are the dictionary content's tail (first chunk of a frame only) */
     u32 firstBlock;    /* index of the chunk's first block in the call's block array */
     u32 blockLog;      /* log2 of the frame's block size: block k of the chunk starts at k << blockLog */
-    u32 pad;
+    u32 dictSlot;      /* its frame's entry in the call's dictionary table */
 } ZbChunk;
 
 typedef struct {
@@ -87,7 +87,7 @@ typedef struct {
     u32 windowLog;
     u32 dictID;
     u32 checksum;      /* 1: Content_Checksum_flag set, 4 bytes are reserved behind the last block (filled in by the host) */
-    u32 pad;
+    u32 dictSlot;      /* its entry in the call's dictionary table */
 } ZbFrame;
 
 typedef struct {       /* produced on the device, one per block */
@@ -132,9 +132,21 @@ typedef struct {
     u32 litDisabled;   /* zstd_compress_internal.h:621-633 */
     u32 windowLog;
     u32 insStep;       /* positions without a candidate enter the table when ((pos - low) % step) < 2, step = insStep + walked / 128 */
-    u32 startRep[2];   /* repcodes the search of a frame's first segment starts with (zstd-format dictionary), 0 = none */
-    u32 codeRep[3];    /* repcode history the decoder holds at a frame's first block: {1,4,8} or the dictionary's */
 } ZbParams;
+
+/* One entry of a call's dictionary table: what the kernels read of a frame's dictionary, through the dictSlot of the frame's
+ * blocks and chunks, at its first chunk (walk) and first block (parse, merge, entropy stages) only.  An entry serves one
+ * dictionary under one set of ZbParams (the image is that parameter group's).  A launch without a table (NULL) has no
+ * dictionary in any frame: first blocks start from the format's repcodes and entropy state. */
+typedef struct {
+    const u8* end;               /* one past the content tail in device memory (ZB_FLAG_DICT blocks read below it) */
+    const ZbDictEntropy* de;     /* a zstd-format dictionary's entropy state, else NULL */
+    const u32* image;            /* the tables walked over the tail under the group's ZbParams (tableN u32, then tableNLong u32 for
+                                  * doubleFast), or NULL: the walk primes them from the tail */
+    u32 startRep[2];             /* repcodes the search of a frame's first segment starts with (zstd-format dictionary), 0 = none */
+    u32 codeRep[3];              /* repcode history the decoder holds at a frame's first block: {1,4,8} or the dictionary's */
+    u32 pad;
+} ZbDictSlot;
 
 /* Per-block strides of the workspace arrays of one call, derived from its largest block (M = that size rounded up to 64):
  * a call of 128 KiB blocks has 128 Ki dist, 32776 seq, 128 KiB + 256 lit and 128 KiB + 1 KiB body per block. */

@@ -802,7 +802,7 @@ static ZSTD_DDict* zbd_createDDict(const void* dict, size_t dictSize, bool byCop
     return dd;
 }
 
-/* Makes dd resident on `device`, zb_residentDict's rule: the buffer is allocated on the first device that uses dd (one device
+/* Makes dd resident on `device`, the compressor's rule for a CDict (ZbRun::prepareDicts): the buffer is allocated on the first device that uses dd (one device
  * per DDict: another gets parameter_unsupported), the bytes are uploaded once per digest, and the upload has completed
  * before another context can use dd.  A resident DDict costs a call nothing: no copy, no synchronisation. */
 static size_t zbd_residentDict(const ZSTD_DDict* dd, int device, cudaStream_t st)

@@ -102,7 +102,7 @@ __device__ inline u32 zbw_fse_normalize(short* norm, u32 tableLog, const u32* co
                 if (v > bestV || (v == bestV && s2 < bestS)) { bestV = v; bestS = s2; }
             }
             if (bestV < 2u) return ZBD_ERR;
-            if ((bestS & 31u) == lane) base[bestS >> 5]--;
+            if ((bestS & 31u) == lane) { if (bestS >> 5) base[1]--; else base[0]--; }   /* a select: an indexed base[] would live in local memory */
         }
     }
 #pragma unroll

@@ -10,15 +10,19 @@ extern "C" {
 
 /* Every launch of K1..K4 works on the workspace rows [0, nbBlocks) (zb_workLayout, zb_common.h), one per block of the
  * launch: K1, K1s-b and K4 take them as `rows`.
+ * d_dicts: the call's dictionary table (ZbDictSlot, zb_common.h), indexed by the dictSlot of a frame's first chunk and
+ * first block; NULL when no frame of the launch has a dictionary.
  * K1: match-finder = K1a candidate walk (one CTA per chunk) + K1b greedy parse (one warp per 16 KiB segment) + K1c merge.
  * d_blocks / d_chunks point at the first block / chunk of the launch; slotFirstBlock = index (in the call's block array)
  * of the block that owns row 0.  Writes meta, seqs and lits; dist, far, segmeta (and doubleFast's dist2, far2) are its
  * own scratch.
- * d_dictEnd: one past the dictionary content in device memory (NULL = no dictionary); chunks / blocks with dictLen > 0
- * take the oldest dictLen bytes of their history from in front of it.  d_image (may be NULL): table already walked
- * over that dictionary tail by zb_launch_dict_image (same ZbParams), prm->tableN u32. */
-cudaError_t zb_launch_dict_image(const u8* d_dictEnd, const ZbChunk* d_dictChunk, const ZbParams* prm, u32* d_image, cudaStream_t stream);
-cudaError_t zb_launch_match(const u8* d_src, const u8* d_dictEnd, const u32* d_image, const ZbBlock* d_blocks, u32 nbBlocks,
+ * Chunks / blocks with dictLen > 0 take the oldest dictLen bytes of their history from in front of their dictionary
+ * entry's end; a first chunk starts from the entry's image when it has one (built by zb_launch_dict_images under the
+ * same ZbParams).  dict: some block of the launch has ZB_FLAG_DICT (the parse's variant that reads two buffers).
+ * zb_launch_dict_images: one CTA per image, image i walks the tail of d_dicts[d_imageChunks[i].dictSlot] (a chunk of
+ * size 0 whose history is that tail) into that entry's image. */
+cudaError_t zb_launch_dict_images(const ZbDictSlot* d_dicts, const ZbChunk* d_imageChunks, u32 nbImages, const ZbParams* prm, cudaStream_t stream);
+cudaError_t zb_launch_match(const u8* d_src, const ZbDictSlot* d_dicts, bool dict, const ZbBlock* d_blocks, u32 nbBlocks,
                             const ZbChunk* d_chunks, u32 nbChunks, u32 slotFirstBlock, const ZbParams* prm, const ZbWorkRows* rows,
                             cudaEvent_t evMid, cudaStream_t stream, const ZbLdmView* ldm = nullptr);
 /* ldm (K1c): the launch's blocks' long-distance matches (zb_launch_ldm), laid over the parse output; NULL = none */
@@ -45,7 +49,7 @@ cudaError_t zb_launch_seq_place(const void* d_seqs, u32 n, int expl, const u64* 
 cudaError_t zb_launch_seq_blocks(const u64* d_blockEnd, const u32* d_blockSeq, u32 nbBlocks, u32 blockMax, u32 dictFlag,
                                  ZbBlock* d_blocks, u32* d_blockFirst, u64* d_blockFirstPos, u64* d_ctrl, cudaStream_t stream);
 cudaError_t zb_launch_seq_convert(const u8* d_src, const ZbBlock* d_blocks, u32 nbBlocks, const u32* d_blockFirst, const u64* d_blockFirstPos,
-                                  const void* d_seqs, u32 n, const ZbParams* prm, const ZbWorkRows* rows, cudaStream_t stream);
+                                  const void* d_seqs, u32 n, const ZbDictSlot* d_dicts, const ZbWorkRows* rows, cudaStream_t stream);
 
 /* host: the format's predefined FSE tables (zb_dict.cu), and their upload to the current device (zb_sequences.cu) */
 void zb_buildDefaultTables(ZbdFseCTable* out3);
@@ -57,13 +61,15 @@ size_t zb_loadDictionary(ZbDictEntropy* de, const u8* dict, size_t dictSize);
 /* K2 and K3 take their arrays one by one: the entropy test harness (tests/entropy_harness.cu) runs them over allocations
  * of its own.  The driver passes the workspace rows of the launch (K3's d_stateBits: the dist rows, see zb_workLayout). */
 /* K2: literals section (histogram, Huffman table, 1/4-stream encode).  One CTA per block.
- * d_de (may be NULL): dictionary entropy state used by ZB_FLAG_DICT blocks. */
+ * The entropy state a frame's first block starts from: its dictionary entry's when d_dicts is given (the driver), else d_de
+ * (NULL: none) for every first block (the entropy harness). */
 cudaError_t zb_launch_literals(const ZbBlock* d_blocks, u32 nbBlocks, const ZbParams* prm, const ZbStrides* sd, const ZbDictEntropy* d_de,
-                               const u8* d_lits, u8* d_body, ZbBlockMeta* d_meta, cudaStream_t stream);
+                               const u8* d_lits, u8* d_body, ZbBlockMeta* d_meta, cudaStream_t stream, const ZbDictSlot* d_dicts = nullptr);
 
 /* K3: sequences section (codes, histograms, FSE tables, tANS bit-stream) + block-type decision. */
 cudaError_t zb_launch_sequences(const u8* d_src, const ZbBlock* d_blocks, u32 nbBlocks, const ZbParams* prm, const ZbStrides* sd, const ZbDictEntropy* d_de,
-                                const u64* d_seqs, u16* d_stateBits, u8* d_body, ZbBlockMeta* d_meta, cudaStream_t stream);
+                                const u64* d_seqs, u16* d_stateBits, u8* d_body, ZbBlockMeta* d_meta, cudaStream_t stream,
+                                const ZbDictSlot* d_dicts = nullptr);
 
 /* K4: stitch — per-block output sizes -> exclusive scan -> frame/block headers + payload copy, for
  * one wave of blocks, from the body and meta rows.  d_blocks/d_outOffsets point at the wave's first block;

@@ -151,8 +151,8 @@ __device__ __forceinline__ void zb_huf_stream(const u8* __restrict__ lit, u32 be
 }
 
 __global__ void __launch_bounds__(LIT_THREADS, LIT_MIN_CTAS)
-zb_literals_kernel(const ZbBlock* __restrict__ blocks, ZbParams prm, ZbStrides sd, const ZbDictEntropy* __restrict__ de,
-                   const u8* __restrict__ lits, u8* __restrict__ body, ZbBlockMeta* __restrict__ meta)
+zb_literals_kernel(const ZbBlock* __restrict__ blocks, ZbParams prm, ZbStrides sd, const ZbDictEntropy* __restrict__ deAll,
+                   const ZbDictSlot* __restrict__ dicts, const u8* __restrict__ lits, u8* __restrict__ body, ZbBlockMeta* __restrict__ meta)
 {
     /* the per-warp (per-stream) histograms live until the stream sizes are known, then hold the encoding windows */
     __shared__ __align__(16) u32 whist[LIT_WARPS][256];
@@ -176,7 +176,9 @@ zb_literals_kernel(const ZbBlock* __restrict__ blocks, ZbParams prm, ZbStrides s
     /* ---------------- decisions (zstd_compress_literals.c:129-191, huf_compress.c:1359-1420) ----------------
      * `repeat` is the HUF_repeat mode of the previous block's table: only a frame's first block behind a
      * zstd-format dictionary has one (ZSTD_loadCEntropy, zstd_compress.c:4997-5005); 0 none, 1 check, 2 valid. */
-    u32 repeat = (de != nullptr && (blocks[b].flags & ZB_FLAG_FIRST) && de->present) ? de->hufRepeat : 0u;
+    ZbBlock const bd = blocks[b];
+    const ZbDictEntropy* const de = (bd.flags & ZB_FLAG_FIRST) ? (dicts ? dicts[bd.dictSlot].de : deAll) : nullptr;
+    u32 repeat = (de != nullptr && de->present) ? de->hufRepeat : 0u;
     bool const preferRepeat = (n <= 1024u);                      /* strategy < lazy, zstd_compress_literals.c:165 */
     u32 const lhSize = 3u + (n >= 1024u) + (n >= 16384u);
     u32 const nbStreams = (n < 256u || (repeat == 2u && lhSize == 3u)) ? 1u : 4u;     /* :142, :171 */
@@ -330,9 +332,9 @@ zb_literals_kernel(const ZbBlock* __restrict__ blocks, ZbParams prm, ZbStrides s
 }
 
 extern "C" cudaError_t zb_launch_literals(const ZbBlock* d_blocks, u32 nbBlocks, const ZbParams* prm, const ZbStrides* sd, const ZbDictEntropy* d_de,
-                                          const u8* d_lits, u8* d_body, ZbBlockMeta* d_meta, cudaStream_t stream)
+                                          const u8* d_lits, u8* d_body, ZbBlockMeta* d_meta, cudaStream_t stream, const ZbDictSlot* d_dicts)
 {
     if (nbBlocks == 0) return cudaSuccess;
-    zb_literals_kernel<<<nbBlocks, LIT_THREADS, 0, stream>>>(d_blocks, *prm, *sd, d_de, d_lits, d_body, d_meta);
+    zb_literals_kernel<<<nbBlocks, LIT_THREADS, 0, stream>>>(d_blocks, *prm, *sd, d_de, d_dicts, d_lits, d_body, d_meta);
     return cudaGetLastError();
 }

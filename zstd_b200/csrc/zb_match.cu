@@ -223,16 +223,18 @@ __device__ __forceinline__ bool zb_walk_batch(u32* __restrict__ table, u32 xa, c
 #endif
 template <int MLS, int P>
 __global__ void __launch_bounds__(ZB_BATCH / P, P == WALK_P_SMALL ? WALK_MINB_SMALL : 1)
-zb_walk_kernel(const u8* __restrict__ src, const u8* __restrict__ dictEnd, const ZbChunk* __restrict__ chunks, u32 insStep, u32 N, ZbStrides sd,
-               u32 slotFirstBlock, u16* __restrict__ dist, u32* __restrict__ far,
-               const u32* __restrict__ imageIn, u32* __restrict__ imageOut)
+zb_walk_kernel(const u8* __restrict__ src, const ZbDictSlot* __restrict__ dicts, const ZbChunk* __restrict__ chunks, u32 insStep, u32 N, ZbStrides sd,
+               u32 slotFirstBlock, u16* __restrict__ dist, u32* __restrict__ far, u32 imageOff, bool buildImage)
 {
     constexpr u32 THREADS = ZB_BATCH / P;
     extern __shared__ __align__(16) u32 table[];
     u32 const t = threadIdx.x;
     ZbChunk const cd = chunks[blockIdx.x];
-    bool const buildImage = imageOut != nullptr;
     u32 const D = cd.dictLen;                                     /* rel position of the frame's first byte when a dictionary is in front */
+    /* the frame's dictionary (first chunk only): its tail's end and the table image of this launch's parameters (buildImage:
+     * the image this CTA writes) */
+    const u8* dictEnd = nullptr; const u32* imageIn = nullptr;
+    if (D) { ZbDictSlot const& ds = dicts[cd.dictSlot]; dictEnd = ds.end; imageIn = ds.image ? ds.image + imageOff : nullptr; }
     u32 const H = cd.histLen;                                     /* rel position of the chunk's first byte */
     u32 const total = buildImage ? D : H + cd.size;               /* rel positions [0, total) are walked; no read at or past total */
     bool const fromImage = imageIn != nullptr && D != 0u && !buildImage;
@@ -353,7 +355,10 @@ zb_walk_kernel(const u8* __restrict__ src, const u8* __restrict__ dictEnd, const
         if (x0 >= xEnd) break;
         doBatch(rawB, shB);
     }
-    if (buildImage) { __syncthreads(); for (u32 i = t; i < N; i += THREADS) imageOut[i] = table[i]; }
+    if (buildImage) {                                             /* the image's address is read again here: not live through the walk */
+        u32* const imageOut = const_cast<u32*>(dicts[chunks[blockIdx.x].dictSlot].image) + imageOff;
+        __syncthreads(); for (u32 i = t; i < N; i += THREADS) imageOut[i] = table[i];
+    }
 }
 
 /* ------------------------------------------------------------------------------------------------
@@ -378,7 +383,7 @@ __device__ __forceinline__ u32 zb_dist_at(const u16* __restrict__ d16, const u32
 
 template <bool DICT>
 __global__ void __launch_bounds__(32 * PARSE_WARPS, DICT ? (40 / PARSE_WARPS) : PARSE_MIN_CTAS)
-zb_parse_kernel(const u8* __restrict__ src, const u8* __restrict__ dictEnd, const ZbBlock* __restrict__ blocks, u32 nbBlocks, ZbParams prm, ZbStrides sd,
+zb_parse_kernel(const u8* __restrict__ src, const ZbDictSlot* __restrict__ dicts, const ZbBlock* __restrict__ blocks, u32 nbBlocks, ZbParams prm, ZbStrides sd,
                 const u16* __restrict__ dist, const u32* __restrict__ far, u64* __restrict__ seqs, ZbBlockMeta* __restrict__ meta, ZbSegMeta* __restrict__ segmeta)
 {
     u32 const lane = threadIdx.x & 31u;
@@ -392,7 +397,7 @@ zb_parse_kernel(const u8* __restrict__ src, const u8* __restrict__ dictEnd, cons
     const u8* const base = src + bd.srcOff - bd.histLen;          /* base + rel addresses the frame's own bytes */
     u32 const bs = bd.histLen, blockEnd = bd.histLen + bd.size;
     ZbSeg sg; sg.hi = base; sg.lo = base; sg.split = 0;
-    if (DICT && (bd.flags & ZB_FLAG_DICT)) { sg.lo = dictEnd - bd.dictLen; sg.split = bd.dictLen; }   /* oldest history = dictionary tail */
+    if (DICT && (bd.flags & ZB_FLAG_DICT)) { sg.lo = dicts[bd.dictSlot].end - bd.dictLen; sg.split = bd.dictLen; }   /* oldest history = dictionary tail */
 
     if (bd.size < 7u) {                                        /* zstd_compress.c:3216 */
         if (lane == 0 && k == 0) {
@@ -412,7 +417,7 @@ zb_parse_kernel(const u8* __restrict__ src, const u8* __restrict__ dictEnd, cons
 
     u32 ip = ss, anchor = ss;                                  /* the search restarts at the anchor: it is searchStart too */
     u32 rep1 = 0, rep2 = 0, nbSeq = 0;
-    if ((bd.flags & ZB_FLAG_FIRST) && k == 0u) { rep1 = prm.startRep[0]; rep2 = prm.startRep[1]; }   /* a zstd-format dictionary's repcodes, zstd_compress.c:5054-5056 */
+    if (dicts && (bd.flags & ZB_FLAG_FIRST) && k == 0u) { rep1 = dicts[bd.dictSlot].startRep[0]; rep2 = dicts[bd.dictSlot].startRep[1]; }   /* a zstd-format dictionary's repcodes, zstd_compress.c:5054-5056 */
 
     /* the 4 bytes at rel position x; x + 8 <= be */
     auto ld4 = [&](u32 x) { return DICT ? (u32)zb_seg_ld64x<DICT>(sg, x) : zb_ld32w2(sg.hi + x); };
@@ -501,7 +506,7 @@ zb_parse_kernel(const u8* __restrict__ src, const u8* __restrict__ dictEnd, cons
  * ---------------------------------------------------------------------------------------------- */
 template <bool DICT>
 __global__ void __launch_bounds__(32 * PARSE_WARPS)
-zb_parse_dfast_kernel(const u8* __restrict__ src, const u8* __restrict__ dictEnd, const ZbBlock* __restrict__ blocks, u32 nbBlocks, ZbParams prm, ZbStrides sd,
+zb_parse_dfast_kernel(const u8* __restrict__ src, const ZbDictSlot* __restrict__ dicts, const ZbBlock* __restrict__ blocks, u32 nbBlocks, ZbParams prm, ZbStrides sd,
                       const u16* __restrict__ distLong, const u32* __restrict__ farLong, const u16* __restrict__ distShort, const u32* __restrict__ farShort,
                       u64* __restrict__ seqs, ZbBlockMeta* __restrict__ meta, ZbSegMeta* __restrict__ segmeta)
 {
@@ -519,7 +524,7 @@ zb_parse_dfast_kernel(const u8* __restrict__ src, const u8* __restrict__ dictEnd
     const u8* const base = src + bd.srcOff - bd.histLen;
     u32 const bs = bd.histLen, blockEnd = bd.histLen + bd.size;
     ZbSeg sg; sg.hi = base; sg.lo = base; sg.split = 0;
-    if (DICT && (bd.flags & ZB_FLAG_DICT)) { sg.lo = dictEnd - bd.dictLen; sg.split = bd.dictLen; }
+    if (DICT && (bd.flags & ZB_FLAG_DICT)) { sg.lo = dicts[bd.dictSlot].end - bd.dictLen; sg.split = bd.dictLen; }
 
     if (bd.size < 7u) {                                        /* zstd_compress.c:3216 */
         if (lane == 0 && k == 0) {
@@ -538,7 +543,7 @@ zb_parse_dfast_kernel(const u8* __restrict__ src, const u8* __restrict__ dictEnd
     u32 const be = blockEnd;
     u32 ip = ss, anchor = ss, searchStart = ss;
     u32 rep1 = 0, rep2 = 0, nbSeq = 0;
-    if ((bd.flags & ZB_FLAG_FIRST) && k == 0u) { rep1 = prm.startRep[0]; rep2 = prm.startRep[1]; }
+    if (dicts && (bd.flags & ZB_FLAG_FIRST) && k == 0u) { rep1 = dicts[bd.dictSlot].startRep[0]; rep2 = dicts[bd.dictSlot].startRep[1]; }
 
     while (ip < se && ip + 9u <= be) {                        /* a lane reads 8 bytes at p and at p+1 */
         u32 const step = 1u + ((ip - searchStart) >> 8);                     /* kStepIncr = 1 << kSearchStrength */
@@ -712,7 +717,7 @@ __device__ u32 zb_ldm_overlay(const u64* __restrict__ P, u32 nP, const u64* __re
  * distScratch: the candidate arrays, dead once the parse is done).  Without LDM the instruction stream is the kernel's own. */
 template <bool LDM>
 __global__ void __launch_bounds__(MERGE_THREADS, MERGE_MIN_CTAS)
-zb_merge_segments_kernel(const u8* __restrict__ src, const ZbBlock* __restrict__ blocks, ZbParams prm, ZbStrides sd, const ZbSegMeta* __restrict__ segmeta,
+zb_merge_segments_kernel(const u8* __restrict__ src, const ZbDictSlot* __restrict__ dicts, const ZbBlock* __restrict__ blocks, ZbStrides sd, const ZbSegMeta* __restrict__ segmeta,
                          u64* __restrict__ seqs, u8* __restrict__ lits, ZbBlockMeta* __restrict__ meta,
                          ZbLdmView ldm, u32* __restrict__ farScratch, u16* __restrict__ distScratch)
 {
@@ -798,14 +803,16 @@ zb_merge_segments_kernel(const u8* __restrict__ src, const ZbBlock* __restrict__
     }
     nbSeq = gTotal;
     }
-    zb_merge_codes(prm.codeRep[0], prm.codeRep[1], prm.codeRep[2], (bd.flags & ZB_FLAG_FIRST) != 0u, myseq, mylit, in, nbSeq, bd.size, meta + b,
+    u32 rep[3] = { 1u, 4u, 8u };                                 /* zstd_internal.h:69, or the frame's dictionary's */
+    if (dicts && (bd.flags & ZB_FLAG_FIRST)) { rep[0] = dicts[bd.dictSlot].codeRep[0]; rep[1] = dicts[bd.dictSlot].codeRep[1]; rep[2] = dicts[bd.dictSlot].codeRep[2]; }
+    zb_merge_codes(rep[0], rep[1], rep[2], (bd.flags & ZB_FLAG_FIRST) != 0u, myseq, mylit, in, nbSeq, bd.size, meta + b,
                    sPos, sLit, sLen, sOff, sR2, sRep, wsumL, wsumA, wmaxU, wmaxK, baseL, baseA);
 }
 
 /* K1c for calls made of short frames (one segment per block: nothing to join): one warp per block, 8 blocks per CTA;
  * every lane converts and gathers the literals of its own sequences, the repcode history runs through the warp. */
 __global__ void __launch_bounds__(MERGE_THREADS)
-zb_merge_small_kernel(const u8* __restrict__ src, const ZbBlock* __restrict__ blocks, u32 nbBlocks, ZbParams prm, ZbStrides sd, const ZbSegMeta* __restrict__ segmeta,
+zb_merge_small_kernel(const u8* __restrict__ src, const ZbDictSlot* __restrict__ dicts, const ZbBlock* __restrict__ blocks, u32 nbBlocks, ZbStrides sd, const ZbSegMeta* __restrict__ segmeta,
                       u64* __restrict__ seqs, u8* __restrict__ lits, ZbBlockMeta* __restrict__ meta)
 {
     u32 const lane = threadIdx.x & 31u;
@@ -818,7 +825,10 @@ zb_merge_small_kernel(const u8* __restrict__ src, const ZbBlock* __restrict__ bl
     const u8* const in = src + bd.srcOff;
     u32 const nbSeq = segmeta[b].nbSeq;
     ZbRepHist hist; hist.r1 = 0; hist.r2 = 0; hist.r3 = 0;
-    if (bd.flags & ZB_FLAG_FIRST) { hist.r1 = prm.codeRep[0]; hist.r2 = prm.codeRep[1]; hist.r3 = prm.codeRep[2]; }
+    if (bd.flags & ZB_FLAG_FIRST) {                              /* zstd_internal.h:69, or the frame's dictionary's */
+        hist.r1 = 1u; hist.r2 = 4u; hist.r3 = 8u;
+        if (dicts) { hist.r1 = dicts[bd.dictSlot].codeRep[0]; hist.r2 = dicts[bd.dictSlot].codeRep[1]; hist.r3 = dicts[bd.dictSlot].codeRep[2]; }
+    }
     u32 posL = 0, posA = 0;
     for (u32 t0 = 0; t0 < nbSeq; t0 += 32u) {
         u32 const i = t0 + lane;
@@ -865,47 +875,49 @@ zb_merge_small_kernel(const u8* __restrict__ src, const ZbBlock* __restrict__ bl
  * 256 threads; <= 113 KiB: 2 CTAs of 512; the doubleFast tables (128 / 200 KiB): one CTA of 1024.  The result does not
  * depend on P (a batch is ZB_BATCH positions whatever the thread count). */
 template <int MLS, int P>
-static cudaError_t zb_launch_walk_p(const u8* d_src, const u8* d_dictEnd, const ZbChunk* d_chunks, u32 nbChunks, u32 N, u32 insStep, const ZbStrides& sd,
-                                    u32 slotFirstBlock, u16* d_dist, u32* d_far, const u32* d_imageIn, u32* d_imageOut, cudaStream_t stream)
+static cudaError_t zb_launch_walk_p(const u8* d_src, const ZbDictSlot* d_dicts, const ZbChunk* d_chunks, u32 nbChunks, u32 N, u32 insStep, const ZbStrides& sd,
+                                    u32 slotFirstBlock, u16* d_dist, u32* d_far, u32 imageOff, bool build, cudaStream_t stream)
 {
     cudaError_t const e = cudaFuncSetAttribute(zb_walk_kernel<MLS, P>, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
     if (e != cudaSuccess) return e;
-    zb_walk_kernel<MLS, P><<<nbChunks, ZB_BATCH / P, (size_t)N * 4u, stream>>>(d_src, d_dictEnd, d_chunks, insStep, N, sd, slotFirstBlock, d_dist, d_far, d_imageIn, d_imageOut);
+    zb_walk_kernel<MLS, P><<<nbChunks, ZB_BATCH / P, (size_t)N * 4u, stream>>>(d_src, d_dicts, d_chunks, insStep, N, sd, slotFirstBlock, d_dist, d_far, imageOff, build);
     return cudaGetLastError();
 }
 template <int MLS>
-static cudaError_t zb_launch_walk_m(const u8* d_src, const u8* d_dictEnd, const ZbChunk* d_chunks, u32 nbChunks, u32 N, u32 insStep, const ZbStrides& sd,
-                                    u32 slotFirstBlock, u16* d_dist, u32* d_far, const u32* d_imageIn, u32* d_imageOut, cudaStream_t stream)
+static cudaError_t zb_launch_walk_m(const u8* d_src, const ZbDictSlot* d_dicts, const ZbChunk* d_chunks, u32 nbChunks, u32 N, u32 insStep, const ZbStrides& sd,
+                                    u32 slotFirstBlock, u16* d_dist, u32* d_far, u32 imageOff, bool build, cudaStream_t stream)
 {
     size_t const smem = (size_t)N * 4u;
-    if (smem <= 56u * 1024u)  return zb_launch_walk_p<MLS, WALK_P_SMALL>(d_src, d_dictEnd, d_chunks, nbChunks, N, insStep, sd, slotFirstBlock, d_dist, d_far, d_imageIn, d_imageOut, stream);
-    if (smem <= 113u * 1024u) return zb_launch_walk_p<MLS, WALK_P_MID>(d_src, d_dictEnd, d_chunks, nbChunks, N, insStep, sd, slotFirstBlock, d_dist, d_far, d_imageIn, d_imageOut, stream);
-    return zb_launch_walk_p<MLS, 1>(d_src, d_dictEnd, d_chunks, nbChunks, N, insStep, sd, slotFirstBlock, d_dist, d_far, d_imageIn, d_imageOut, stream);
+    if (smem <= 56u * 1024u)  return zb_launch_walk_p<MLS, WALK_P_SMALL>(d_src, d_dicts, d_chunks, nbChunks, N, insStep, sd, slotFirstBlock, d_dist, d_far, imageOff, build, stream);
+    if (smem <= 113u * 1024u) return zb_launch_walk_p<MLS, WALK_P_MID>(d_src, d_dicts, d_chunks, nbChunks, N, insStep, sd, slotFirstBlock, d_dist, d_far, imageOff, build, stream);
+    return zb_launch_walk_p<MLS, 1>(d_src, d_dicts, d_chunks, nbChunks, N, insStep, sd, slotFirstBlock, d_dist, d_far, imageOff, build, stream);
 }
-static cudaError_t zb_launch_walk(const u8* d_src, const u8* d_dictEnd, const ZbChunk* d_chunks, u32 nbChunks, u32 mls, u32 N, u32 insStep, const ZbStrides& sd,
-                                  u32 slotFirstBlock, u16* d_dist, u32* d_far, const u32* d_imageIn, u32* d_imageOut, cudaStream_t stream)
+static cudaError_t zb_launch_walk(const u8* d_src, const ZbDictSlot* d_dicts, const ZbChunk* d_chunks, u32 nbChunks, u32 mls, u32 N, u32 insStep, const ZbStrides& sd,
+                                  u32 slotFirstBlock, u16* d_dist, u32* d_far, u32 imageOff, bool build, cudaStream_t stream)
 {
     switch (mls) {
-    case 4: return zb_launch_walk_m<4>(d_src, d_dictEnd, d_chunks, nbChunks, N, insStep, sd, slotFirstBlock, d_dist, d_far, d_imageIn, d_imageOut, stream);
-    case 5: return zb_launch_walk_m<5>(d_src, d_dictEnd, d_chunks, nbChunks, N, insStep, sd, slotFirstBlock, d_dist, d_far, d_imageIn, d_imageOut, stream);
-    case 6: return zb_launch_walk_m<6>(d_src, d_dictEnd, d_chunks, nbChunks, N, insStep, sd, slotFirstBlock, d_dist, d_far, d_imageIn, d_imageOut, stream);
-    case 7: return zb_launch_walk_m<7>(d_src, d_dictEnd, d_chunks, nbChunks, N, insStep, sd, slotFirstBlock, d_dist, d_far, d_imageIn, d_imageOut, stream);
-    default: return zb_launch_walk_m<8>(d_src, d_dictEnd, d_chunks, nbChunks, N, insStep, sd, slotFirstBlock, d_dist, d_far, d_imageIn, d_imageOut, stream);
+    case 4: return zb_launch_walk_m<4>(d_src, d_dicts, d_chunks, nbChunks, N, insStep, sd, slotFirstBlock, d_dist, d_far, imageOff, build, stream);
+    case 5: return zb_launch_walk_m<5>(d_src, d_dicts, d_chunks, nbChunks, N, insStep, sd, slotFirstBlock, d_dist, d_far, imageOff, build, stream);
+    case 6: return zb_launch_walk_m<6>(d_src, d_dicts, d_chunks, nbChunks, N, insStep, sd, slotFirstBlock, d_dist, d_far, imageOff, build, stream);
+    case 7: return zb_launch_walk_m<7>(d_src, d_dicts, d_chunks, nbChunks, N, insStep, sd, slotFirstBlock, d_dist, d_far, imageOff, build, stream);
+    default: return zb_launch_walk_m<8>(d_src, d_dicts, d_chunks, nbChunks, N, insStep, sd, slotFirstBlock, d_dist, d_far, imageOff, build, stream);
     }
 }
 
-/* one-CTA launches that walk the dictionary tail and store the table(s) in d_image: prm->tableN u32 of the (short) table,
- * followed for doubleFast by prm->tableNLong u32 of the 8-byte-hash table */
-extern "C" cudaError_t zb_launch_dict_image(const u8* d_dictEnd, const ZbChunk* d_dictChunk, const ZbParams* prm, u32* d_image, cudaStream_t stream)
+/* the table images of nbImages dictionaries under one ZbParams, one CTA per image: image i walks the tail of
+ * d_dicts[d_imageChunks[i].dictSlot] and stores the table(s) in that entry's image: prm->tableN u32 of the (short) table,
+ * followed for doubleFast (a second launch) by prm->tableNLong u32 of the 8-byte-hash table */
+extern "C" cudaError_t zb_launch_dict_images(const ZbDictSlot* d_dicts, const ZbChunk* d_imageChunks, u32 nbImages, const ZbParams* prm, cudaStream_t stream)
 {
+    if (nbImages == 0) return cudaSuccess;
     ZbStrides const sd = zb_strides(ZB_BLOCK_MAX);               /* unused: no block row is written */
-    cudaError_t e = zb_launch_walk(nullptr, d_dictEnd, d_dictChunk, 1, prm->mls, prm->tableN, prm->insStep, sd, 0, nullptr, nullptr, nullptr, d_image, stream);
+    cudaError_t e = zb_launch_walk(nullptr, d_dicts, d_imageChunks, nbImages, prm->mls, prm->tableN, prm->insStep, sd, 0, nullptr, nullptr, 0, true, stream);
     if (e == cudaSuccess && prm->strategy == 2)
-        e = zb_launch_walk(nullptr, d_dictEnd, d_dictChunk, 1, 8, prm->tableNLong, prm->insStep, sd, 0, nullptr, nullptr, nullptr, d_image + prm->tableN, stream);
+        e = zb_launch_walk(nullptr, d_dicts, d_imageChunks, nbImages, 8, prm->tableNLong, prm->insStep, sd, 0, nullptr, nullptr, prm->tableN, true, stream);
     return e;
 }
 
-extern "C" cudaError_t zb_launch_match(const u8* d_src, const u8* d_dictEnd, const u32* d_image, const ZbBlock* d_blocks, u32 nbBlocks,
+extern "C" cudaError_t zb_launch_match(const u8* d_src, const ZbDictSlot* d_dicts, bool dict, const ZbBlock* d_blocks, u32 nbBlocks,
                                        const ZbChunk* d_chunks, u32 nbChunks, u32 slotFirstBlock, const ZbParams* prm, const ZbWorkRows* rows,
                                        cudaEvent_t evMid, cudaStream_t stream, const ZbLdmView* ldm)
 {
@@ -918,22 +930,22 @@ extern "C" cudaError_t zb_launch_match(const u8* d_src, const u8* d_dictEnd, con
     u32 const sgrid = (u32)(((u64)nbBlocks * segs + PARSE_WARPS - 1) / PARSE_WARPS);                       /* one warp per segment */
     if (prm->strategy == 2) {
         /* doubleFast: one candidate walk per table */
-        e = zb_launch_walk(d_src, d_dictEnd, d_chunks, nbChunks, 8, prm->tableNLong, prm->insStep, sd, slotFirstBlock, d_dist, d_far, d_image ? d_image + prm->tableN : nullptr, nullptr, stream); if (e != cudaSuccess) return e;
-        e = zb_launch_walk(d_src, d_dictEnd, d_chunks, nbChunks, prm->mls, prm->tableN, prm->insStep, sd, slotFirstBlock, d_dist2, d_far2, d_image, nullptr, stream); if (e != cudaSuccess) return e;
+        e = zb_launch_walk(d_src, d_dicts, d_chunks, nbChunks, 8, prm->tableNLong, prm->insStep, sd, slotFirstBlock, d_dist, d_far, prm->tableN, false, stream); if (e != cudaSuccess) return e;
+        e = zb_launch_walk(d_src, d_dicts, d_chunks, nbChunks, prm->mls, prm->tableN, prm->insStep, sd, slotFirstBlock, d_dist2, d_far2, 0, false, stream); if (e != cudaSuccess) return e;
         if (evMid) cudaEventRecord(evMid, stream);
-        if (d_dictEnd) zb_parse_dfast_kernel<true><<<sgrid, 32 * PARSE_WARPS, 0, stream>>>(d_src, d_dictEnd, d_blocks, nbBlocks, *prm, sd, d_dist, d_far, d_dist2, d_far2, d_seqs, d_meta, d_segmeta);
-        else           zb_parse_dfast_kernel<false><<<sgrid, 32 * PARSE_WARPS, 0, stream>>>(d_src, nullptr, d_blocks, nbBlocks, *prm, sd, d_dist, d_far, d_dist2, d_far2, d_seqs, d_meta, d_segmeta);
+        if (dict) zb_parse_dfast_kernel<true><<<sgrid, 32 * PARSE_WARPS, 0, stream>>>(d_src, d_dicts, d_blocks, nbBlocks, *prm, sd, d_dist, d_far, d_dist2, d_far2, d_seqs, d_meta, d_segmeta);
+        else      zb_parse_dfast_kernel<false><<<sgrid, 32 * PARSE_WARPS, 0, stream>>>(d_src, d_dicts, d_blocks, nbBlocks, *prm, sd, d_dist, d_far, d_dist2, d_far2, d_seqs, d_meta, d_segmeta);
     } else {
-        e = zb_launch_walk(d_src, d_dictEnd, d_chunks, nbChunks, prm->mls, prm->tableN, prm->insStep, sd, slotFirstBlock, d_dist, d_far, d_image, nullptr, stream); if (e != cudaSuccess) return e;
+        e = zb_launch_walk(d_src, d_dicts, d_chunks, nbChunks, prm->mls, prm->tableN, prm->insStep, sd, slotFirstBlock, d_dist, d_far, 0, false, stream); if (e != cudaSuccess) return e;
         if (evMid) cudaEventRecord(evMid, stream);
-        if (d_dictEnd) zb_parse_kernel<true><<<sgrid, 32 * PARSE_WARPS, 0, stream>>>(d_src, d_dictEnd, d_blocks, nbBlocks, *prm, sd, d_dist, d_far, d_seqs, d_meta, d_segmeta);
-        else           zb_parse_kernel<false><<<sgrid, 32 * PARSE_WARPS, 0, stream>>>(d_src, nullptr, d_blocks, nbBlocks, *prm, sd, d_dist, d_far, d_seqs, d_meta, d_segmeta);
+        if (dict) zb_parse_kernel<true><<<sgrid, 32 * PARSE_WARPS, 0, stream>>>(d_src, d_dicts, d_blocks, nbBlocks, *prm, sd, d_dist, d_far, d_seqs, d_meta, d_segmeta);
+        else      zb_parse_kernel<false><<<sgrid, 32 * PARSE_WARPS, 0, stream>>>(d_src, d_dicts, d_blocks, nbBlocks, *prm, sd, d_dist, d_far, d_seqs, d_meta, d_segmeta);
     }
     if (segs == 1u && sd.dist <= 8192u)
-        zb_merge_small_kernel<<<(nbBlocks + MERGE_THREADS / 32u - 1u) / (MERGE_THREADS / 32u), MERGE_THREADS, 0, stream>>>(d_src, d_blocks, nbBlocks, *prm, sd, d_segmeta, d_seqs, d_lits, d_meta);
+        zb_merge_small_kernel<<<(nbBlocks + MERGE_THREADS / 32u - 1u) / (MERGE_THREADS / 32u), MERGE_THREADS, 0, stream>>>(d_src, d_dicts, d_blocks, nbBlocks, sd, d_segmeta, d_seqs, d_lits, d_meta);
     else if (ldm)                                                /* scratch in the dead candidate rows: far, then dist (zb_workLayout) */
-        zb_merge_segments_kernel<true><<<nbBlocks, MERGE_THREADS, 0, stream>>>(d_src, d_blocks, *prm, sd, d_segmeta, d_seqs, d_lits, d_meta, *ldm, d_far, d_dist);
+        zb_merge_segments_kernel<true><<<nbBlocks, MERGE_THREADS, 0, stream>>>(d_src, d_dicts, d_blocks, sd, d_segmeta, d_seqs, d_lits, d_meta, *ldm, d_far, d_dist);
     else
-        zb_merge_segments_kernel<false><<<nbBlocks, MERGE_THREADS, 0, stream>>>(d_src, d_blocks, *prm, sd, d_segmeta, d_seqs, d_lits, d_meta, ZbLdmView(), nullptr, nullptr);
+        zb_merge_segments_kernel<false><<<nbBlocks, MERGE_THREADS, 0, stream>>>(d_src, d_dicts, d_blocks, sd, d_segmeta, d_seqs, d_lits, d_meta, ZbLdmView(), nullptr, nullptr);
     return cudaGetLastError();
 }

@@ -137,7 +137,7 @@ __global__ void zb_seq_blocks_kernel(const u64* __restrict__ blockEnd, const u32
     if (k >= nbBlocks) return;
     u64 const start = k ? blockEnd[k - 1u] : 0ull, e = blockEnd[k];
     if (e - start > blockMax) atomicMin(errIdx, (unsigned long long)blockSeq[k]);
-    ZbBlock b; b.srcOff = start; b.size = (u32)min(e - start, (u64)blockMax); b.histLen = 0; b.frame = 0; b.dictLen = 0; b.pad = 0;
+    ZbBlock b; b.srcOff = start; b.size = (u32)min(e - start, (u64)blockMax); b.histLen = 0; b.frame = 0; b.dictLen = 0; b.dictSlot = 0;
     b.flags = (k == 0u ? ZB_FLAG_FIRST | dictFlag : 0u) | (k + 1u == nbBlocks ? ZB_FLAG_LAST : 0u);
     blocks[k] = b;
     blockFirst[k] = k ? blockSeq[k - 1u] + 1u : 0u;
@@ -148,7 +148,7 @@ __global__ void zb_seq_blocks_kernel(const u64* __restrict__ blockEnd, const u32
 /* K1s-b: one CTA per block */
 __global__ void __launch_bounds__(MERGE_THREADS)
 zb_seq_convert_kernel(const u8* __restrict__ src, const ZbBlock* __restrict__ blocks, const u32* __restrict__ blockFirst, const u64* __restrict__ blockFirstPos,
-                      const uint4* __restrict__ seqsIn, u32 n, ZbParams prm, ZbStrides sd,
+                      const uint4* __restrict__ seqsIn, u32 n, const ZbDictSlot* __restrict__ dicts, ZbStrides sd,
                       u64* __restrict__ seqs, u8* __restrict__ lits, ZbBlockMeta* __restrict__ meta)
 {
     __shared__ u32 sPos[MERGE_TILE], sLit[MERGE_TILE], sLen[MERGE_TILE], sOff[MERGE_TILE];
@@ -208,7 +208,9 @@ zb_seq_convert_kernel(const u8* __restrict__ src, const ZbBlock* __restrict__ bl
         }
         __syncthreads();
     }
-    zb_merge_codes(prm.codeRep[0], prm.codeRep[1], prm.codeRep[2], (bd.flags & ZB_FLAG_FIRST) != 0u, myseq, mylit, in, carryK, bd.size, meta + b,
+    u32 rep[3] = { 1u, 4u, 8u };                                 /* zstd_internal.h:69, or the dictionary's */
+    if (dicts && (bd.flags & ZB_FLAG_FIRST)) { rep[0] = dicts[bd.dictSlot].codeRep[0]; rep[1] = dicts[bd.dictSlot].codeRep[1]; rep[2] = dicts[bd.dictSlot].codeRep[2]; }
+    zb_merge_codes(rep[0], rep[1], rep[2], (bd.flags & ZB_FLAG_FIRST) != 0u, myseq, mylit, in, carryK, bd.size, meta + b,
                    sPos, sLit, sLen, sOff, sR2, sRep, wsumL, wsumA, wmaxU, wmaxK, baseL, baseA);
 }
 
@@ -245,10 +247,10 @@ extern "C" cudaError_t zb_launch_seq_blocks(const u64* d_blockEnd, const u32* d_
 }
 
 extern "C" cudaError_t zb_launch_seq_convert(const u8* d_src, const ZbBlock* d_blocks, u32 nbBlocks, const u32* d_blockFirst, const u64* d_blockFirstPos,
-                                             const void* d_seqs, u32 n, const ZbParams* prm, const ZbWorkRows* rows, cudaStream_t stream)
+                                             const void* d_seqs, u32 n, const ZbDictSlot* d_dicts, const ZbWorkRows* rows, cudaStream_t stream)
 {
     if (nbBlocks == 0) return cudaSuccess;
-    zb_seq_convert_kernel<<<nbBlocks, MERGE_THREADS, 0, stream>>>(d_src, d_blocks, d_blockFirst, d_blockFirstPos, (const uint4*)d_seqs, n, *prm, rows->sd,
+    zb_seq_convert_kernel<<<nbBlocks, MERGE_THREADS, 0, stream>>>(d_src, d_blocks, d_blockFirst, d_blockFirstPos, (const uint4*)d_seqs, n, d_dicts, rows->sd,
                                                                  rows->seqs, rows->lits, rows->meta);
     return cudaGetLastError();
 }

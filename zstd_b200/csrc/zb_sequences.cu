@@ -120,7 +120,8 @@ struct ZbdStreamWork {
 };
 
 __global__ void __launch_bounds__(SEQ_THREADS)
-zb_sequences_kernel(const u8* __restrict__ src, const ZbBlock* __restrict__ blocks, ZbParams prm, ZbStrides sd, const ZbDictEntropy* __restrict__ de,
+zb_sequences_kernel(const u8* __restrict__ src, const ZbBlock* __restrict__ blocks, ZbParams prm, ZbStrides sd, const ZbDictEntropy* __restrict__ deAll,
+                    const ZbDictSlot* __restrict__ dicts,
                     const u64* __restrict__ seqs, u16* __restrict__ stateBits,
                     u8* __restrict__ body, ZbBlockMeta* __restrict__ meta)
 {
@@ -137,6 +138,7 @@ zb_sequences_kernel(const u8* __restrict__ src, const ZbBlock* __restrict__ bloc
     ZbBlockMeta const m = meta[b];
     ZbBlock const bd = blocks[b];
     if (m.forceRaw) return;
+    const ZbDictEntropy* const de = (bd.flags & ZB_FLAG_FIRST) ? (dicts ? dicts[bd.dictSlot].de : deAll) : nullptr;
     u32 const nbSeq = m.nbSeq;
     const u64* const myseq = seqs + (size_t)b * sd.seq;
     u16* const myst = stateBits + (size_t)b * sd.dist;       /* the block's (dead) candidate-distance area */
@@ -179,7 +181,7 @@ zb_sequences_kernel(const u8* __restrict__ src, const ZbBlock* __restrict__ bloc
             for (u32 o = 16; o > 0; o >>= 1) mostFrequent = ::max(mostFrequent, __shfl_xor_sync(ZB_FULL, mostFrequent, o));
             u32 const defLog = st == 1 ? 5u : 6u;
             bool const defAllowed = st == 1 ? (max <= DefaultMaxOff) : true;
-            u32 const prevRepeat = (de != nullptr && (bd.flags & ZB_FLAG_FIRST) && de->present) ? de->fseRepeat[st] : 0u;
+            u32 const prevRepeat = (de != nullptr && de->present) ? de->fseRepeat[st] : 0u;
             u32 const type = zbd_selectEncodingType(mostFrequent, nbSeq, defLog, defAllowed, prm.strategy, prevRepeat);
             if (lane == 0) { w->type = type; w->err = 0; w->ncSize = 0; }
             __syncwarp();
@@ -356,9 +358,10 @@ zb_sequences_kernel(const u8* __restrict__ src, const ZbBlock* __restrict__ bloc
 }
 
 extern "C" cudaError_t zb_launch_sequences(const u8* d_src, const ZbBlock* d_blocks, u32 nbBlocks, const ZbParams* prm, const ZbStrides* sd, const ZbDictEntropy* d_de,
-                                           const u64* d_seqs, u16* d_stateBits, u8* d_body, ZbBlockMeta* d_meta, cudaStream_t stream)
+                                           const u64* d_seqs, u16* d_stateBits, u8* d_body, ZbBlockMeta* d_meta, cudaStream_t stream,
+                                           const ZbDictSlot* d_dicts)
 {
     if (nbBlocks == 0) return cudaSuccess;
-    zb_sequences_kernel<<<nbBlocks, SEQ_THREADS, 0, stream>>>(d_src, d_blocks, *prm, *sd, d_de, d_seqs, d_stateBits, d_body, d_meta);
+    zb_sequences_kernel<<<nbBlocks, SEQ_THREADS, 0, stream>>>(d_src, d_blocks, *prm, *sd, d_de, d_dicts, d_seqs, d_stateBits, d_body, d_meta);
     return cudaGetLastError();
 }
