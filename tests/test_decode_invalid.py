@@ -28,7 +28,6 @@ import seqgen
 import zref
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-BUILD = os.path.join(HERE, "_build")
 needs_ref = pytest.mark.skipif(not zref.have_ref(), reason="reference library not built")
 _sz, _vp = ctypes.c_size_t, ctypes.c_void_p
 GUARD = 0xA5
@@ -49,10 +48,15 @@ DIFFERENCES = {
 
 # ---------------------------------------------------------------------------------------------------- decoders
 @pytest.fixture(scope="module")
-def H():
+def build_dir(tmp_path_factory):
+    """where the harness is compiled: a fresh directory, since the tree may not be writable by whoever runs the tests"""
+    return str(tmp_path_factory.mktemp("hostdecode"))
+
+
+@pytest.fixture(scope="module")
+def H(build_dir):
     """the CPU harness: the decoder's format code, block after block"""
-    so = os.path.join(BUILD, "libzb_hostdecode_invalid.so")
-    os.makedirs(BUILD, exist_ok=True)
+    so = os.path.join(build_dir, "libzb_hostdecode_invalid.so")
     subprocess.check_call(["g++", "-O2", "-fPIC", "-shared", "-Wall", "-Wextra", "-Werror", "-Wno-unused-function", "-x", "c++",
                            "-o", so, os.path.join(HERE, "host_decode.cpp")])
     h = ctypes.CDLL(so)
@@ -417,11 +421,10 @@ VALID = zref.synthetic(50_000, 80, 0.6)
 
 
 # ---------------------------------------------------------------------------------------------------- CPU half
-def _sanitized(cases):
+def _sanitized(cases, build_dir):
     """the harness as a program under AddressSanitizer and UndefinedBehaviorSanitizer over all cases: [(return value,
     output checksum, guard kept)]"""
-    exe = os.path.join(BUILD, "zb_hostdecode_sanitized")
-    os.makedirs(BUILD, exist_ok=True)
+    exe = os.path.join(build_dir, "zb_hostdecode_sanitized")
     subprocess.check_call(["g++", "-O1", "-g", "-fsanitize=address,undefined", "-fno-sanitize-recover=all", "-DZBH_CORPUS_MAIN",
                            "-Wall", "-Wextra", "-Werror", "-Wno-unused-function", "-x", "c++", "-o", exe, os.path.join(HERE, "host_decode.cpp")])
     rec = bytearray()
@@ -464,7 +467,7 @@ def test_raw_rle_block_over_window(H):
 
 
 @needs_ref
-def test_invalid_inputs_harness(H):
+def test_invalid_inputs_harness(H, build_dir):
     """every constructed case and CORPUS_CPU corpus cases through the harness, judged against the reference; then the
     same inputs once through the harness built with sanitizers, which must report nothing and agree"""
     cases = constructed() + corpus(CORPUS_CPU, 1)
@@ -481,7 +484,7 @@ def test_invalid_inputs_harness(H):
             assert harness(H, zref.ref_compress(VALID, 3), len(VALID))[0] == VALID
     print("\nverdicts (corpus?, class):", dict(classes), "\nreference accepts, decoder refuses:", dict(diffs))
     assert classes[(True, "both-accept")] > 100 and classes[(True, "both-refuse")] > 1000
-    san = _sanitized(cases)
+    san = _sanitized(cases, build_dir)
     assert len(san) == len(cases)
     for (name, _, cap, _), ours, (r, h, guard) in zip(cases, seen, san):
         assert guard == 1, name

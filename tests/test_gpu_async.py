@@ -108,11 +108,13 @@ def test_same_bytes_as_compress_device(n, level, big):
     src = big if n == 300 << 20 else _input(n)
     ctx = zstd_b200.ZSTD_CCtx()
     want = _sync(ctx, src, level)
+    sync_launches = ctx.stats().launches
     d_src = _dev(src)
     d_dst, res = _async(ctx, d_src, n, level, stream=torch.cuda.Stream())
     torch.cuda.synchronize()
     assert _frame(d_dst, res) == want
     assert ctx.stats().launches > 0 and ctx.stats().kernel_ms == 0.0
+    assert ctx.stats().launches == sync_launches          # the same kernels, the verdict kernel included
     if level == 3 and n in (5000, 3 << 20):
         assert zstd_b200.ZSTD_DCtx().decompress(want, n) == src
         if zref.have_ref():

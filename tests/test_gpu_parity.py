@@ -532,7 +532,9 @@ def test_wave_executor_at_small_sizes():
     """The executor's ways through a call, with 512 KiB waves taking turns on 2 workspace slots so that a few MiB make many
     waves: device buffers in waves, host buffers in waves, one wave on one stream (ZSTDB200_SERIAL=1) and one wave on a
     caller-supplied stream give the same bytes and sizes, equal to the oracle's frames.  One call has several frames with
-    content checksums, the other 24 frames against a dictionary (the table-image path)."""
+    content checksums, the other 24 frames against a dictionary (the table-image path).  A capacity one byte short of the
+    frames gives dstSize_tooSmall in each way, and nothing is written past it.  ZSTDB200_compressDevice, which passes no
+    size array, compresses the first frame alone, in waves and in one wave."""
     import torch
     knobs = ("ZSTDB200_WAVE_BLOCKS", "ZSTDB200_HOST_WAVE_BLOCKS", "ZSTDB200_WAVE_SLOTS", "ZSTDB200_SERIAL")
     saved = {k: os.environ.get(k) for k in knobs}
@@ -550,12 +552,13 @@ def test_wave_executor_at_small_sizes():
                 os.environ[k] = v
     d = zref.golden_input("zdict-16k-synthetic-seed77")
     side = torch.cuda.Stream()
+    guard = b"\xa5" * 64
     for sizes, dict_bytes, checksum in (([3 << 20, 1000, 0, 700_001, (1 << 20) + 5], None, True), ([150_000] * 16 + [1024] * 8, d, False)):
         src = zref.synthetic(sum(sizes), 61, 0.5)
         offs, o = [], 0
         for n in sizes:
             offs.append(o); o += n
-        cap = sum(zstd_b200.ZSTD_compressBound(n) + 32 for n in sizes)
+        bound = sum(zstd_b200.ZSTD_compressBound(n) + 32 for n in sizes)
         d_src = torch.frombuffer(bytearray(src), dtype=torch.uint8).cuda()
         sbuf = ctypes.create_string_buffer(src, len(src))
         want = []
@@ -563,25 +566,48 @@ def test_wave_executor_at_small_sizes():
             part = src[off:off + n]
             f = zref.oracle_compress(part, 1) if dict_bytes is None else zref.oracle_compress_using_dict(part, dict_bytes, 1)
             want.append(_with_checksum(f, part) if checksum else f)
+        first = zref.oracle_compress(src[:sizes[0]], 1)
+        first = _with_checksum(first, src[:sizes[0]]) if checksum else first
         for c in (waves, serial):
             c.set_parameter("checksum_flag", int(checksum))
 
-        def run(c, device=True, stream=0):
-            if not device:
-                h_dst = ctypes.create_string_buffer(cap)
-                total, csz = c.compress_frames(ctypes.addressof(h_dst), cap, ctypes.addressof(sbuf), offs, sizes, level=1,
-                                               device_memory=False, dict_bytes=dict_bytes)
-                return h_dst.raw[:total], csz, c.stats()
-            d_dst = torch.zeros(cap, dtype=torch.uint8, device="cuda")
-            total, csz = c.compress_frames(d_dst.data_ptr(), cap, d_src.data_ptr(), offs, sizes, level=1, dict_bytes=dict_bytes, stream=stream)
-            return bytes(d_dst[:total].cpu().numpy()), csz, c.stats()
+        def run(c, device=True, stream=0, cap=bound, one=False):
+            """compress_frames (one: compress_device of the first frame) into cap bytes followed by 64 guard bytes; returns
+            (output, sizes, stats, guard bytes after the call), or the ZstdError code in place of the output"""
+            n = cap + 64
+            if device:
+                dst = torch.full((n,), 0xA5, dtype=torch.uint8, device="cuda")
+                torch.cuda.synchronize()                                # filled before the call's streams write it
+                ptr, sp, read = dst.data_ptr(), d_src.data_ptr(), lambda: bytes(dst.cpu().numpy())
+            else:
+                dst = ctypes.create_string_buffer(guard[:1] * n, n)
+                ptr, sp, read = ctypes.addressof(dst), ctypes.addressof(sbuf), lambda: dst.raw
+            try:
+                if one:
+                    total, csz = c.compress_device(ptr, cap, sp, sizes[0], 1, stream), None
+                else:
+                    total, csz = c.compress_frames(ptr, cap, sp, offs, sizes, level=1, device_memory=device, dict_bytes=dict_bytes,
+                                                   stream=stream)
+            except zstd_b200.ZstdError as e:
+                return e.code, None, None, read()[cap:]
+            out = read()
+            return out[:total], csz, c.stats(), out[cap:]
 
-        got = {"device waves": run(waves), "host waves": run(waves, device=False), "serial": run(serial),
-               "caller stream": run(waves, stream=side.cuda_stream)}
-        for name, (out, csz, st) in got.items():
+        ways = {"device waves": dict(c=waves), "host waves": dict(c=waves, device=False), "serial": dict(c=serial),
+                "caller stream": dict(c=waves, stream=side.cuda_stream)}
+        for name, kw in ways.items():
+            out, csz, st, tail = run(**kw)
             assert csz == [len(f) for f in want], name
             assert out == b"".join(want), name
+            assert tail == guard, name
             assert (st.literals_ms > 0) == (name in ("serial", "caller stream")), name     # per-phase times: one-wave calls only
+            code, _, _, tail = run(**kw, cap=len(out) - 1)
+            assert (code, tail) == (70, guard), name
+        for name, c in (("device waves", waves), ("serial", serial)):
+            out, _, _, tail = run(c, one=True)
+            assert (out, tail) == (first, guard), name
+            code, _, _, tail = run(c, one=True, cap=len(first) - 1)
+            assert (code, tail) == (70, guard), name
     waves.close()
     serial.close()
 

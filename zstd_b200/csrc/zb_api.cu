@@ -200,9 +200,12 @@ struct ZSTD_CCtx_s {
     u32 hostWaveBlocks;            /* host-memory calls: blocks per wave */
     ZbDevBuf<ZbBlock> d_blocks; ZbDevBuf<ZbFrame> d_frames;
     ZbDevBuf<ZbDictSlot> d_dicts; ZbDevBuf<ZbChunk> d_imageChunks;   /* the call's dictionary table, its image builds */
-    ZbDevBuf<u64> d_outOffsets, d_frameSizes;
+    ZbDevBuf<u64> d_outOffsets;
     ZbDevBuf<u64> d_totals;        /* d_totals[w]: bytes produced up to and including wave w */
     ZbHostBuf<u64> h_totals;       /* mirror of d_totals */
+    /* a synchronous call's verdict kernel writes here, [0] the total or an error code, [1 + f] frame f's size: one copy reads
+     * both back into the mirror */
+    ZbDevBuf<unsigned long long> d_verdict; ZbHostBuf<unsigned long long> h_verdict;
     /* host-pointer path staging */
     ZbDevBuf<u8> d_in, d_out;
     std::unique_ptr<ZSTD_CDict, ZbCDictFree> callDict;   /* digest of the dictionary bytes the current call passes; reads the caller's buffer in place */
@@ -314,7 +317,7 @@ static size_t zb_ensureDesc(ZSTD_CCtx* c, size_t nbBlocks, size_t nbFrames, size
 {
     TRY(c->d_chunks.ensure(nbChunks));
     TRY(c->d_blocks.ensure(nbBlocks)); TRY(c->d_outOffsets.ensure(nbBlocks + 1));
-    TRY(c->d_frames.ensure(nbFrames)); TRY(c->d_frameSizes.ensure(nbFrames));
+    TRY(c->d_frames.ensure(nbFrames)); TRY(c->d_verdict.ensure(nbFrames + 1)); TRY(c->h_verdict.ensure(nbFrames + 1));
     TRY(c->d_totals.ensure(nbWaves)); TRY(c->h_totals.ensure(nbWaves));
     return 0;
 }
@@ -733,16 +736,16 @@ static ZbWaves zb_wavePlan(const ZSTD_CCtx* c, const ZbPlan& P, const ZbCall& a)
 }
 
 /* One compression call as its stages see it: zb_compress plans it (zb_plan, zb_wavePlan), sizes its buffers, enqueues it and
- * ends it in one of three ways (DESIGN.md section 2) */
+ * ends it in one of two ways, by where its buffers are (DESIGN.md section 2) */
 struct ZbRun {
     ZSTD_CCtx* c; const ZbCall& a; ZbPlan& P; ZbWaves W;
     cudaStream_t sCopy;                             /* descriptors, dictionaries, input */
     bool timeline;                                  /* ZSTDB200_TIMELINE: print each wave's milestones */
     ZbWorkRows work;                                /* the rows of every slot */
-    u8* d_in; u8* d_out; cudaStream_t sD2H, last;   /* kernel input and output, download stream, the last wave's stream */
+    u8* d_in; u8* d_out; cudaStream_t sD2H;         /* kernel input and output, download stream */
+    unsigned long long *d_result, *d_sizes;         /* where the verdict kernel writes: the caller's memory, or c->d_verdict */
     unsigned launches; size_t err, prefixUp;        /* err: a launch failed; the call still finishes what it queued */
     double t0, hostEnq; std::vector<double> hostDone;   /* host clock: enqueue start and duration, each wave's size seen */
-    std::vector<u64> fsz;                           /* per-frame sizes, read back by synchronous calls */
     std::vector<std::pair<ZSTD_CDict*, u32>> building;   /* images (CDict, index) this call builds; ready once built */
     /* The call's dictionaries on the device, in bulk and one CDict lock at a time (CDicts are shared between contexts on other
      * threads): the tails and entropy states not yet resident are uploaded, then the call synchronises once if a caller's CDict
@@ -848,6 +851,7 @@ struct ZbRun {
         bool const async = a.result != nullptr, ldm = !P.ldm.empty();
         d_in = a.deviceMemory ? (u8*)a.src : c->d_in.p; d_out = a.deviceMemory ? (u8*)a.dst : c->d_out.p;
         sD2H = a.deviceMemory ? (cudaStream_t)0 : c->waveStream[ZB_WAVE_SLOTS_MAX].s;
+        d_result = async ? a.result : c->d_verdict.p; d_sizes = async ? a.d_cSizes : c->d_verdict.p + 1;
         hostDone.assign(W.nbWaves, 0.0);
         t0 = zb_now();
         TRY(call.enter(sCopy));
@@ -865,7 +869,6 @@ struct ZbRun {
         if (async && !call.capturing) { CK(cudaEventRecord(c->evStage[stageSlot], sCopy)); c->stageBusy[stageSlot] = true; }
         if (W.single && !async) CK(cudaEventRecord(c->ev[EV_K0], sCopy));   /* events around each phase of a synchronous wave */
         TRY(runImageBuilds());
-        last = sCopy;
         if (ldm) {
             /* host buffers: the whole input goes up first (a block may copy from any earlier wave), so this upload does not
              * overlap the kernels as the per-wave uploads do */
@@ -894,7 +897,6 @@ struct ZbRun {
                 st = c->waveStream[w % W.slots];
                 CK(cudaStreamWaitEvent(st, c->evH2D[w], 0));
             }
-            last = st;
             err = zb_runBlocks(c, P, d_in, d_dicts, b0, b1, W.wc[w], W.wc[w + 1], rows, st, W.single && !async, &launches);
             if (err) break;
             if (w > 0) CK(cudaStreamWaitEvent(st, c->evStitch[w - 1], 0));
@@ -912,7 +914,8 @@ struct ZbRun {
         hostEnq = zb_now() - t0;
         return 0;
     }
-    /* a stream-ordered call's end: the waves join the caller's stream, which then runs the checksum and verdict kernels */
+    /* the end of every call on device buffers: the waves join sCopy, which then runs the checksum and verdict kernels; a
+     * stream-ordered call then records the context's order event, a synchronous one waits for its verdict */
     size_t finishOrdered(ZbOrder::Call& call) {
         if (!err) {
             if (!W.single) for (u32 s = 0; s < W.slots; s++) {
@@ -920,26 +923,30 @@ struct ZbRun {
                 CK(cudaStreamWaitEvent(sCopy, c->evJoin[s], 0));
             }
             if (a.checksum) { CK(zb_launch_checksums(d_in, c->d_frames, (u32)a.nbFrames, c->d_outOffsets, d_out, W.outCap, sCopy)); launches++; }
-            CK(zb_launch_call_result(c->d_frames, (u32)a.nbFrames, c->d_outOffsets, c->d_totals + W.nbWaves - 1, a.dstCapacity, a.d_cSizes, a.result, sCopy));
+            CK(zb_launch_call_result(c->d_frames, (u32)a.nbFrames, c->d_outOffsets, c->d_totals + W.nbWaves - 1, a.dstCapacity, d_sizes, d_result, sCopy));
             launches++;
         }
-        TRY(call.leave(sCopy));
-        c->stats.launches = launches; c->stats.nbBlocks = (u32)P.blocks.size();
-        return err;
+        if (a.result) { TRY(call.leave(sCopy)); c->stats.launches = launches; c->stats.nbBlocks = (u32)P.blocks.size(); return err; }
+        CK(cudaEventRecord(c->ev[W.single ? EV_KEND : EV_END], sCopy));
+        if (timeline) for (u32 w = 0; w < W.nbWaves && !err; w++) {   /* each wave's milestones, as for host buffers */
+            CK(cudaEventSynchronize(c->evSize[w]));
+            hostDone[w] = zb_now() - t0;
+            CK(cudaEventRecord(c->evD2H[w], sCopy));
+        }
+        return endSync(sCopy, a.cSizes != nullptr);
     }
-    /* the per-frame sizes the frame-sizes kernel wrote on `last`, read back into fsz and the caller's cSizes */
-    size_t readSizes() {
-        fsz.resize(a.nbFrames);
-        CK(cudaMemcpyAsync(fsz.data(), c->d_frameSizes, a.nbFrames * sizeof(u64), cudaMemcpyDeviceToHost, last));
-        CK(cudaStreamSynchronize(last));
-        if (a.cSizes) for (size_t f = 0; f < a.nbFrames; f++) a.cSizes[f] = (size_t)fsz[f];
-        return 0;
-    }
-    /* what both synchronous ends share once their last work is queued: every stream drained, the timeline, the stats */
-    size_t endSync() {
-        if (!W.single) for (u32 s = 0; s < W.slots; s++) if (c->waveStream[s]) CK(cudaStreamSynchronize(c->waveStream[s]));
-        CK(cudaStreamSynchronize(sCopy));
-        u64 const total = err ? 0 : c->h_totals[W.nbWaves - 1];
+    /* what both synchronous ends share once the verdict kernel is queued on `st` behind all of the call's kernels: one copy
+     * reads the verdict back (with every frame's size when `sizes`) and the host waits for it; then the timeline and the
+     * stats.  After a failed launch the host waits for every stream instead. */
+    size_t endSync(cudaStream_t st, bool sizes) {
+        if (err) {
+            if (!W.single) for (u32 s = 0; s < W.slots; s++) CK(cudaStreamSynchronize(c->waveStream[s]));
+            CK(cudaStreamSynchronize(sCopy));
+            return err;
+        }
+        CK(cudaMemcpyAsync(c->h_verdict, c->d_verdict, (sizes ? 1 + a.nbFrames : 1) * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        if (a.cSizes) for (size_t f = 0; f < a.nbFrames; f++) a.cSizes[f] = (size_t)c->h_verdict[1 + f];
         if (timeline) {
             fprintf(stderr, "zstd_b200 timeline (ms after the call's first enqueue; host enqueue loop took %.3f ms; %s)\n", 1e3 * hostEnq,
                     a.deviceMemory ? "device buffers" : "per-wave downloads");
@@ -951,7 +958,6 @@ struct ZbRun {
                         w, W.wb[w], W.wb[w + 1], up, st, 1e3 * hostDone[w], dn);
             }
         }
-        if (err) return err;
         float ms = 0;
         if (W.single) {
             cudaEventElapsedTime(&ms, c->ev[EV_K0], c->ev[EV_KEND]); c->stats.kernel_ms = ms;
@@ -963,29 +969,16 @@ struct ZbRun {
         } else { cudaEventElapsedTime(&ms, c->ev[EV_START], c->ev[EV_END]); c->stats.kernel_ms = ms; }
         c->stats.total_ms = c->stats.kernel_ms;
         c->stats.launches = launches; c->stats.nbBlocks = (u32)P.blocks.size();
-        if (!a.deviceMemory) { c->stats.h2d_bytes = W.inEnd + prefixUp; c->stats.d2h_bytes = (size_t)total; }
-        if (total > a.dstCapacity) return ZB_ERR(ZB_error_dstSize_tooSmall);
-        return (size_t)total;
+        if (!a.deviceMemory) { c->stats.h2d_bytes = W.inEnd + prefixUp; c->stats.d2h_bytes = (size_t)c->h_totals[W.nbWaves - 1]; }
+        return (size_t)c->h_verdict[0];
     }
-    /* a synchronous call's end on device buffers: the checksum kernel (a warp per frame), the frame sizes, the read-back */
-    size_t finishDevice() {
-        if (a.checksum && !err) { CK(zb_launch_checksums(d_in, c->d_frames, (u32)a.nbFrames, c->d_outOffsets, d_out, W.outCap, last)); launches++; }
-        if (timeline) for (u32 w = 0; w < W.nbWaves && !err; w++) {   /* each wave's milestones, as for host buffers */
-            CK(cudaEventSynchronize(c->evSize[w]));
-            hostDone[w] = zb_now() - t0;
-            CK(cudaEventRecord(c->evD2H[w], last));
-        }
-        if (!err && a.cSizes) { CK(zb_launch_frame_sizes(c->d_frames, (u32)a.nbFrames, c->d_outOffsets, c->d_frameSizes, last)); launches += W.single; }   /* a multi-wave call's count leaves it out */
-        if (W.single) CK(cudaEventRecord(c->ev[EV_KEND], last));
-        if (!err && !timeline) CK(cudaMemcpyAsync(c->h_totals + W.nbWaves - 1, c->d_totals + W.nbWaves - 1, sizeof(u64), cudaMemcpyDeviceToHost, last));
-        if (!err && a.cSizes) TRY(readSizes());
-        if (!W.single) CK(cudaEventRecord(c->ev[EV_END], last));      /* the last wave's stitch is ordered behind every earlier one */
-        return endSync();
-    }
-    /* a synchronous call's end on host buffers: XXH64 on up to 8 host threads while the GPU works, each wave downloaded as its
-     * size arrives, the checksums written into the 4 bytes the size scan left free behind every frame */
+    /* a synchronous call's end on host buffers: the verdict kernel behind the last wave's stitch (host calls always run in
+     * waves), XXH64 on up to 8 host threads while the GPU works, each wave downloaded as its size arrives, the checksums
+     * written into the 4 bytes the size scan left free behind every frame */
     size_t finishHost() {
         const u8* const src = (const u8*)a.src; u8* const dst = (u8*)a.dst;
+        cudaStream_t const last = c->waveStream[(W.nbWaves - 1u) % W.slots];   /* ordered behind every earlier wave's stitch */
+        if (!err) { CK(zb_launch_call_result(c->d_frames, (u32)a.nbFrames, c->d_outOffsets, c->d_totals + W.nbWaves - 1, a.dstCapacity, d_sizes, d_result, last)); launches++; }
         std::vector<u64> xxh;
         if (a.checksum && !err) {
             xxh.resize(a.nbFrames);
@@ -1005,11 +998,10 @@ struct ZbRun {
             if (total <= W.outCap) prev = total;
             if (timeline) CK(cudaEventRecord(c->evD2H[w], sD2H));
         }
-        if (!err && (a.cSizes || a.checksum)) { CK(zb_launch_frame_sizes(c->d_frames, (u32)a.nbFrames, c->d_outOffsets, c->d_frameSizes, last)); TRY(readSizes()); }   /* host calls are never single: not counted */
         CK(cudaEventRecord(c->ev[EV_END], sD2H)); CK(cudaStreamSynchronize(sD2H));
-        size_t const total = endSync();
+        size_t const total = endSync(last, a.cSizes || a.checksum);
         if (!zb_isErr(total) && a.checksum) for (size_t f = 0, end = 0; f < a.nbFrames; f++) {
-            end += fsz[f];
+            end += c->h_verdict[1 + f];
             if (end < 4 || end > total) break;
             u32 const ck = (u32)xxh[f];
             dst[end - 4] = (u8)ck; dst[end - 3] = (u8)(ck >> 8); dst[end - 2] = (u8)(ck >> 16); dst[end - 1] = (u8)(ck >> 24);
@@ -1042,8 +1034,7 @@ static size_t zb_compress(ZSTD_CCtx* c, const ZbCall& a)
     r.timeline = !r.W.single && !async && getenv("ZSTDB200_TIMELINE") != NULL;
     TRY(call.size([&] { return r.sizeBuffers(); }));
     TRY(r.enqueue(call));
-    if (async) return r.finishOrdered(call);
-    return a.deviceMemory ? r.finishDevice() : r.finishHost();
+    return a.deviceMemory ? r.finishOrdered(call) : r.finishHost();
 }
 
 /* dictionary bytes passed to a call, digested into the context's callDict (*out = NULL without a dictionary) */

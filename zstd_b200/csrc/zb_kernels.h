@@ -79,9 +79,7 @@ cudaError_t zb_launch_stitch(const u8* d_src, const ZbBlock* d_blocks, u32 nbBlo
                              u64* d_outOffsets, const u64* d_base, u64* d_total,
                              u8* d_dst, u64 dstCapacity, cudaStream_t stream);
 cudaError_t zb_launch_checksums(const u8* d_src, const ZbFrame* d_frames, u32 nbFrames, const u64* d_outOffsets, u8* d_dst, u64 dstCapacity, cudaStream_t stream);
-cudaError_t zb_launch_frame_sizes(const ZbFrame* d_frames, u32 nbFrames, const u64* d_outOffsets,
-                                  u64* d_frameSizes, cudaStream_t stream);
-/* the last kernel of a stream-ordered call: d_cSizes[f] (d_cSizes may be NULL) and *d_result = *d_total, or dstSize_tooSmall
+/* the last kernel of a call: d_cSizes[f] (d_cSizes may be NULL) and *d_result = *d_total, or dstSize_tooSmall
  * when *d_total > dstCapacity; d_total NULL (no frames): 0 */
 cudaError_t zb_launch_call_result(const ZbFrame* d_frames, u32 nbFrames, const u64* d_outOffsets, const u64* d_total,
                                   u64 dstCapacity, unsigned long long* d_cSizes, unsigned long long* d_result, cudaStream_t stream);

@@ -72,19 +72,9 @@ zb_sizes_scan_kernel(const ZbBlock* __restrict__ blocks, u32 nbBlocks, const ZbF
     if (tid == SCAN_THREADS - 1) { outOffsets[nbBlocks] = base + part[SCAN_THREADS - 1]; *total = base + part[SCAN_THREADS - 1]; }
 }
 
-/* per-frame compressed sizes from the (final) block offsets */
-__global__ void zb_frame_sizes_kernel(const ZbFrame* __restrict__ frames, u32 nbFrames,
-                                      const u64* __restrict__ outOffsets, u64* __restrict__ frameSizes)
-{
-    u32 const f = blockIdx.x * blockDim.x + threadIdx.x;
-    if (f >= nbFrames) return;
-    ZbFrame const fr = frames[f];
-    frameSizes[f] = outOffsets[fr.firstBlock + fr.nbBlocks] - outOffsets[fr.firstBlock];
-}
-
-/* the verdict of a stream-ordered call (ZSTDB200_compressDeviceAsync / ZSTDB200_compressFramesAsync), left in device memory:
- * each frame's size (cSizes may be NULL) and the call's total, or dstSize_tooSmall when the frames did not fit in dstCapacity
- * (K4 wrote nothing past it).  total NULL: a call without frames, whose total is 0. */
+/* the verdict of a call, left in device memory (the caller's for a stream-ordered call, else the context's, which the host
+ * reads back): each frame's size (cSizes may be NULL) and the call's total, or dstSize_tooSmall when the frames did not fit
+ * in dstCapacity (K4 wrote nothing past it).  total NULL: a call without frames, whose total is 0. */
 __global__ void zb_call_result_kernel(const ZbFrame* __restrict__ frames, u32 nbFrames, const u64* __restrict__ outOffsets,
                                       const u64* __restrict__ total, u64 dstCapacity, unsigned long long* cSizes, unsigned long long* result)
 {
@@ -254,14 +244,6 @@ extern "C" cudaError_t zb_launch_checksums(const u8* d_src, const ZbFrame* d_fra
 {
     if (nbFrames == 0) return cudaSuccess;
     zb_checksum_kernel<<<(nbFrames + XXH_WARPS - 1u) / XXH_WARPS, 32 * XXH_WARPS, 0, stream>>>(d_src, d_frames, nbFrames, d_outOffsets, d_dst, dstCapacity);
-    return cudaGetLastError();
-}
-
-extern "C" cudaError_t zb_launch_frame_sizes(const ZbFrame* d_frames, u32 nbFrames, const u64* d_outOffsets,
-                                             u64* d_frameSizes, cudaStream_t stream)
-{
-    if (nbFrames == 0) return cudaSuccess;
-    zb_frame_sizes_kernel<<<(nbFrames + 255) / 256, 256, 0, stream>>>(d_frames, nbFrames, d_outOffsets, d_frameSizes);
     return cudaGetLastError();
 }
 
