@@ -5,7 +5,9 @@ counts which path every probe takes.  TEST INFRASTRUCTURE ONLY.
 The restatement is fed the candidate arrays of the oracle's own walk (zbo_walkChunk) and is driven block by block as
 zbo_compress_usingDict drives zbo_parseBlock (oracle/zb_frame.c); tests/test_gpu_dfast_paths.py proves it equal to
 zbo_parseBlock on every block, so its path counts are the oracle's.  Switches replace one rule by a neighbouring wrong
-one: the inputs must tell each of them apart from the rule."""
+one: the inputs must tell each of them apart from the rule.
+
+frame_blocks and the join of parse_block serve the fast parse's restatement too (tests/fastgen.py)."""
 import ctypes
 import random
 
@@ -361,18 +363,18 @@ def patch_reps(dict_bytes: bytes, reps) -> bytes:
 class Block:
     """one block as zbo_parseBlock sees it: the buffer (dictionary tail + frame), the chunk's candidate arrays (as lists,
     index = position - chunk start), the block's bounds and its history limit"""
-    __slots__ = ("buf", "dL", "dS", "c0", "low", "chunk_low", "bs", "be", "frame_start", "start_reps", "code_reps", "oracle_seqs")
+    __slots__ = ("buf", "dL", "dS", "c0", "low", "chunk_low", "window", "bs", "be", "frame_start", "start_reps", "code_reps",
+                 "strategy", "mls", "step_size", "oracle_seqs")
 
 
 def frame_blocks(src: bytes, level: int, dict_bytes=None):
     """the blocks of one frame, driven as zbo_compress_usingDict drives the match finder (oracle/zb_frame.c:117-186); each
-    carries zbo_parseBlock's own sequences.  Only doubleFast frames."""
+    carries zbo_parseBlock's own sequences.  Fast frames (strategy 1) have no long candidates: dL is None."""
     O = _oracle()
     use = dict_bytes is not None and len(dict_bytes) >= 8
     cp = O.zbo_getCParams(level, len(src), len(dict_bytes) if use else 0)
     plan = OPlan()
     O.zbo_makePlan(ctypes.byref(plan), ctypes.byref(cp))
-    assert plan.strategy == 2, (level, len(src))
     D, start_reps, code_reps, buf = 0, (0, 0), (1, 4, 8), src
     if use:
         de = DictEntropy()
@@ -408,15 +410,16 @@ def frame_blocks(src: bytes, level: int, dict_bytes=None):
                 cc = ChunkCand()
                 O.zbo_walkChunk(ctypes.byref(plan), buf, len(buf), cs + D, ce + D, ctypes.byref(cc))
                 m = cc.end - cc.start
-                lists = (np.ctypeslib.as_array(cc.dL, shape=(m,)).tolist() + [0] * 8,
+                lists = (np.ctypeslib.as_array(cc.dL, shape=(m,)).tolist() + [0] * 8 if plan.strategy == 2 else None,
                          np.ctypeslib.as_array(cc.dS, shape=(m,)).tolist() + [0] * 8)
             nb = O.zbo_parseBlock(ctypes.byref(plan), buf, ctypes.byref(cc), bs + D, bsz, seqs, lit, ctypes.byref(lsz))
             b = Block()
             b.buf, b.dL, b.dS, b.c0 = buf, lists[0], lists[1], cc.start
             b.bs, b.be, b.frame_start = bs + D, bs + D + bsz, D
-            b.chunk_low = cc.low
+            b.chunk_low, b.window = cc.low, W
             b.low = cc.low if not (b.be > W and b.be - W > cc.low) else b.be - W     # block_low
             b.start_reps, b.code_reps = start_reps, code_reps
+            b.strategy, b.mls, b.step_size = plan.strategy, plan.mls, plan.stepSize
             b.oracle_seqs = [(seqs[i].offBase, seqs[i].litLen, seqs[i].matchLen) for i in range(nb)]
             blocks.append(b)
     finally:
@@ -638,14 +641,16 @@ def parse_segment(blk: Block, ss: int, se: int, sw=frozenset(), cnt=None):
     return out
 
 
-def parse_block(blk: Block, sw=frozenset(), cnt=None):
-    """zbo_parseBlock (oracle/zb_match.c:308-352): the segments' raw sequences joined, repcodes assigned over the block"""
+def parse_block(blk: Block, sw=frozenset(), cnt=None, segment=None):
+    """zbo_parseBlock (oracle/zb_match.c:308-352): the segments' raw sequences joined, repcodes assigned over the block.
+    `segment` parses one segment (default: the doubleFast parse above; fastgen.parse_segment for the fast parse)."""
     c = cnt if cnt is not None else {}
+    segment = segment or parse_segment
     cur, seqs = blk.bs, []
     r1, r2, r3 = blk.code_reps if blk.bs == blk.frame_start else (0, 0, 0)
     for ss in range(blk.bs, blk.be, SEG):
         se = min(ss + SEG, blk.be)
-        for ms, mlen, off in parse_segment(blk, ss, se, sw, c):
+        for ms, mlen, off in segment(blk, ss, se, sw, c):
             if ms + mlen <= cur:
                 c["join_drop"] = c.get("join_drop", 0) + 1
                 continue
