@@ -364,15 +364,23 @@ class Block:
     """one block as zbo_parseBlock sees it: the buffer (dictionary tail + frame), the chunk's candidate arrays (as lists,
     index = position - chunk start), the block's bounds and its history limit"""
     __slots__ = ("buf", "dL", "dS", "c0", "low", "chunk_low", "window", "bs", "be", "frame_start", "start_reps", "code_reps",
-                 "strategy", "mls", "step_size", "oracle_seqs")
+                 "strategy", "mls", "step_size", "oracle_seqs", "index", "ldm_reps")
 
 
-def frame_blocks(src: bytes, level: int, dict_bytes=None):
+def frame_blocks(src: bytes, level: int, dict_bytes=None, ldm=False):
     """the blocks of one frame, driven as zbo_compress_usingDict drives the match finder (oracle/zb_frame.c:117-186); each
-    carries zbo_parseBlock's own sequences.  Fast frames (strategy 1) have no long candidates: dL is None."""
+    carries zbo_parseBlock's own sequences.  Fast frames (strategy 1) have no long candidates: dL is None.
+    ldm: a frame of more than 512 KiB with long-distance matching, driven as zbo_compress_ldm_usingDict does
+    (oracle/zb_ldm.c): the LDM cParams, and each block's repcodes for the overlay in ldm_reps (the frame's codeRep in its
+    first block, else none); block k of the frame has index k."""
     O = _oracle()
     use = dict_bytes is not None and len(dict_bytes) >= 8
-    cp = O.zbo_getCParams(level, len(src), len(dict_bytes) if use else 0)
+    if ldm:
+        import ldmref
+        assert len(src) > 4 * BLOCK, "frames of at most one chunk are compressed as without LDM"
+        cp = ldmref.cparams_ldm(level, len(src), len(dict_bytes) if use else 0)
+    else:
+        cp = O.zbo_getCParams(level, len(src), len(dict_bytes) if use else 0)
     plan = OPlan()
     O.zbo_makePlan(ctypes.byref(plan), ctypes.byref(cp))
     D, start_reps, code_reps, buf = 0, (0, 0), (1, 4, 8), src
@@ -421,6 +429,8 @@ def frame_blocks(src: bytes, level: int, dict_bytes=None):
             b.start_reps, b.code_reps = start_reps, code_reps
             b.strategy, b.mls, b.step_size = plan.strategy, plan.mls, plan.stepSize
             b.oracle_seqs = [(seqs[i].offBase, seqs[i].litLen, seqs[i].matchLen) for i in range(nb)]
+            b.index = bs // block_max
+            b.ldm_reps = code_reps if bs == 0 else (0, 0, 0)
             blocks.append(b)
     finally:
         if cc is not None:

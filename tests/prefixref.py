@@ -12,13 +12,7 @@ INDEX_MAX = 1 << 27                   # the prefix bytes a block can reach: the 
 LDM_MIN = 512 << 10                   # LDM runs when indexed prefix + frame is larger
 
 
-class _Match(ctypes.Structure):
-    _fields_ = [("start", ctypes.c_uint), ("len", ctypes.c_uint), ("off", ctypes.c_uint)]
-
-
-class _Lists(ctypes.Structure):
-    _fields_ = [("nbBlocks", _sz), ("nbSurvivors", _sz), ("first", ctypes.POINTER(ctypes.c_uint64)), ("cnt", ctypes.POINTER(ctypes.c_uint)),
-                ("m", ctypes.POINTER(_Match))]
+_Lists = ldmref.LdmLists              # zbo_ldm_free is bound once, for both list producers
 
 
 def _o():
