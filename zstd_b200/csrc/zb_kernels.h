@@ -22,6 +22,14 @@ extern "C" {
  * zb_launch_dict_images: one CTA per image, image i walks the tail of d_dicts[d_imageChunks[i].dictSlot] (a chunk of
  * size 0 whose history is that tail) into that entry's image. */
 cudaError_t zb_launch_dict_images(const ZbDictSlot* d_dicts, const ZbChunk* d_imageChunks, u32 nbImages, const ZbParams* prm, cudaStream_t stream);
+/* K1a alone, one table (zb_launch_match runs it once per table; the walk test harness, tests/walk_harness.cu, on its own):
+ * one CTA per chunk walks the chunk's history and bytes with `mls`-byte hashes into a table of N buckets (N * 4 bytes of
+ * shared memory, at most 226 KiB).  build = false: writes dist (u16, ZB_FAR = see far) and far (u32, only where dist is
+ * ZB_FAR) at [0, size) of row firstBlock - slotFirstBlock + k of block k of each chunk (rows sd.dist apart), and nothing
+ * else.  build = true (d_src NULL): walks each chunk's dictionary tail and writes the table to d_dicts[dictSlot].image +
+ * imageOff (N u32), and nothing else.  A first chunk whose dictionary entry has an image starts from image + imageOff. */
+cudaError_t zb_launch_walk(const u8* d_src, const ZbDictSlot* d_dicts, const ZbChunk* d_chunks, u32 nbChunks, u32 mls, u32 N, u32 insStep,
+                           const ZbStrides& sd, u32 slotFirstBlock, u16* d_dist, u32* d_far, u32 imageOff, bool build, cudaStream_t stream);
 cudaError_t zb_launch_match(const u8* d_src, const ZbDictSlot* d_dicts, bool dict, const ZbBlock* d_blocks, u32 nbBlocks,
                             const ZbChunk* d_chunks, u32 nbChunks, u32 slotFirstBlock, const ZbParams* prm, const ZbWorkRows* rows,
                             cudaEvent_t evMid, cudaStream_t stream, const ZbLdmView* ldm = nullptr);

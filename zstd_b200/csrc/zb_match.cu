@@ -892,8 +892,8 @@ static cudaError_t zb_launch_walk_m(const u8* d_src, const ZbDictSlot* d_dicts, 
     if (smem <= 113u * 1024u) return zb_launch_walk_p<MLS, WALK_P_MID>(d_src, d_dicts, d_chunks, nbChunks, N, insStep, sd, slotFirstBlock, d_dist, d_far, imageOff, build, stream);
     return zb_launch_walk_p<MLS, 1>(d_src, d_dicts, d_chunks, nbChunks, N, insStep, sd, slotFirstBlock, d_dist, d_far, imageOff, build, stream);
 }
-static cudaError_t zb_launch_walk(const u8* d_src, const ZbDictSlot* d_dicts, const ZbChunk* d_chunks, u32 nbChunks, u32 mls, u32 N, u32 insStep, const ZbStrides& sd,
-                                  u32 slotFirstBlock, u16* d_dist, u32* d_far, u32 imageOff, bool build, cudaStream_t stream)
+extern "C" cudaError_t zb_launch_walk(const u8* d_src, const ZbDictSlot* d_dicts, const ZbChunk* d_chunks, u32 nbChunks, u32 mls, u32 N, u32 insStep, const ZbStrides& sd,
+                                      u32 slotFirstBlock, u16* d_dist, u32* d_far, u32 imageOff, bool build, cudaStream_t stream)
 {
     switch (mls) {
     case 4: return zb_launch_walk_m<4>(d_src, d_dicts, d_chunks, nbChunks, N, insStep, sd, slotFirstBlock, d_dist, d_far, imageOff, build, stream);
