@@ -652,46 +652,15 @@ def parse_segment(blk: Block, ss: int, se: int, sw=frozenset(), cnt=None):
 
 
 def parse_block(blk: Block, sw=frozenset(), cnt=None, segment=None):
-    """zbo_parseBlock (oracle/zb_match.c:308-352): the segments' raw sequences joined, repcodes assigned over the block.
+    """zbo_parseBlock (oracle/zb_match.c:308-352): the segments' raw sequences joined, repcodes assigned over the block
+    (mergegen.join, the restatement the merge kernels are tested against).
     `segment` parses one segment (default: the doubleFast parse above; fastgen.parse_segment for the fast parse)."""
+    import mergegen
     c = cnt if cnt is not None else {}
     segment = segment or parse_segment
-    cur, seqs = blk.bs, []
-    r1, r2, r3 = blk.code_reps if blk.bs == blk.frame_start else (0, 0, 0)
-    for ss in range(blk.bs, blk.be, SEG):
-        se = min(ss + SEG, blk.be)
-        for ms, mlen, off in segment(blk, ss, se, sw, c):
-            if ms + mlen <= cur:
-                c["join_drop"] = c.get("join_drop", 0) + 1
-                continue
-            if ms < cur:
-                if ms + mlen - cur < 3:
-                    c["join_drop"] = c.get("join_drop", 0) + 1
-                    continue
-                c["join_trim"] = c.get("join_trim", 0) + 1
-                mlen, ms = ms + mlen - cur, cur
-            ll = ms - cur
-            if ll > 0:
-                if off == r1:
-                    ob = 1
-                elif off == r2:
-                    ob, r2, r1 = 2, r1, off
-                elif off == r3:
-                    ob, r3, r2, r1 = 3, r2, r1, off
-                else:
-                    ob, r3, r2, r1 = off + 3, r2, r1, off
-            else:
-                if off == r2:
-                    ob, r2, r1 = 1, r1, off
-                elif off == r3:
-                    ob, r3, r2, r1 = 2, r2, r1, off
-                elif r1 > 1 and off == r1 - 1:
-                    ob, r3, r2, r1 = 3, r2, r1, off
-                else:
-                    ob, r3, r2, r1 = off + 3, r2, r1, off
-            seqs.append((ob, ll, mlen))
-            cur = ms + mlen
-    return seqs
+    segs = [segment(blk, ss, min(ss + SEG, blk.be), sw, c) for ss in range(blk.bs, blk.be, SEG)]
+    reps = blk.code_reps if blk.bs == blk.frame_start else (0, 0, 0)
+    return mergegen.join(segs, reps, blk.bs, sw, c)
 
 
 # -------------------------------------------------------------------------------------------------- the GPU cases

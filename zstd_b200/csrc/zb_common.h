@@ -199,6 +199,12 @@ static inline ZB_HD u64 zb_pack_seq(u32 offBase, u32 litLen, u32 matchLen)
 #define ZB_SEQ_OFFBASE(q) ((u32)(q) & 0xFFFFFFFu)
 #define ZB_SEQ_LL(q)      ((u32)((q) >> 28) & 0x3FFFFu)
 #define ZB_SEQ_ML(q)      ((u32)((q) >> 46) & 0x3FFFFu)
+/* a raw sequence, as the parse kernels (K1b) leave it for the merge (K1c): real offset (24 bits), match length (18 bits),
+ * match start relative to the block above them */
+static inline ZB_HD u64 zb_pack_raw(u32 off, u32 mlen, u32 msRel) { return (u64)off | ((u64)mlen << 24) | ((u64)msRel << 42); }
+#define ZB_RAW_OFF(r)  ((u32)(r) & 0xFFFFFFu)
+#define ZB_RAW_MLEN(r) ((u32)((r) >> 24) & 0x3FFFFu)
+#define ZB_RAW_MS(r)   ((u32)((r) >> 42))
 
 /* Long-distance matching (zb_ldm.cu; the rule: oracle/zb_ldm.c).  Frames of more than one chunk only. */
 #define ZB_LDM_WINDOW_LOG 27u                                  /* ZSTD_LDM_DEFAULT_WINDOW_LOG, zstd_ldm.h:25 */

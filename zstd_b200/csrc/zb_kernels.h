@@ -34,6 +34,16 @@ cudaError_t zb_launch_match(const u8* d_src, const ZbDictSlot* d_dicts, bool dic
                             const ZbChunk* d_chunks, u32 nbChunks, u32 slotFirstBlock, const ZbParams* prm, const ZbWorkRows* rows,
                             cudaEvent_t evMid, cudaStream_t stream, const ZbLdmView* ldm = nullptr);
 /* ldm (K1c): the launch's blocks' long-distance matches (zb_launch_ldm), laid over the parse output; NULL = none */
+/* K1c alone (zb_launch_match runs it behind the parse; the merge test harness, tests/merge_harness.cu, on its own): joins
+ * each block's parse segments, assigns the repcodes and gathers the literals.  zb_merge_small_kernel (one warp per block)
+ * when the rows hold one segment of at most 8192 bytes, else zb_merge_segments_kernel (one CTA per block), its LDM variant
+ * when ldm is given.  Reads, for each block b of at least 7 bytes: rows->segmeta (zb_segsPerRow records of row b), the
+ * raw sequences (zb_pack_raw) of segment k at seq slot k * ZB_PARSE_SEG / 4 of row b, d_src at the block, d_blocks[b],
+ * d_dicts[dictSlot].codeRep of a first block (d_dicts NULL: {1,4,8}) and, for LDM, ldm->match[first[b], + cnt[b]).
+ * Writes seqs[0, nbSeq) (zb_pack_seq: offBase, litLength, matchLength), lits[0, litSize) and meta of those blocks, and
+ * for LDM the block's far and dist rows as scratch; blocks of fewer than 7 bytes (meta written by the parse) not at all. */
+cudaError_t zb_launch_merge(const u8* d_src, const ZbDictSlot* d_dicts, const ZbBlock* d_blocks, u32 nbBlocks, const ZbWorkRows* rows,
+                            const ZbLdmView* ldm, cudaStream_t stream);
 
 /* Long-distance matching of one frame of n bytes at d_frame behind P indexed prefix bytes at d_prefix (P = 0: none; the two
  * need not be adjacent) (zb_ldm.cu): nbBlocks blocks of ZB_BLOCK_MAX bytes, the frame's; block k's matches go to

@@ -60,12 +60,6 @@ __device__ __forceinline__ u32 zb_back_coop(const ZbSeg& sg, u32 probe, u32 offs
     }
 }
 
-/* raw sequence of the parse kernels: real offset, match length, match start relative to the block */
-__device__ __forceinline__ u64 zb_pack_raw(u32 off, u32 mlen, u32 msRel) { return (u64)off | ((u64)mlen << 24) | ((u64)msRel << 42); }
-#define ZB_RAW_OFF(r)  ((u32)(r) & 0xFFFFFFu)
-#define ZB_RAW_MLEN(r) ((u32)((r) >> 24) & 0x3FFFFu)
-#define ZB_RAW_MS(r)   ((u32)((r) >> 42))
-
 /* ------------------------------------------------------------------------------------------------
  * K1a — candidate walk (parse-independent).  One CTA per chunk, table in shared memory.
  * dist[p] = distance from p to its candidate: the latest earlier position that was inserted into p's bucket and has
@@ -924,7 +918,7 @@ extern "C" cudaError_t zb_launch_match(const u8* d_src, const ZbDictSlot* d_dict
     if (nbBlocks == 0) return cudaSuccess;
     ZbStrides const sd = rows->sd;
     u16* const d_dist = rows->dist; u32* const d_far = rows->far; u16* const d_dist2 = rows->dist2; u32* const d_far2 = rows->far2;
-    u64* const d_seqs = rows->seqs; u8* const d_lits = rows->lits; ZbBlockMeta* const d_meta = rows->meta; ZbSegMeta* const d_segmeta = rows->segmeta;
+    u64* const d_seqs = rows->seqs; ZbBlockMeta* const d_meta = rows->meta; ZbSegMeta* const d_segmeta = rows->segmeta;
     cudaError_t e;
     u32 const segs = zb_segsPerRow(sd);
     u32 const sgrid = (u32)(((u64)nbBlocks * segs + PARSE_WARPS - 1) / PARSE_WARPS);                       /* one warp per segment */
@@ -941,11 +935,20 @@ extern "C" cudaError_t zb_launch_match(const u8* d_src, const ZbDictSlot* d_dict
         if (dict) zb_parse_kernel<true><<<sgrid, 32 * PARSE_WARPS, 0, stream>>>(d_src, d_dicts, d_blocks, nbBlocks, *prm, sd, d_dist, d_far, d_seqs, d_meta, d_segmeta);
         else      zb_parse_kernel<false><<<sgrid, 32 * PARSE_WARPS, 0, stream>>>(d_src, d_dicts, d_blocks, nbBlocks, *prm, sd, d_dist, d_far, d_seqs, d_meta, d_segmeta);
     }
+    return zb_launch_merge(d_src, d_dicts, d_blocks, nbBlocks, rows, ldm, stream);
+}
+
+extern "C" cudaError_t zb_launch_merge(const u8* d_src, const ZbDictSlot* d_dicts, const ZbBlock* d_blocks, u32 nbBlocks, const ZbWorkRows* rows,
+                                       const ZbLdmView* ldm, cudaStream_t stream)
+{
+    if (nbBlocks == 0) return cudaSuccess;
+    ZbStrides const sd = rows->sd;
+    u32 const segs = zb_segsPerRow(sd);
     if (segs == 1u && sd.dist <= 8192u)
-        zb_merge_small_kernel<<<(nbBlocks + MERGE_THREADS / 32u - 1u) / (MERGE_THREADS / 32u), MERGE_THREADS, 0, stream>>>(d_src, d_dicts, d_blocks, nbBlocks, sd, d_segmeta, d_seqs, d_lits, d_meta);
+        zb_merge_small_kernel<<<(nbBlocks + MERGE_THREADS / 32u - 1u) / (MERGE_THREADS / 32u), MERGE_THREADS, 0, stream>>>(d_src, d_dicts, d_blocks, nbBlocks, sd, rows->segmeta, rows->seqs, rows->lits, rows->meta);
     else if (ldm)                                                /* scratch in the dead candidate rows: far, then dist (zb_workLayout) */
-        zb_merge_segments_kernel<true><<<nbBlocks, MERGE_THREADS, 0, stream>>>(d_src, d_dicts, d_blocks, sd, d_segmeta, d_seqs, d_lits, d_meta, *ldm, d_far, d_dist);
+        zb_merge_segments_kernel<true><<<nbBlocks, MERGE_THREADS, 0, stream>>>(d_src, d_dicts, d_blocks, sd, rows->segmeta, rows->seqs, rows->lits, rows->meta, *ldm, rows->far, rows->dist);
     else
-        zb_merge_segments_kernel<false><<<nbBlocks, MERGE_THREADS, 0, stream>>>(d_src, d_dicts, d_blocks, sd, d_segmeta, d_seqs, d_lits, d_meta, ZbLdmView(), nullptr, nullptr);
+        zb_merge_segments_kernel<false><<<nbBlocks, MERGE_THREADS, 0, stream>>>(d_src, d_dicts, d_blocks, sd, rows->segmeta, rows->seqs, rows->lits, rows->meta, ZbLdmView(), nullptr, nullptr);
     return cudaGetLastError();
 }
