@@ -307,6 +307,47 @@ ZSTDB200_API size_t ZSTDB200_decompressDeviceAsync(ZSTD_DCtx* dctx, void* d_dst,
                                                    const void* d_src, size_t srcSize,
                                                    unsigned long long* d_result, void* stream);
 
+/* Decompress a batch of independent entries in one call (the counterpart of ZSTDB200_compressFrames): each entry into its
+ * own slot of the output, each with its own result, the entries' headers walked side by side on the GPU.
+ * Buffers and arrays.  d_src and d_dst are device memory.  srcOffsets, srcSizes, dstOffsets and dstCapacities are host
+ * arrays of nbEntries values, read before the call returns.
+ * Entry i is d_src[srcOffsets[i], + srcSizes[i]).  It may hold anything ZSTDB200_decompressDevice accepts: one or more frames,
+ * skippable frames.  Its result equals what ZSTDB200_decompressDevice(dctx, d_dst + dstOffsets[i], dstCapacities[i],
+ * d_src + srcOffsets[i], srcSizes[i], ...) returns with the same sticky dictionary: the decompressed size or an error code.
+ * Content checksums are not verified, as on that call.  An entry of 0 bytes gives 0.
+ * Writes.  Nothing is written outside an entry's slot d_dst[dstOffsets[i], + dstCapacities[i]).  An error found before an
+ * entry's output is placed (a corrupt header or block, a content size that does not match, dstSize_tooSmall (70)) leaves its
+ * slot untouched.
+ * Per-entry results.  dSizes[i] (host array) or d_dSizes[i] (device, managed or mapped page-locked memory) receives entry i's
+ * result; either may be NULL.
+ * Return value.  ZSTDB200_decompressFrames returns the sum of the entries' sizes when every entry decoded, otherwise the error
+ * code of the lowest-index entry that failed: ZSTD_isError on it says "look at the sizes".  ZSTDB200_decompressFramesAsync
+ * returns 0 once the work is enqueued, and *d_result receives that same value in stream order.
+ * Refusals, decided before anything is enqueued (dSizes is then not written): ZSTD_error_GENERIC (1) without a device, with
+ * d_result NULL or an array NULL; parameter_unsupported (40) while a ZSTD_DCtx_refPrefix is pending (the prefix is forgotten);
+ * parameter_outOfBound (42) when a source range lies outside [0, srcSize), a slot outside [0, dstCapacity), or the slots are
+ * not ascending and disjoint (dstOffsets[i] + dstCapacities[i] <= dstOffsets[i + 1]; overlapping slots would race); checked
+ * in O(nbEntries); memory_allocation (64); stage_wrong (60) under capture, as below.  nbEntries = 0 gives 0.
+ * Workspace.  Sized from host-known numbers, as for ZSTDB200_decompressDeviceAsync, so the host reads no header: up to
+ * B + nbEntries blocks and as many frames, B = srcSize / 16 + dstCapacity / 1024 + 1024, literals and sequences sized from
+ * the sum of dstCapacities.  An entry whose blocks or frames fall past that bound gets workSpace_tooSmall (66); the others
+ * still decode.  The workspace is given out in entry order, and an entry that gets 66 takes none of it.
+ * Ordering, capture and stats: as for ZSTDB200_decompressDeviceAsync.  The calls made on one context run in the order they
+ * are made; a context sized by an earlier call of the same shape or a larger one neither synchronises nor allocates; a CUDA
+ * graph captured after such a call replays on whatever bytes lie at d_src, with the offsets and capacities of the captured
+ * call.  The offset arrays are staged in a ring of ZSTDB200_ASYNC_SLOTS page-locked slots (the host waits when the next
+ * slot's call has not uploaded them yet).  ZSTDB200_getLastDStats fills launches, which does not depend on nbEntries.
+ * ZSTDB200_decompressFrames is the stream-ordered call plus one read-back of the verdict and the sizes; a NULL stream
+ * means the context's own stream, as for ZSTDB200_decompressDevice. */
+ZSTDB200_API size_t ZSTDB200_decompressFrames(ZSTD_DCtx* dctx,
+        void* d_dst, size_t dstCapacity, const size_t* dstOffsets, const size_t* dstCapacities,
+        const void* d_src, size_t srcSize, const size_t* srcOffsets, const size_t* srcSizes,
+        size_t nbEntries, size_t* dSizes, void* stream);
+ZSTDB200_API size_t ZSTDB200_decompressFramesAsync(ZSTD_DCtx* dctx,
+        void* d_dst, size_t dstCapacity, const size_t* dstOffsets, const size_t* dstCapacities,
+        const void* d_src, size_t srcSize, const size_t* srcOffsets, const size_t* srcSizes,
+        size_t nbEntries, unsigned long long* d_dSizes, unsigned long long* d_result, void* stream);
+
 
 /* Compress one frame whose input and output already live in device memory (HBM).  The call returns when the frame is
  * complete (it synchronises to read the size).

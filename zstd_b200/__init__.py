@@ -151,6 +151,11 @@ def lib() -> ctypes.CDLL:
         if hasattr(L, "ZSTDB200_decompressDeviceAsync"):                                # absent from older development builds
             L.ZSTDB200_decompressDeviceAsync.restype = _sz
             L.ZSTDB200_decompressDeviceAsync.argtypes = [_vp, _vp, _sz, _vp, _sz, _vp, _vp]
+        if hasattr(L, "ZSTDB200_decompressFrames"):                                     # absent from older development builds
+            L.ZSTDB200_decompressFrames.restype = _sz
+            L.ZSTDB200_decompressFrames.argtypes = [_vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp]
+            L.ZSTDB200_decompressFramesAsync.restype = _sz
+            L.ZSTDB200_decompressFramesAsync.argtypes = [_vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp]
         L.ZSTDB200_getLastDStats.restype = None
         L.ZSTDB200_getLastDStats.argtypes = [_vp, ctypes.POINTER(DStats)]
     if hasattr(L, "ZSTD_createDDict"):                                                  # absent from older development builds
@@ -569,6 +574,35 @@ class ZSTD_DCtx:
         torch.cuda.current_stream().cuda_stream; 0 = the legacy default stream).  Returns once the work is enqueued; the
         decompressed size, or an error code, lands in the 8 bytes at d_result in stream order (see result_error)."""
         _check(lib().ZSTDB200_decompressDeviceAsync(self._h, d_dst, dst_capacity, d_src, src_size, d_result, stream))
+
+    def decompress_frames(self, d_dst: int, dst_capacity: int, dst_offsets: Sequence[int], dst_capacities: Sequence[int],
+                          d_src: int, src_size: int, src_offsets: Sequence[int], src_sizes: Sequence[int], stream: int = 0):
+        """ZSTDB200_decompressFrames: entry i = d_src[src_offsets[i], + src_sizes[i]) decoded into its own slot
+        d_dst[dst_offsets[i], + dst_capacities[i]) (device pointers as ints).  Returns (result, [result per entry]): the sum
+        of the sizes, or the error code of the lowest-index entry that failed, and each entry's size or error code (see
+        result_error).  Raises ZstdError when the call is refused before any entry is decoded."""
+        n = len(src_sizes)
+        if not (len(src_offsets) == len(dst_offsets) == len(dst_capacities) == n):
+            raise ValueError("src_offsets, src_sizes, dst_offsets and dst_capacities differ in length")
+        so, ss, do, dc = ((_sz * n)(*a) for a in (src_offsets, src_sizes, dst_offsets, dst_capacities))
+        sizes = (_sz * n)()
+        L = lib()
+        r = L.ZSTDB200_decompressFrames(self._h, d_dst, dst_capacity, do, dc, d_src, src_size, so, ss, n, sizes, stream)
+        if L.ZSTD_isError(r) and not any(L.ZSTD_isError(v) for v in sizes):
+            _check(r)                                       # refused: no entry holds the error
+        return r, list(sizes)
+
+    def decompress_frames_async(self, d_dst: int, dst_capacity: int, dst_offsets: Sequence[int], dst_capacities: Sequence[int],
+                                d_src: int, src_size: int, src_offsets: Sequence[int], src_sizes: Sequence[int], d_result: int,
+                                d_d_sizes: int = 0, stream: int = 0) -> None:
+        """ZSTDB200_decompressFramesAsync: decompress_frames enqueued on `stream`; its result lands in the 8 bytes at d_result
+        and (d_d_sizes, 0 = none) each entry's result in one u64 per entry, in stream order."""
+        n = len(src_sizes)
+        if not (len(src_offsets) == len(dst_offsets) == len(dst_capacities) == n):
+            raise ValueError("src_offsets, src_sizes, dst_offsets and dst_capacities differ in length")
+        so, ss, do, dc = ((_sz * n)(*a) for a in (src_offsets, src_sizes, dst_offsets, dst_capacities))
+        _check(lib().ZSTDB200_decompressFramesAsync(self._h, d_dst, dst_capacity, do, dc, d_src, src_size, so, ss, n,
+                                                    d_d_sizes or None, d_result, stream))
 
     def stats(self) -> DStats:
         s = DStats()

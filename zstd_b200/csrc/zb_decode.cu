@@ -68,6 +68,19 @@ typedef struct {
     u64 frameOff;          /* first output byte of its frame (D3) */
 } ZbdBlockOut;
 
+/* Batch calls (ZSTDB200_decompressFrames): entry i's ranges as the caller gave them, uploaded ... */
+typedef struct { u64 srcOff, srcSize, dstOff, dstCap; } ZbdSpan;
+/* ... and what the kernels find out about it.  Entries that failed in the walk or lie past the workspace own no block and no
+ * frame; the others own blocks [block, block + nb) and frames [frame, frame + nf) of the call's arrays. */
+typedef struct {
+    u64 lit, seq;          /* count pass: literal bytes and sequences the walk counts; scan: the entry's first of each in the workspace */
+    u64 out, size;         /* D3: the offset of its output in the back-to-back sum, and its size */
+    u32 nb, nf;            /* blocks and frames */
+    u32 block, frame;      /* scan: its first block and frame */
+    u32 status;            /* 0 or the entry's error code: the first stage that fails it writes it, later stages skip it */
+    u32 pad;
+} ZbdEntry;
+
 /* d_res, the call's results in device memory.  [0, 5): the walk's error, blocks, frames, literal bytes, sequences.  A
  * stream-ordered call also uses [5, 7): the blocks and frames the kernels run (0 when the walk failed or the workspace holds
  * fewer), [10, 12): D3's error and output size, [12, 15): the frames of each D5 width.  [9]: D4 / D5's error (u32). */
@@ -118,6 +131,129 @@ zbd_walk_kernel(const u8* __restrict__ src, u64 size, ZbdBlock* blocks, u32 capB
         for (u64 a = lo + 128u * t; a < end; a += 128u * nt) asm volatile("prefetch.global.L1 [%0];" :: "l"(src + a));
         done = end;
     }
+}
+
+/* ------------------------------------------------------------------------------------------------ D0 for batch calls
+ * The entries' header chains are independent of each other, so one thread walks each entry: a count pass, a scan that gives
+ * every entry its place in the call's arrays, and a fill pass that walks again and writes the descriptors there, shifted
+ * into the call's coordinates.  zbd_walk is the same function as everywhere else. */
+#define ZBD_ENTRY_THREADS 128
+#define ZBD_ENTRY_SCAN    1024        /* the one CTA of the entry scan and of the verdict */
+__global__ void __launch_bounds__(ZBD_ENTRY_THREADS)
+zbd_entries_count_kernel(const u8* __restrict__ src, const ZbdSpan* __restrict__ spans, ZbdEntry* __restrict__ entries, u32 nbEntries,
+                         u32 dictEntropy, u32 dictID)
+{
+    u32 const e = blockIdx.x * ZBD_ENTRY_THREADS + threadIdx.x;
+    if (e >= nbEntries) return;
+    ZbdSpan const s = spans[e];
+    u32 nb = 0, nf = 0; u64 lit = 0, seq = 0;
+    u32 const err = zbd_walk(src + s.srcOff, s.srcSize, NULL, 0, NULL, 0, &nb, &nf, &lit, &seq, dictEntropy != 0u, dictID);
+    ZbdEntry E; memset(&E, 0, sizeof(E));
+    E.status = err;
+    if (!err) { E.nb = nb; E.nf = nf; E.lit = lit; E.seq = seq; }
+    entries[e] = E;
+}
+
+/* One CTA: the entries' places in the block, frame, literal and sequence arrays, given out in entry order.  An entry's share
+ * of the literal and sequence areas is capped at what its slot allows (dstCap + 16 bytes per block, dstCap / 3); a block
+ * behind the cap can only belong to an entry that fails, and the fill pass sends it to the area behind the workspace that
+ * nothing reads, as the single-input path does.  An entry whose blocks or frames do not fit in what the entries in front of
+ * it left of capB / capF gets workSpace_tooSmall and takes nothing, so the entries behind it keep their room.  A chunk of
+ * entries that fits whole takes its places from a parallel prefix sum; one that does not is admitted entry by entry by one
+ * thread, from the counts in shared memory.  res[0 .. 5) and res[ZBD_RES_RUN ..] as the walk kernel leaves them: the
+ * blocks, frames, literal bytes and sequences of the entries that fit. */
+#define ZBD_REFUSED (~0ull)
+__global__ void __launch_bounds__(ZBD_ENTRY_SCAN)
+zbd_entries_scan_kernel(const ZbdSpan* __restrict__ spans, ZbdEntry* __restrict__ entries, u32 nbEntries, u32 capB, u32 capF, u64* __restrict__ res)
+{
+    __shared__ u64 warpSum[4][ZBD_ENTRY_SCAN / 32];
+    __shared__ u64 carry[4];
+    __shared__ u64 chunk[4][ZBD_ENTRY_SCAN];                         /* a chunk admitted one by one: counts in, first places out */
+    u32 const tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    if (tid < 4u) carry[tid] = 0;
+    __syncthreads();
+    for (u32 e0 = 0; e0 < nbEntries; e0 += ZBD_ENTRY_SCAN) {
+        u32 const e = e0 + tid, n = nbEntries - e0 < ZBD_ENTRY_SCAN ? nbEntries - e0 : ZBD_ENTRY_SCAN;
+        u64 v[4] = { 0, 0, 0, 0 };
+        if (e < nbEntries) {
+            ZbdEntry const E = entries[e];
+            u64 const cap = spans[e].dstCap, litMax = (cap + 16u * (u64)E.nb + 15u) & ~15ull;
+            v[0] = E.nb; v[1] = E.nf; v[2] = E.lit < litMax ? E.lit : litMax; v[3] = E.seq < cap / 3u ? E.seq : cap / 3u;
+        }
+        u64 inc[4], first[4], total[4];
+#pragma unroll
+        for (u32 k = 0; k < 4u; k++) {
+            inc[k] = v[k];
+#pragma unroll
+            for (u32 o = 1; o < 32u; o <<= 1) { u64 const x = __shfl_up_sync(ZB_FULL, inc[k], o); if (lane >= o) inc[k] += x; }
+            if (lane == 31u) warpSum[k][warp] = inc[k];
+        }
+        __syncthreads();
+#pragma unroll
+        for (u32 k = 0; k < 4u; k++) {
+            first[k] = carry[k] + inc[k] - v[k]; total[k] = carry[k];
+            for (u32 w = 0; w < ZBD_ENTRY_SCAN / 32u; w++) { if (w < warp) first[k] += warpSum[k][w]; total[k] += warpSum[k][w]; }
+        }
+        bool const whole = total[0] <= capB && total[1] <= capF;      /* the same for every thread */
+        bool admitted = true;
+        if (!whole) {
+            for (u32 k = 0; k < 4u; k++) chunk[k][tid] = v[k];
+            __syncthreads();
+            if (tid == 0) {
+                u64 c[4] = { carry[0], carry[1], carry[2], carry[3] };
+                for (u32 j = 0; j < n; j++) {
+                    u64 const nb = chunk[0][j], nf = chunk[1][j];
+                    if (nb && (c[0] + nb > capB || c[1] + nf > capF)) { chunk[0][j] = ZBD_REFUSED; continue; }
+                    for (u32 k = 0; k < 4u; k++) { u64 const x = chunk[k][j]; chunk[k][j] = c[k]; c[k] += x; }
+                }
+                for (u32 k = 0; k < 4u; k++) carry[k] = c[k];
+            }
+            __syncthreads();
+            admitted = chunk[0][tid] != ZBD_REFUSED;
+            for (u32 k = 0; k < 4u; k++) first[k] = chunk[k][tid];
+        }
+        if (e < nbEntries) {
+            ZbdEntry& E = entries[e];
+            if (!admitted) { E.status = ZB_error_workSpace_tooSmall; E.nb = 0; E.nf = 0; }
+            E.block = (u32)first[0]; E.frame = (u32)first[1]; E.lit = first[2]; E.seq = first[3];
+        }
+        __syncthreads();                                             /* everyone has read carry and chunk */
+        if (whole && tid == 0) for (u32 k = 0; k < 4u; k++) carry[k] = total[k];
+        __syncthreads();
+    }
+    if (tid == 0) {
+        res[0] = 0; res[1] = carry[0]; res[2] = carry[1]; res[3] = carry[2]; res[4] = carry[3];
+        res[ZBD_RES_RUN] = carry[0]; res[ZBD_RES_RUN + 1] = carry[1];
+    }
+}
+
+/* One thread per entry that fits: its descriptors at the places the scan gave it.  Offsets into the input, frame and block
+ * indices (the block whose tables a treeless or repeat-mode block reuses included) and literal and sequence positions move
+ * from the entry's coordinates to the call's; every frame records its entry in frameEntry. */
+__global__ void __launch_bounds__(ZBD_ENTRY_THREADS)
+zbd_entries_fill_kernel(const u8* __restrict__ src, const ZbdSpan* __restrict__ spans, const ZbdEntry* __restrict__ entries, u32 nbEntries,
+                        ZbdBlock* __restrict__ blocks, ZbdFrame* __restrict__ frames, u32* __restrict__ frameEntry, u32 dictEntropy, u32 dictID,
+                        u64 litCap, u64 seqCap)
+{
+    u32 const e = blockIdx.x * ZBD_ENTRY_THREADS + threadIdx.x;
+    if (e >= nbEntries) return;
+    ZbdEntry const E = entries[e];
+    if (E.status || E.nb == 0) return;
+    ZbdSpan const s = spans[e];
+    ZbdBlock* const B = blocks + E.block;
+    ZbdFrame* const F = frames + E.frame;
+    u32 nb = 0, nf = 0; u64 lit = 0, seq = 0;
+    zbd_walk(src + s.srcOff, s.srcSize, B, E.nb, F, E.nf, &nb, &nf, &lit, &seq, dictEntropy != 0u, dictID);   /* the count pass's walk: it succeeds */
+    u64 const litMax = s.dstCap + 16u * (u64)E.nb, seqMax = s.dstCap / 3u;
+    for (u32 k = 0; k < E.nb; k++) {
+        ZbdBlock& b = B[k];
+        b.srcOff += s.srcOff; b.frame += E.frame;
+        if (b.hufSrc < ZBD_DICT) b.hufSrc += E.block;              /* ZBD_NONE and ZBD_DICT stay */
+        for (u32 t = 0; t < 3u; t++) if (b.fseSrc[t] < ZBD_DICT) b.fseSrc[t] += E.block;
+        b.litPos = b.litPos + b.litRegen <= litMax ? E.lit + b.litPos : litCap;
+        b.seqPos = b.seqPos + b.nbSeq <= seqMax ? E.seq + b.seqPos : seqCap;
+    }
+    for (u32 k = 0; k < E.nf; k++) { F[k].srcOff += s.srcOff; F[k].firstBlock += E.block; frameEntry[E.frame + k] = e; }
 }
 
 /* ------------------------------------------------------------------------------------------------ D1 literals */
@@ -238,11 +374,17 @@ zbd_sequences_kernel(const u8* __restrict__ src, const ZbdBlock* __restrict__ bl
  * warp per frame walks its blocks, 32 transfer functions per round.  res[0] = first error, res[1] = total output bytes.
  * Stream-ordered calls (walk: the call's d_res): the counts are the walk's, and every frame with matches goes to the list
  * of the D5 width that zbd_run would pick for it (classList + k * capF, k = 0: 1024 threads, 1: 128, 2: 32; res[2 + k]
- * frames each). */
+ * frames each).
+ * Batch calls (ENTRIES): the sums run over the entries back to back as above, then each entry is moved to its own slot.  Block
+ * errors, content sizes and the capacity are checked per entry, into the entry's status word (first error wins: an entry that
+ * failed in the walk owns no block); only frames of entries still alive are listed for D5.  res[0] = 0 and res[1] =
+ * dstCapacity (the whole buffer), the bound of the tile index the clear kernel resets and D5's bound on a match's end. */
 #define SCAN_THREADS 1024
+template <bool ENTRIES>
 __global__ void __launch_bounds__(SCAN_THREADS)
 zbd_scan_kernel(const ZbdBlock* __restrict__ blocks, u32 nbBlocks, const ZbdFrame* __restrict__ frames, u32 nbFrames, ZbdBlockOut* __restrict__ bout,
-                u64 dstCapacity, u64* __restrict__ res, ZbdDictInfo di, const u64* __restrict__ walk, u32* __restrict__ classList, u32 capF)
+                u64 dstCapacity, u64* __restrict__ res, ZbdDictInfo di, const u64* __restrict__ walk, u32* __restrict__ classList, u32 capF,
+                const ZbdSpan* __restrict__ spans, ZbdEntry* __restrict__ entries, const u32* __restrict__ frameEntry, u32 nbEntries)
 {
     __shared__ u64 warpSum[SCAN_THREADS / 32];
     __shared__ u64 carry;
@@ -255,7 +397,10 @@ zbd_scan_kernel(const ZbdBlock* __restrict__ blocks, u32 nbBlocks, const ZbdFram
     for (u32 b0 = 0; b0 < nbBlocks; b0 += SCAN_THREADS) {
         u32 const i = b0 + tid;
         u64 v = 0;
-        if (i < nbBlocks) { v = bout[i].regen; if (bout[i].err) atomicMax(&firstErr, bout[i].err); }
+        if (i < nbBlocks) {
+            v = bout[i].regen;
+            if (bout[i].err) atomicMax(ENTRIES ? &entries[frameEntry[blocks[i].frame]].status : &firstErr, bout[i].err);
+        }
         u64 inc = v;
 #pragma unroll
         for (u32 o = 1; o < 32u; o <<= 1) { u64 const x = __shfl_up_sync(ZB_FULL, inc, o); if (lane >= o) inc += x; }
@@ -271,6 +416,16 @@ zbd_scan_kernel(const ZbdBlock* __restrict__ blocks, u32 nbBlocks, const ZbdFram
     u64 const total = carry;
     u32 const blockErr = firstErr;                                   /* a block that failed has no size: no content-size check over it hides its code */
     __syncthreads();
+    /* a frame with matches goes to the list of the D5 width that zbd_run would pick for it */
+    auto classify = [&](u32 f, const ZbdFrame& fr) {
+        if (!fr.nbBlocks) return;
+        ZbdBlock const& bl = blocks[fr.firstBlock + fr.nbBlocks - 1u];
+        u64 const matches = bl.seqPos + (bl.type == ZB_BT_COMPRESSED ? bl.nbSeq : 0u) - blocks[fr.firstBlock].seqPos;
+        if (matches) {
+            u32 const k = matches >= 8192u ? 0u : (matches >= 256u ? 1u : 2u);
+            classList[(size_t)k * capF + atomicAdd(&classCount[k], 1u)] = f;
+        }
+    };
     /* per frame: content size, start offset, repcode histories */
     for (u32 f = warp; f < nbFrames; f += SCAN_THREADS / 32u) {
         ZbdFrame const fr = frames[f];
@@ -291,20 +446,36 @@ zbd_scan_kernel(const ZbdBlock* __restrict__ blocks, u32 nbBlocks, const ZbdFram
             }
             if (k < fr.nbBlocks) { ZbdBlockOut& o = bout[fr.firstBlock + k]; o.start = mine; o.frameOff = fOff; }
         }
-        if (lane == 0 && !blockErr && fr.contentSize != ZBD_CONTENTSIZE_UNKNOWN) {
+        u32* const status = ENTRIES ? &entries[frameEntry[f]].status : &firstErr;
+        if (lane == 0 && !(ENTRIES ? *(volatile u32*)status : blockErr) && fr.contentSize != ZBD_CONTENTSIZE_UNKNOWN) {
             u64 const end = (fr.firstBlock + fr.nbBlocks < nbBlocks) ? bout[fr.firstBlock + fr.nbBlocks].dstOff : total;
-            if (end - fOff != fr.contentSize) atomicMax(&firstErr, ZBD_CORRUPT);
+            if (end - fOff != fr.contentSize) atomicMax(status, ZBD_CORRUPT);
         }
-        if (walk && lane == 0 && fr.nbBlocks) {
-            ZbdBlock const& bl = blocks[fr.firstBlock + fr.nbBlocks - 1u];
-            u64 const matches = bl.seqPos + (bl.type == ZB_BT_COMPRESSED ? bl.nbSeq : 0u) - blocks[fr.firstBlock].seqPos;
-            if (matches) {
-                u32 const k = matches >= 8192u ? 0u : (matches >= 256u ? 1u : 2u);
-                classList[(size_t)k * capF + atomicAdd(&classCount[k], 1u)] = f;
-            }
-        }
+        if (!ENTRIES && walk && lane == 0) classify(f, fr);
     }
     __syncthreads();
+    if (ENTRIES) {
+        for (u32 e = tid; e < nbEntries; e += SCAN_THREADS) {
+            ZbdEntry& E = entries[e];
+            E.out = 0; E.size = 0;
+            if (E.status || E.nb == 0) continue;
+            u64 const start = bout[E.block].dstOff, end = E.block + E.nb < nbBlocks ? bout[E.block + E.nb].dstOff : total;
+            E.out = start; E.size = end - start;
+            if (end - start > spans[e].dstCap) E.status = 70u;      /* dstSize_tooSmall */
+        }
+        __syncthreads();
+        for (u32 i = tid; i < nbBlocks; i += SCAN_THREADS) {        /* into the entry's slot */
+            u32 const e = frameEntry[blocks[i].frame];
+            u64 const shift = spans[e].dstOff - entries[e].out;
+            bout[i].dstOff += shift; bout[i].frameOff += shift;
+        }
+        for (u32 f = tid; f < nbFrames; f += SCAN_THREADS) {
+            if (entries[frameEntry[f]].status == 0u) classify(f, frames[f]);
+        }
+        __syncthreads();
+        if (tid == 0) { res[0] = 0; res[1] = dstCapacity; res[2] = classCount[0]; res[3] = classCount[1]; res[4] = classCount[2]; }
+        return;
+    }
     if (tid == 0) {
         u32 e = firstErr;
         if (!e && total > dstCapacity) e = 70u;                      /* dstSize_tooSmall */
@@ -320,16 +491,21 @@ zbd_scan_kernel(const ZbdBlock* __restrict__ blocks, u32 nbBlocks, const ZbdFram
  * each other.  A match that begins in the dictionary's content gets those bytes here and continues as an ordinary match
  * behind them.  seqs[g] becomes offset | length << 28, matchPos[g] the match's first output byte, and for every 64-byte
  * tile of the output tileFirst[] the first match (in the call's match order) that ends behind the tile's first byte:
- * what D5 needs to find the matches a source range depends on. */
+ * what D5 needs to find the matches a source range depends on.
+ * Batch calls (ENTRIES): blocks of entries that have failed are skipped, an error goes to the entry's status word, and an
+ * entry's first block lowers the tile that holds the entry's first byte to its first match (the tile may begin in front of
+ * the slot, where nothing else writes it, or in the previous entry's output: any value up to that match is right for D5,
+ * which never looks below a frame's first match). */
 #define ZBD_TILE_LOG 6u
-template <bool PERSISTENT>
+template <bool PERSISTENT, bool ENTRIES>
 __global__ void __launch_bounds__(32 * ZBD_WARPS)
 zbd_place_kernel(const u8* __restrict__ src, const ZbdBlock* __restrict__ blocks, u32 nbBlocks, const u8* __restrict__ lits, u64* __restrict__ seqs,
                  u64* __restrict__ matchPos, u32* __restrict__ tileFirst, const ZbdBlockOut* __restrict__ bout, u8* __restrict__ dst,
-                 const u8* __restrict__ dictContent, u32 dictContentSize, u32* __restrict__ execErr, const u64* __restrict__ res)
+                 const u8* __restrict__ dictContent, u32 dictContentSize, u32* __restrict__ execErr, const u64* __restrict__ res,
+                 const u32* __restrict__ frameEntry, ZbdEntry* __restrict__ entries)
 {
     u32 const lane = threadIdx.x & 31u;
-    auto block = [&](u32 bi) {
+    auto block = [&](u32 bi, u32* errWord, bool entryFirst) {
     ZbdBlock const b = blocks[bi];
     ZbdBlockOut const o = bout[bi];
     u8* const out = dst + o.dstOff;
@@ -342,8 +518,9 @@ zbd_place_kernel(const u8* __restrict__ src, const ZbdBlock* __restrict__ blocks
     if (b.type != ZB_BT_COMPRESSED) {
         if (b.type == ZB_BT_RAW) { for (u32 i = lane; i < b.rawSize; i += 32u) out[i] = src[b.srcOff + i]; }
         else { u8 const v = src[b.srcOff]; for (u32 i = lane; i < b.rawSize; i += 32u) out[i] = v; }
-        if (o.dstOff == 0 && lane == 0) tileFirst[0] = gNext;
-        tiles(o.dstOff, o.dstOff + o.regen, gNext);                  /* no match ends in here: the next block's first one is the first behind these tiles */
+        if (ENTRIES && entryFirst && lane == 0) atomicMin(&tileFirst[o.dstOff >> ZBD_TILE_LOG], gNext);
+        if (!ENTRIES && o.dstOff == 0 && lane == 0) tileFirst[0] = gNext;
+        tiles(o.dstOff, o.dstOff + o.regen, gNext);                 /* no match ends in here: the next block's first one is the first behind these tiles */
         return;
     }
     const u8* const lit = lits + b.litPos;
@@ -352,7 +529,8 @@ zbd_place_kernel(const u8* __restrict__ src, const ZbdBlock* __restrict__ blocks
     ZbdRep rep = o.start;
     u64 const inFrame = o.dstOff - o.frameOff;                       /* bytes of the frame in front of this block */
     u32 op = 0, lp = 0, err = 0, failedAt = 0;
-    if (o.dstOff == 0 && lane == 0) tileFirst[0] = gFirst;
+    if (ENTRIES && entryFirst && lane == 0) atomicMin(&tileFirst[o.dstOff >> ZBD_TILE_LOG], gFirst);
+    if (!ENTRIES && o.dstOff == 0 && lane == 0) tileFirst[0] = gFirst;
     for (u32 i0 = 0; i0 < b.nbSeq; i0 += 32u) {
         u32 const n = min(32u, b.nbSeq - i0);
         u64 const q = (lane < n) ? sq[i0 + lane] : 0ull;
@@ -391,7 +569,7 @@ zbd_place_kernel(const u8* __restrict__ src, const ZbdBlock* __restrict__ blocks
     }
     if (err) {                                                       /* the call fails; D5 must not follow what is left of this block */
         for (u32 i = failedAt - (failedAt % 32u) + lane; i < b.nbSeq; i += 32u) { sq[i] = 1ull; mp[i] = o.dstOff; }
-        if (lane == 0) atomicMax(execErr, err);
+        if (lane == 0) atomicMax(errWord, err);
         tiles(o.dstOff, o.dstOff + o.regen, gNext);
         return;
     }
@@ -399,9 +577,13 @@ zbd_place_kernel(const u8* __restrict__ src, const ZbdBlock* __restrict__ blocks
     for (u32 k = lane; k < rest; k += 32u) out[op + k] = lit[lp + k];
     tiles(o.dstOff + op, o.dstOff + o.regen, gNext);                 /* behind the block's last match */
     };
-    if (!PERSISTENT) { u32 const bi = blockIdx.x * ZBD_WARPS + (threadIdx.x >> 5); if (bi < nbBlocks) block(bi); return; }
+    if (!PERSISTENT) { u32 const bi = blockIdx.x * ZBD_WARPS + (threadIdx.x >> 5); if (bi < nbBlocks) block(bi, execErr, false); return; }
     u32 const n = zbd_liveBlocks(res, nbBlocks, true);
-    for (u32 bi = blockIdx.x * ZBD_WARPS + (threadIdx.x >> 5); bi < n; bi += gridDim.x * ZBD_WARPS) block(bi);
+    for (u32 bi = blockIdx.x * ZBD_WARPS + (threadIdx.x >> 5); bi < n; bi += gridDim.x * ZBD_WARPS) {
+        if (!ENTRIES) { block(bi, execErr, false); continue; }
+        ZbdEntry* const E = entries + frameEntry[blocks[bi].frame];
+        if (E->status == 0u) block(bi, &E->status, bi == E->block);
+    }
 }
 
 /* Stream-ordered calls: what zbd_run clears with two memsets once it knows the output size, sized here from D3's total and
@@ -580,18 +762,27 @@ zbd_matches_kernel(const ZbdBlock* __restrict__ blocks, const ZbdFrame* __restri
     zbd_matchesFrame<THREADS>(blockIdx.x, &sTicket, blocks, frames, seqs, matchPos, tileFirst, totalOut, dst, done, execErr);
 }
 /* stream-ordered calls: a persistent grid over the frames D3 listed for this width (list, res[ZBD_RES_CLASS + cls] of them),
- * the ticket reset between frames; nothing when the call failed */
-template <int THREADS>
+ * the ticket reset between frames; nothing when the call failed.  Batch calls (ENTRIES): a frame whose entry failed in D4 is
+ * skipped, and an error goes to the entry's status word. */
+template <int THREADS, bool ENTRIES>
 __global__ void __launch_bounds__(THREADS)
 zbd_matches_list_kernel(const ZbdBlock* __restrict__ blocks, const ZbdFrame* __restrict__ frames, const u64* __restrict__ seqs, const u64* __restrict__ matchPos,
                         const u32* __restrict__ tileFirst, u8* __restrict__ dst, u8* done, u32* __restrict__ execErr,
-                        const u32* __restrict__ list, const u64* __restrict__ res, u32 cls)
+                        const u32* __restrict__ list, const u64* __restrict__ res, u32 cls, const u32* __restrict__ frameEntry, ZbdEntry* __restrict__ entries)
 {
     __shared__ u32 sTicket;
+    __shared__ u32 sFailed;
     if (res[ZBD_RES_SCAN] || !res[ZBD_RES_RUN]) return;
     u64 const n = res[ZBD_RES_CLASS + cls], totalOut = res[ZBD_RES_SCAN + 1];
     for (u64 k = blockIdx.x; k < n; k += gridDim.x) {
-        zbd_matchesFrame<THREADS>(list[k], &sTicket, blocks, frames, seqs, matchPos, tileFirst, totalOut, dst, done, execErr);
+        u32 const f = list[k];
+        if (!ENTRIES) zbd_matchesFrame<THREADS>(f, &sTicket, blocks, frames, seqs, matchPos, tileFirst, totalOut, dst, done, execErr);
+        else {
+            u32* const status = &entries[frameEntry[f]].status;
+            if (threadIdx.x == 0) sFailed = *(volatile u32*)status;   /* one reading for the whole CTA: the frame loop below synchronises */
+            __syncthreads();
+            if (!sFailed) zbd_matchesFrame<THREADS>(f, &sTicket, blocks, frames, seqs, matchPos, tileFirst, totalOut, dst, done, status);
+        }
         __syncthreads();                                             /* every warp is done with the frame before the ticket is reset */
     }
 }
@@ -644,6 +835,12 @@ struct ZSTD_DCtx_s {
     ZbOrder order;
     ZbDevBuf<u32> d_class;
     u32 grid[7];
+    /* batch calls (ZSTDB200_decompressFrames[Async]): the entries' spans are staged in a ring of page-locked slots, as the
+     * compressor stages its descriptors (slot s is free again once evStage[s], recorded behind its upload, has completed);
+     * d_verdict holds a synchronous call's result and sizes for its one read-back into h_verdict */
+    ZbDevBuf<ZbdSpan> d_spans; ZbDevBuf<ZbdEntry> d_entries; ZbDevBuf<u32> d_frameEntry;   /* the entry of every frame */
+    ZbHostBuf<ZbdSpan> stage[ZSTDB200_ASYNC_SLOTS]; bool stageBusy[ZSTDB200_ASYNC_SLOTS]; u32 stageNext; ZbEvents evStage;
+    ZbDevBuf<unsigned long long> d_verdict; ZbHostBuf<unsigned long long> h_verdict;
 };
 
 /* one decompression call, as an entry point describes it */
@@ -686,11 +883,11 @@ static size_t zbd_ctxInit(ZSTD_DCtx* d)
         int per[7] = { 0 };
         CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per[0], zbd_literals_kernel<true>, 32 * ZBD_WARPS, 0));
         CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per[1], zbd_sequences_kernel<true>, 32 * ZBD_WARPS, 0));
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per[2], zbd_place_kernel<true>, 32 * ZBD_WARPS, 0));
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per[2], zbd_place_kernel<true, false>, 32 * ZBD_WARPS, 0));
         CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per[3], zbd_clear_kernel, 256, 0));
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per[4], zbd_matches_list_kernel<1024>, 1024, 0));
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per[5], zbd_matches_list_kernel<128>, 128, 0));
-        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per[6], zbd_matches_list_kernel<32>, 32, 0));
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per[4], zbd_matches_list_kernel<1024, false>, 1024, 0));
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per[5], zbd_matches_list_kernel<128, false>, 128, 0));
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per[6], zbd_matches_list_kernel<32, false>, 32, 0));
         for (int k = 0; k < 7; k++) d->grid[k] = (u32)(per[k] > 0 ? per[k] : 1) * (u32)(sms > 0 ? sms : 1);
         d->stream = std::move(st); d->ev = std::move(ev); d->order = std::move(order);
         d->device = dev;
@@ -724,7 +921,7 @@ static size_t zbd_run(ZSTD_DCtx* d, u8* d_dst, size_t dstCapacity, const u8* d_s
     CK(cudaEventRecord(d->ev[2], st));
     zbd_sequences_kernel<false><<<grid, 32 * ZBD_WARPS, 0, st>>>(d_src, d->d_blocks, nb, d->d_seqs, d->d_bout, d_dict, di, NULL, 0);
     CK(cudaEventRecord(d->ev[3], st));
-    zbd_scan_kernel<<<1, SCAN_THREADS, 0, st>>>(d->d_blocks, nb, d->d_frames, nf, d->d_bout, (u64)dstCapacity, d->d_res, di, NULL, NULL, 0);
+    zbd_scan_kernel<false><<<1, SCAN_THREADS, 0, st>>>(d->d_blocks, nb, d->d_frames, nf, d->d_bout, (u64)dstCapacity, d->d_res, di, NULL, NULL, 0, NULL, NULL, NULL, 0);
     CK(cudaMemcpyAsync(d->h_res, d->d_res, 2 * sizeof(u64), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));                                  /* nothing is written to dst before the sizes are known to fit */
     if (d->h_res[0]) return ZB_ERR((u32)d->h_res[0]);
@@ -736,8 +933,8 @@ static size_t zbd_run(ZSTD_DCtx* d, u8* d_dst, size_t dstCapacity, const u8* d_s
     TRY(zbd_reserve(d->d_done, (size_t)seqCount + 4));
     CK(cudaMemsetAsync(d->d_tileFirst, 0xFF, ((total >> ZBD_TILE_LOG) + 4) * sizeof(u32), st));
     CK(cudaMemsetAsync(d->d_done, 0, (size_t)seqCount + 4, st));
-    zbd_place_kernel<false><<<grid, 32 * ZBD_WARPS, 0, st>>>(d_src, d->d_blocks, nb, d->d_lits, d->d_seqs, d->d_matchPos, d->d_tileFirst, d->d_bout, d_dst,
-                                                      d_dictContent, dictContent, d->d_execErr, NULL);
+    zbd_place_kernel<false, false><<<grid, 32 * ZBD_WARPS, 0, st>>>(d_src, d->d_blocks, nb, d->d_lits, d->d_seqs, d->d_matchPos, d->d_tileFirst, d->d_bout, d_dst,
+                                                             d_dictContent, dictContent, d->d_execErr, NULL, NULL, NULL);
     CK(cudaEventRecord(d->ev[6], st));
     if (seqCount) {                                                  /* threads per frame by the matches a frame holds */
         u64 const perFrame = seqCount / (nf ? nf : 1u);
@@ -1086,17 +1283,17 @@ static size_t zbd_decompressAsync(ZSTD_DCtx* d, void* dst, size_t dstCapacity, c
     zbd_walk_kernel<<<1, ZBD_WALK_THREADS, 0, st>>>(in, (u64)srcSize, d->d_blocks, capB, d->d_frames, capF, res, di.entropy, di.dictID);
     zbd_literals_kernel<true><<<grid(0, blockGrid), 32 * ZBD_WARPS, 0, st>>>(in, d->d_blocks, capB, d->d_lits, d->d_bout, d_dict, di, res, litCap);
     zbd_sequences_kernel<true><<<grid(1, blockGrid), 32 * ZBD_WARPS, 0, st>>>(in, d->d_blocks, capB, d->d_seqs, d->d_bout, d_dict, di, res, seqCap);
-    zbd_scan_kernel<<<1, SCAN_THREADS, 0, st>>>(d->d_blocks, capB, d->d_frames, capF, d->d_bout, (u64)dstCapacity, res + ZBD_RES_SCAN, di, res,
-                                                d->d_class, capF);
+    zbd_scan_kernel<false><<<1, SCAN_THREADS, 0, st>>>(d->d_blocks, capB, d->d_frames, capF, d->d_bout, (u64)dstCapacity, res + ZBD_RES_SCAN, di, res,
+                                                       d->d_class, capF, NULL, NULL, NULL, 0);
     zbd_clear_kernel<<<grid(3, (u32)(seqCap / 256u) + 1u), 256, 0, st>>>(res, d->d_tileFirst, d->d_done);
-    zbd_place_kernel<true><<<grid(2, blockGrid), 32 * ZBD_WARPS, 0, st>>>(in, d->d_blocks, capB, d->d_lits, d->d_seqs, d->d_matchPos, d->d_tileFirst, d->d_bout,
-                                                                    (u8*)dst, d_dictContent, dictContent, d->d_execErr, res);
-    zbd_matches_list_kernel<1024><<<grid(4, capF), 1024, 0, st>>>(d->d_blocks, d->d_frames, d->d_seqs, d->d_matchPos, d->d_tileFirst, (u8*)dst, d->d_done,
-                                                            d->d_execErr, d->d_class, res, 0);
-    zbd_matches_list_kernel<128><<<grid(5, capF), 128, 0, st>>>(d->d_blocks, d->d_frames, d->d_seqs, d->d_matchPos, d->d_tileFirst, (u8*)dst, d->d_done,
-                                                          d->d_execErr, d->d_class + capF, res, 1);
-    zbd_matches_list_kernel<32><<<grid(6, capF), 32, 0, st>>>(d->d_blocks, d->d_frames, d->d_seqs, d->d_matchPos, d->d_tileFirst, (u8*)dst, d->d_done,
-                                                        d->d_execErr, d->d_class + 2 * (size_t)capF, res, 2);
+    zbd_place_kernel<true, false><<<grid(2, blockGrid), 32 * ZBD_WARPS, 0, st>>>(in, d->d_blocks, capB, d->d_lits, d->d_seqs, d->d_matchPos, d->d_tileFirst, d->d_bout,
+                                                                           (u8*)dst, d_dictContent, dictContent, d->d_execErr, res, NULL, NULL);
+    zbd_matches_list_kernel<1024, false><<<grid(4, capF), 1024, 0, st>>>(d->d_blocks, d->d_frames, d->d_seqs, d->d_matchPos, d->d_tileFirst, (u8*)dst, d->d_done,
+                                                            d->d_execErr, d->d_class, res, 0, NULL, NULL);
+    zbd_matches_list_kernel<128, false><<<grid(5, capF), 128, 0, st>>>(d->d_blocks, d->d_frames, d->d_seqs, d->d_matchPos, d->d_tileFirst, (u8*)dst, d->d_done,
+                                                          d->d_execErr, d->d_class + capF, res, 1, NULL, NULL);
+    zbd_matches_list_kernel<32, false><<<grid(6, capF), 32, 0, st>>>(d->d_blocks, d->d_frames, d->d_seqs, d->d_matchPos, d->d_tileFirst, (u8*)dst, d->d_done,
+                                                        d->d_execErr, d->d_class + 2 * (size_t)capF, res, 2, NULL, NULL);
     zbd_result_kernel<<<1, 1, 0, st>>>(res, capB, capF, result);
     CK(cudaGetLastError());
     TRY(call.leave(st));
@@ -1108,6 +1305,152 @@ extern "C" size_t ZSTDB200_decompressDeviceAsync(ZSTD_DCtx* d, void* d_dst, size
                                                  unsigned long long* d_result, void* stream)
 {
     return zbd_decompressAsync(d, d_dst, dstCapacity, d_src, srcSize, d_result, (cudaStream_t)stream);
+}
+
+/* ------------------------------------------------------------------------------------------------ batch calls
+ * ZSTDB200_decompressFrames[Async] (include/zstd_b200.h states the contract): the stream-ordered pipeline above with D0 walked
+ * entry by entry and D3 .. D5 in their per-entry mode, then this verdict.  One CTA: every entry's size or error code to
+ * sizes (NULL: none), and to *result the sum of the sizes, or the error code of the lowest-index entry that failed. */
+__global__ void __launch_bounds__(ZBD_ENTRY_SCAN)
+zbd_entries_result_kernel(const ZbdEntry* __restrict__ entries, u32 nbEntries, unsigned long long* sizes, unsigned long long* result)
+{
+    __shared__ u32 firstBad;
+    __shared__ unsigned long long total;
+    if (threadIdx.x == 0) { firstBad = 0xFFFFFFFFu; total = 0; }
+    __syncthreads();
+    u64 sum = 0;
+    for (u32 e = threadIdx.x; e < nbEntries; e += ZBD_ENTRY_SCAN) {
+        ZbdEntry const& E = entries[e];
+        if (E.status) atomicMin(&firstBad, e); else sum += E.size;
+        if (sizes) sizes[e] = E.status ? (unsigned long long)ZB_ERR(E.status) : E.size;
+    }
+#pragma unroll
+    for (u32 o = 16; o > 0; o >>= 1) sum += __shfl_down_sync(ZB_FULL, sum, o);
+    if ((threadIdx.x & 31u) == 0) atomicAdd(&total, (unsigned long long)sum);
+    __syncthreads();
+    if (threadIdx.x == 0) *result = firstBad != 0xFFFFFFFFu ? (unsigned long long)ZB_ERR(entries[firstBad].status) : total;
+}
+
+/* ownVerdict: the result and sizes go to the context's d_verdict (the synchronous call) instead of result / sizes */
+static size_t zbd_decompressFrames(ZSTD_DCtx* d, u8* dst, size_t dstCapacity, const size_t* dstOffsets, const size_t* dstCapacities,
+                                   const u8* src, size_t srcSize, const size_t* srcOffsets, const size_t* srcSizes, size_t n,
+                                   unsigned long long* sizes, unsigned long long* result, bool ownVerdict, cudaStream_t st)
+{
+    if (!d || (!result && !ownVerdict)) return ZB_ERR(ZB_error_GENERIC);
+    if (n && (!dstOffsets || !dstCapacities || !srcOffsets || !srcSizes)) return ZB_ERR(ZB_error_GENERIC);
+    if (d->dictUses == ZBD_DICT_USE_ONCE) { zbd_clearDict(d); return ZB_ERR(ZB_error_parameter_unsupported); }   /* a prefix is forgotten */
+    u64 sumCap = 0;
+    for (size_t i = 0; i < n; i++) {            /* source ranges inside the input; slots inside the output, ascending and disjoint */
+        if (srcOffsets[i] > srcSize || srcSizes[i] > srcSize - srcOffsets[i]) return ZB_ERR(ZB_error_parameter_outOfBound);
+        if (dstOffsets[i] > dstCapacity || dstCapacities[i] > dstCapacity - dstOffsets[i]) return ZB_ERR(ZB_error_parameter_outOfBound);
+        if (i + 1 < n && dstOffsets[i] + dstCapacities[i] > dstOffsets[i + 1]) return ZB_ERR(ZB_error_parameter_outOfBound);
+        sumCap += dstCapacities[i];
+    }
+    ZbDeviceGuard guard;
+    ZbOrder::Call call(d->order);
+    TRY(call.begin(d->device, st));
+    TRY(zbd_ctxInit(d));
+    memset(&d->stats, 0, sizeof(d->stats));
+    const ZSTD_DDict* dd = zbd_getDDict(d);
+    if (dd && dd->size == 0) dd = NULL;                               /* an empty dictionary is none */
+    if (dd && call.capturing && !zbd_dictResident(dd, d->device)) return ZB_ERR(ZB_error_stage_wrong);
+    u64 const cap = zbd_asyncBlocks(srcSize, dstCapacity) + (u64)n;
+    if (cap > 0x7FFFFFFFull) return ZB_ERR(ZB_error_memory_allocation);
+    u32 const capB = (u32)cap, capF = (u32)cap, nbEntries = (u32)n;
+    u64 const litCap = sumCap + 32u * cap, seqCap = sumCap / 3u;      /* the entries' shares (zbd_entries_scan_kernel) fit */
+    size_t const slots = n ? n : 1;
+    TRY(call.size([&]() -> size_t {
+        TRY(zbd_reserve(d->d_blocks, capB));
+        TRY(d->d_bout.ensure((size_t)capB + 1, capB / 8 + 64));
+        TRY(zbd_reserve(d->d_frames, capF)); TRY(zbd_reserve(d->d_frameEntry, capF));
+        TRY(zbd_reserve(d->d_class, 3 * (size_t)capF));
+        TRY(zbd_reserve(d->d_lits, litCap + ZB_BLOCK_MAX + 32));
+        TRY(zbd_reserve(d->d_seqs, seqCap + ZBD_NBSEQ_MAX + 1));
+        TRY(zbd_reserve(d->d_matchPos, seqCap + 1));
+        TRY(zbd_reserve(d->d_done, seqCap + 4));
+        TRY(zbd_reserve(d->d_tileFirst, (dstCapacity >> ZBD_TILE_LOG) + 4));
+        TRY(zbd_reserve(d->d_spans, slots)); TRY(zbd_reserve(d->d_entries, slots));
+        TRY(d->evStage.ensure(ZSTDB200_ASYNC_SLOTS, false));
+        for (u32 s = 0; s < ZSTDB200_ASYNC_SLOTS; s++)               /* every slot, so that any can serve a capture */
+            if (d->stage[s].cap < slots) { TRY(d->stage[s].ensure(slots, slots / 8 + 64)); d->stageBusy[s] = false; }
+        if (ownVerdict) { TRY(zbd_reserve(d->d_verdict, slots + 1)); TRY(d->h_verdict.ensure(slots + 1, slots / 8 + 64)); }
+        return 0;
+    }));
+    if (dd) TRY(zbd_residentDict(dd, d->device, d->stream));           /* no copy once resident */
+    ZbdDictInfo const di = zbd_dictInfo(dd);
+    const u8* const d_dict = dd ? (const u8*)dd->d_dict : (const u8*)NULL;
+    u32 const dictContent = dd ? (u32)(dd->size - di.contentOff) : 0u;
+    const u8* const d_dictContent = dd ? d_dict + di.contentOff : (const u8*)NULL;
+    if (ownVerdict) { result = d->d_verdict; sizes = sizes ? d->d_verdict + 1 : NULL; }
+    /* the spans, into the next slot of the ring; under capture the wait needs the relaxed mode (the event was recorded outside the graph) */
+    u32 const slot = d->stageNext;
+    d->stageNext = (slot + 1u) % ZSTDB200_ASYNC_SLOTS;
+    if (d->stageBusy[slot]) {
+        cudaStreamCaptureMode m = cudaStreamCaptureModeRelaxed;
+        CK(cudaThreadExchangeStreamCaptureMode(&m));
+        cudaError_t const e = cudaEventSynchronize(d->evStage[slot]);
+        cudaThreadExchangeStreamCaptureMode(&m);
+        CK(e);
+        d->stageBusy[slot] = false;
+    }
+    ZbdSpan* const h = d->stage[slot];
+    for (size_t i = 0; i < n; i++) { h[i].srcOff = srcOffsets[i]; h[i].srcSize = srcSizes[i]; h[i].dstOff = dstOffsets[i]; h[i].dstCap = dstCapacities[i]; }
+    TRY(call.enter(st));
+    if (n) CK(cudaMemcpyAsync(d->d_spans, h, n * sizeof(ZbdSpan), cudaMemcpyHostToDevice, st));
+    if (!call.capturing) { CK(cudaEventRecord(d->evStage[slot], st)); d->stageBusy[slot] = true; }
+    u64* const res = d->d_res;
+    u32 const blockGrid = (capB + ZBD_WARPS - 1u) / ZBD_WARPS, entryGrid = (nbEntries + ZBD_ENTRY_THREADS - 1u) / ZBD_ENTRY_THREADS + (n == 0);
+    auto grid = [&](int k, u32 most) { return d->grid[k] < most ? d->grid[k] : most; };
+    zbd_entries_count_kernel<<<entryGrid, ZBD_ENTRY_THREADS, 0, st>>>(src, d->d_spans, d->d_entries, nbEntries, di.entropy, di.dictID);
+    zbd_entries_scan_kernel<<<1, ZBD_ENTRY_SCAN, 0, st>>>(d->d_spans, d->d_entries, nbEntries, capB, capF, res);
+    zbd_entries_fill_kernel<<<entryGrid, ZBD_ENTRY_THREADS, 0, st>>>(src, d->d_spans, d->d_entries, nbEntries, d->d_blocks, d->d_frames, d->d_frameEntry,
+                                                                     di.entropy, di.dictID, litCap, seqCap);
+    zbd_literals_kernel<true><<<grid(0, blockGrid), 32 * ZBD_WARPS, 0, st>>>(src, d->d_blocks, capB, d->d_lits, d->d_bout, d_dict, di, res, litCap);
+    zbd_sequences_kernel<true><<<grid(1, blockGrid), 32 * ZBD_WARPS, 0, st>>>(src, d->d_blocks, capB, d->d_seqs, d->d_bout, d_dict, di, res, seqCap);
+    zbd_scan_kernel<true><<<1, SCAN_THREADS, 0, st>>>(d->d_blocks, capB, d->d_frames, capF, d->d_bout, (u64)dstCapacity, res + ZBD_RES_SCAN, di, res,
+                                                      d->d_class, capF, d->d_spans, d->d_entries, d->d_frameEntry, nbEntries);
+    zbd_clear_kernel<<<grid(3, (u32)(seqCap / 256u) + 1u), 256, 0, st>>>(res, d->d_tileFirst, d->d_done);
+    zbd_place_kernel<true, true><<<grid(2, blockGrid), 32 * ZBD_WARPS, 0, st>>>(src, d->d_blocks, capB, d->d_lits, d->d_seqs, d->d_matchPos, d->d_tileFirst,
+                                                                              d->d_bout, dst, d_dictContent, dictContent, d->d_execErr, res, d->d_frameEntry,
+                                                                              d->d_entries);
+    zbd_matches_list_kernel<1024, true><<<grid(4, capF), 1024, 0, st>>>(d->d_blocks, d->d_frames, d->d_seqs, d->d_matchPos, d->d_tileFirst, dst, d->d_done,
+                                                                        d->d_execErr, d->d_class, res, 0, d->d_frameEntry, d->d_entries);
+    zbd_matches_list_kernel<128, true><<<grid(5, capF), 128, 0, st>>>(d->d_blocks, d->d_frames, d->d_seqs, d->d_matchPos, d->d_tileFirst, dst, d->d_done,
+                                                                      d->d_execErr, d->d_class + capF, res, 1, d->d_frameEntry, d->d_entries);
+    zbd_matches_list_kernel<32, true><<<grid(6, capF), 32, 0, st>>>(d->d_blocks, d->d_frames, d->d_seqs, d->d_matchPos, d->d_tileFirst, dst, d->d_done,
+                                                                    d->d_execErr, d->d_class + 2 * (size_t)capF, res, 2, d->d_frameEntry, d->d_entries);
+    zbd_entries_result_kernel<<<1, ZBD_ENTRY_SCAN, 0, st>>>(d->d_entries, nbEntries, sizes, result);
+    CK(cudaGetLastError());
+    TRY(call.leave(st));
+    d->stats.launches = 12;
+    return 0;
+}
+
+extern "C" size_t ZSTDB200_decompressFramesAsync(ZSTD_DCtx* d, void* d_dst, size_t dstCapacity, const size_t* dstOffsets, const size_t* dstCapacities,
+                                                 const void* d_src, size_t srcSize, const size_t* srcOffsets, const size_t* srcSizes,
+                                                 size_t nbEntries, unsigned long long* d_dSizes, unsigned long long* d_result, void* stream)
+{
+    return zbd_decompressFrames(d, (u8*)d_dst, dstCapacity, dstOffsets, dstCapacities, (const u8*)d_src, srcSize, srcOffsets, srcSizes, nbEntries,
+                                d_dSizes, d_result, false, (cudaStream_t)stream);
+}
+
+/* the stream-ordered call on the caller's stream (NULL: the context's), then one read-back of the verdict and the sizes */
+extern "C" size_t ZSTDB200_decompressFrames(ZSTD_DCtx* d, void* d_dst, size_t dstCapacity, const size_t* dstOffsets, const size_t* dstCapacities,
+                                            const void* d_src, size_t srcSize, const size_t* srcOffsets, const size_t* srcSizes,
+                                            size_t nbEntries, size_t* dSizes, void* stream)
+{
+    if (!d) return ZB_ERR(ZB_error_GENERIC);
+    ZbDeviceGuard guard;
+    TRY(zbd_ctxInit(d));
+    cudaStream_t const st = stream ? (cudaStream_t)stream : (cudaStream_t)d->stream;
+    unsigned long long marker = 0;                                    /* non-NULL: the sizes are wanted */
+    TRY(zbd_decompressFrames(d, (u8*)d_dst, dstCapacity, dstOffsets, dstCapacities, (const u8*)d_src, srcSize, srcOffsets, srcSizes, nbEntries,
+                             dSizes ? &marker : NULL, NULL, true, st));
+    size_t const words = 1 + (dSizes ? nbEntries : 0);
+    CK(cudaMemcpyAsync(d->h_verdict, d->d_verdict, words * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    for (size_t i = 0; dSizes && i < nbEntries; i++) dSizes[i] = (size_t)d->h_verdict[1 + i];
+    return (size_t)d->h_verdict[0];
 }
 
 /* ------------------------------------------------------------------------------------------------ one-shot calls */
