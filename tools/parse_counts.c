@@ -15,9 +15,13 @@
  *   fwd rounds        256-byte rounds of forward compares per match (floor(counted / 256) + 1, counted from the probe for
  *                     a table hit, from probe + 4 for a repcode hit);
  *   back rounds       32-byte rounds of backward catch-up per match (floor(back / 32) + 1);
- *   back > 4          matches whose catch-up exceeds 4 bytes (the in-lane repcode-1 catch-up of the kernel before stopped there).
- * From these it prints the dependent memory round trips per segment of the kernel before and after the change that
- * gave each step one round trip (DESIGN.md section 2, K1b). */
+ *   back > 4          matches whose catch-up exceeds 4 bytes (the in-lane repcode-1 catch-up of the kernel before stopped there);
+ *   catch-up split    matches whose catch-up lane 31's 8-byte window answers (fewer than 8 bytes) and those that go on to
+ *                     the cooperative 32-byte rounds (8 or more); the forward rounds past the first window (31 lanes,
+ *                     248 bytes, then 256 per round).
+ * From these it prints the dependent memory round trips per segment of three kernels: two per step; one per step with a
+ * hit's first rounds waiting twice; and the current one, where a hit's windows all go out before the first is compared
+ * (DESIGN.md section 2, K1b). */
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -28,7 +32,7 @@ static size_t count_eq(const u8* a, const u8* b, const u8* end) { const u8* s = 
 
 typedef struct {
     double segs, steps, matches, h3, h2, h1, tried, tagFalse, farTried, farLost, farWon, fwdRounds, backRounds, back4,
-           fwdExtra, backExtra, backRoundsTable, rep1Coop;
+           fwdExtra, backExtra, backRoundsTable, rep1Coop, backInWin, backCoop, fwdExtraWin, backExtraWin;
 } counts;
 
 static void parse_segment(const zbo_plan* plan, const u8* frame, const u32* dist, size_t bs, size_t be, size_t ss, size_t se,
@@ -76,6 +80,11 @@ static void parse_segment(const zbo_plan* plan, const u8* frame, const u32* dist
             c->backExtra += (double)(back / 32);
             if (wtype == 1) c->backRoundsTable += (double)(back / 32 + 1);
             if (back > 4) { c->back4++; if (wtype == 2) c->rep1Coop += (double)((back - 4) / 32 + 1); }
+            if (back < 8) c->backInWin++;
+            else { c->backCoop++; c->backExtraWin += (double)((back - 8) / 32 + 1); }
+            {   size_t const counted = (wtype == 1) ? fwd + 4 : fwd;
+                if (counted >= 248) c->fwdExtraWin += (double)((counted - 248) / 256 + 1);
+            }
             if (wtype == 3) { u32 const t = rep2; rep2 = rep1; rep1 = t; }
             else if (wtype == 1) { rep2 = rep1; rep1 = offset; }
             ip = ms + mlen; anchor = ip; searchStart = ip;
@@ -126,19 +135,24 @@ int main(int argc, char** argv)
         /* before: 2 round trips per step (the dist row, then the windows and the far distance); per match the forward
          * rounds and the backward rounds of a table hit or of a repcode-1 hit with more than 4 bytes of catch-up, plus one
          * for the repcode-1 in-lane catch-up's window; one forward round per tried false positive.
-         * after: 1 per step, 1 per far lane tried; per match and per tried false positive the first forward and backward
-         * rounds, which go out together but wait twice in the sm_90a SASS (the compare of the current window is scheduled
-         * before the loads of the candidate window and of the catch-up bytes), then the extra rounds of each */
+         * waiting twice: 1 per step, 1 per far lane tried; per match and per tried false positive the first forward and
+         * backward rounds, which went out together but waited twice in the sm_90a SASS (the compare of the current window
+         * was scheduled before the loads of the candidate window and of the catch-up bytes), then the extra rounds of each;
+         * now: the same, but a hit's two windows per lane (lane 31's holding the catch-up) wait once, and the extra rounds
+         * start past 248 bytes forward and 8 bytes backward */
         double const rtOld = 2 * c.steps + c.fwdRounds + c.backRoundsTable + c.h2 + c.rep1Coop + c.tagFalse;
-        double const rtNew = c.steps + c.farTried + 2 * (M + c.tagFalse) + c.fwdExtra + c.backExtra;
+        double const rtTwice = c.steps + c.farTried + 2 * (M + c.tagFalse) + c.fwdExtra + c.backExtra;
+        double const rtNow = c.steps + c.farTried + (M + c.tagFalse) + c.fwdExtraWin + c.backExtraWin;
         printf("{\"input_bytes\": %zu, \"level\": %d, \"segments\": %.0f, \"per_segment\": {\"steps\": %.2f, \"matches\": %.2f, "
                "\"rep2\": %.2f, \"rep1\": %.2f, \"table\": %.2f, \"tried\": %.2f, \"tag_false\": %.3f, \"far_tried\": %.3f, "
-               "\"far_out_of_reach\": %.3f, \"far_won\": %.3f, \"back_gt4\": %.2f, \"fwd_rounds\": %.2f, \"back_rounds\": %.2f}, "
+               "\"far_out_of_reach\": %.3f, \"far_won\": %.3f, \"back_gt4\": %.2f, \"fwd_rounds\": %.2f, \"back_rounds\": %.2f, "
+               "\"catchup_in_window\": %.2f, \"catchup_cooperative\": %.2f, \"fwd_past_window\": %.2f}, "
                "\"per_match\": {\"steps\": %.3f, \"fwd_rounds\": %.3f, \"back_rounds\": %.3f}, "
-               "\"round_trips_per_segment\": {\"before\": %.1f, \"after\": %.1f}}\n",
+               "\"round_trips_per_segment\": {\"two_per_step\": %.1f, \"hit_waits_twice\": %.1f, \"hit_waits_once\": %.1f}}\n",
                n, level, S, c.steps / S, M / S, c.h3 / S, c.h2 / S, c.h1 / S, c.tried / S, c.tagFalse / S, c.farTried / S,
                c.farLost / S, c.farWon / S, c.back4 / S, c.fwdRounds / S, c.backRounds / S,
-               c.steps / M, c.fwdRounds / M, c.backRounds / M, rtOld / S, rtNew / S);
+               c.backInWin / S, c.backCoop / S, c.fwdExtraWin / S,
+               c.steps / M, c.fwdRounds / M, c.backRounds / M, rtOld / S, rtTwice / S, rtNow / S);
     }
     free(src);
     return 0;

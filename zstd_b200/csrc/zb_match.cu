@@ -375,6 +375,19 @@ __device__ __forceinline__ u32 zb_dist_at(const u16* __restrict__ d16, const u32
     return d == ZB_FAR ? far[i] : d;
 }
 
+/* zb_seg_ld64x for the hit path: the same three words, the third addressed as the word of the last byte, (p + 7) & ~3,
+ * which takes three instructions where choosing between the second and third word after p takes seven */
+template <bool DICT>
+__device__ __forceinline__ u64 zb_hit_ld64(const ZbSeg& sg, u32 rel)
+{
+    if (DICT && rel < sg.split && rel + 12u > sg.split) return zb_seg_ld64x<true>(sg, rel);
+    const u8* const p = zb_seg_ptr<DICT>(sg, rel);
+    const u32* const w = (const u32*)((uintptr_t)p & ~(uintptr_t)3);
+    u32 const sh = ((u32)(uintptr_t)p & 3u) * 8u;
+    u32 const x = __ldg(w), y = __ldg(w + 1), z = __ldg((const u32*)((uintptr_t)(p + 7) & ~(uintptr_t)3));
+    return ((u64)__funnelshift_r(y, z, sh) << 32) | __funnelshift_r(x, y, sh);
+}
+
 template <bool DICT>
 __global__ void __launch_bounds__(32 * PARSE_WARPS, DICT ? (40 / PARSE_WARPS) : PARSE_MIN_CTAS)
 zb_parse_kernel(const u8* __restrict__ src, const ZbDictSlot* __restrict__ dicts, const ZbBlock* __restrict__ blocks, u32 nbBlocks, ZbParams prm, ZbStrides sd,
@@ -443,7 +456,7 @@ zb_parse_kernel(const u8* __restrict__ src, const ZbDictSlot* __restrict__ dicts
         bool found = false;
         while (tent) {
             u32 const winner = (u32)__ffs((int)tent) - 1u;
-            probe = ip + (winner >> 1) * step + (winner & 1u);
+            probe = __shfl_sync(ZB_FULL, p, winner);
             u32 const w = __shfl_sync(ZB_FULL, hd, winner);
             wtype = w & 3u;
             offset = (wtype == 3u) ? rep2 : ((wtype == 2u) ? rep1 : w >> 2);
@@ -451,28 +464,31 @@ zb_parse_kernel(const u8* __restrict__ src, const ZbDictSlot* __restrict__ dicts
                 offset = myfar[probe - bs];
                 if (probe < offset) { tent &= tent - 1u; continue; }
             }
-            /* one round trip for the first forward round and the first backward round (zstd_fast.c:387-391) together: a
-             * table hit is counted from the probe itself (its first 4 bytes are not verified yet), a repcode hit from
-             * probe + 4.  A repcode-2 hit sits at the anchor: it has nothing to catch up */
+            /* one round trip for the first forward round and the first backward round (zstd_fast.c:387-391) together, in
+             * one pair of 8-byte windows per lane.  Lanes 0..30 count forward, 248 bytes: a table hit from the probe itself
+             * (its first 4 bytes are not verified yet), a repcode hit from probe + 4.  Lane 31 reads the 8 bytes in front of
+             * the probe (fewer where the candidate would leave the history) and counts the catch-up from its top byte down,
+             * bit-reversed so that every lane counts equal bytes from its bottom.  Only a catch-up that fills lane 31's
+             * window goes on to the cooperative rounds.  A repcode-2 hit sits at the anchor: it has nothing to catch up */
             u32 const a = (wtype == 1u) ? probe : probe + 4u;
-            u32 const kb = lane + 1u;                     /* backward: bytes probe - kb and probe - offset - kb */
-            bool const bIn = (probe >= anchor + kb) && (probe >= offset + kb);
-            u32 const b0 = bIn ? zb_seg_byte<DICT>(sg, probe - kb) : 0u;
-            u32 const b1 = bIn ? zb_seg_byte<DICT>(sg, probe - offset - kb) : 0u;
+            bool const cu = lane == 31u;
             u32 const pa = a + 8u * lane;                 /* forward: this lane's 8 bytes, read at q so that no lane branches */
-            u32 const q = min(pa, be - 8u);               /* (probe + 8 <= be, so q >= probe >= offset) */
-            u64 const xf = zb_seg_ld64x<DICT>(sg, q) ^ zb_seg_ld64x<DICT>(sg, q - offset);
-            u64 const xs = xf >> (8u * min(pa - q, 7u));
-            u32 m = xs ? (u32)((__ffsll((long long)xs) - 1) >> 3) : 8u;
-            m = pa >= be ? 0u : min(m, be - pa);
-            u32 const okb = __ballot_sync(ZB_FULL, bIn && b0 == b1);
-            u32 const inc = __ballot_sync(ZB_FULL, m != 8u);
+            u32 const db = min(8u, probe - offset);       /* catch-up bytes lane 31 may read: q - offset stays >= 0 */
+            u32 const q = cu ? probe - db : min(pa, be - 8u);   /* (probe + 8 <= be, so q >= probe - db >= offset) */
+            u64 const xf = zb_hit_ld64<DICT>(sg, q) ^ zb_hit_ld64<DICT>(sg, q - offset);
+            u64 const xs = (cu ? __brevll(xf) : xf) >> (8u * min(cu ? 8u - db : pa - q, 7u));
+            u32 const lo = (u32)xs, hi = (u32)(xs >> 32);
+            u32 m = (lo ? __clz(__brev(lo)) : 32u + __clz(__brev(hi))) >> 3;          /* equal bytes from the bottom, 8 if all */
+            m = min(m, cu ? min(probe - anchor, db) : (pa >= be ? 0u : be - pa));
+            u32 const stop = __ballot_sync(ZB_FULL, m != 8u);
+            u32 const inc = stop & (ZB_FULL >> 1);
             u32 fwd;
-            if (inc == 0u) fwd = 256u + zb_count_fwd<DICT>(sg, a + 256u, offset, be, lane);
+            if (inc == 0u) fwd = 248u + zb_count_fwd<DICT>(sg, a + 248u, offset, be, lane);
             else { int const f = __ffs((int)inc) - 1; fwd = 8u * (u32)f + __shfl_sync(ZB_FULL, m, f); }
             if (wtype == 1u && fwd < 4u) { tent &= tent - 1u; continue; }      /* tag collision */
             fwdFrom4 = (wtype == 1u) ? fwd - 4u : fwd;
-            back = (okb == ZB_FULL) ? 32u + zb_back_coop<DICT>(sg, probe - 32u, offset, anchor, lane) : (u32)(__ffs((int)~okb) - 1);
+            back = __shfl_sync(ZB_FULL, m, 31);
+            if (!(stop >> 31)) back = 8u + zb_back_coop<DICT>(sg, probe - 8u, offset, anchor, lane);
             found = true;
             break;
         }
