@@ -18,28 +18,52 @@
  *   back > 4          matches whose catch-up exceeds 4 bytes (the in-lane repcode-1 catch-up of the kernel before stopped there);
  *   catch-up split    matches whose catch-up lane 31's 8-byte window answers (fewer than 8 bytes) and those that go on to
  *                     the cooperative 32-byte rounds (8 or more); the forward rounds past the first window (31 lanes,
- *                     248 bytes, then 256 per round).
- * From these it prints the dependent memory round trips per segment of three kernels: two per step; one per step with a
- * hit's first rounds waiting twice; and the current one, where a hit's windows all go out before the first is compared
- * (DESIGN.md section 2, K1b). */
+ *                     248 bytes, then 256 per round);
+ *   pairs             iterations of the current kernel, which probes two steps per iteration (a pair of positions per
+ *                     lane); its winners in the first half (the step at ip) and in the second (the step after it), and
+ *                     those found in a later iteration than the first after the anchor; tries per iteration.
+ * From these it prints the dependent memory round trips per segment of four kernels: two per step; one per step with a
+ * hit's first rounds waiting twice; one per step with a hit's windows all out before the first is compared; and the
+ * current one, one per iteration of two steps (DESIGN.md section 2, K1b).  It also prints the issue floor of config 2 of
+ * the last two kernels from their SASS instruction counts. */
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 #include "../oracle/zb_oracle.h"
+
+/* warp instructions of zb_parse_kernel<false> per path, counted in `cuobjdump -sass` of the sm_90a build (DESIGN.md
+ * section 10): one step of one position per lane without a hit and with a table hit (through the store of the
+ * sequence), and the same for one iteration of the pair kernel (two steps, a pair of positions per lane) */
+#define SASS_STEP_MISS 84
+#define SASS_STEP_HIT 216
+#define SASS_PAIR_MISS 88
+#define SASS_PAIR_HIT 239
 
 static u32 rd32(const u8* p) { u32 v; memcpy(&v, p, 4); return v; }
 static size_t count_eq(const u8* a, const u8* b, const u8* end) { const u8* s = a; while (a < end && *a == *b) { a++; b++; } return (size_t)(a - s); }
 
 typedef struct {
     double segs, steps, matches, h3, h2, h1, tried, tagFalse, farTried, farLost, farWon, fwdRounds, backRounds, back4,
-           fwdExtra, backExtra, backRoundsTable, rep1Coop, backInWin, backCoop, fwdExtraWin, backExtraWin;
+           fwdExtra, backExtra, backRoundsTable, rep1Coop, backInWin, backCoop, fwdExtraWin, backExtraWin,
+           iters, winFirstHalf, winSecondHalf, winLater;
 } counts;
+
+/* two steps of the rule per iteration of the pair kernel: a match found after j steps without a hit is found in iteration
+ * j / 2 after the anchor, in its first half when j is even; s steps without a hit at a segment's end take (s + 1) / 2 */
+static void pair_iters(counts* c, double j, int hit)
+{
+    if (!hit) { c->iters += (double)(((size_t)j + 1) / 2); return; }
+    c->iters += (double)((size_t)j / 2 + 1);
+    if ((size_t)j % 2 == 0) c->winFirstHalf++; else c->winSecondHalf++;
+    if (j >= 2) c->winLater++;
+}
 
 static void parse_segment(const zbo_plan* plan, const u8* frame, const u32* dist, size_t bs, size_t be, size_t ss, size_t se,
                           size_t lowLimit, counts* c)
 {
     size_t ip = ss, anchor = ss, searchStart = ss;
     u32 rep1 = 0, rep2 = 0;
+    double misses = 0;                                   /* steps without a hit since the anchor */
     c->segs++;
     while (ip < se && ip + 8 <= be) {
         u32 const step = plan->stepSize + (u32)((ip - searchStart) >> 7);
@@ -63,7 +87,9 @@ static void parse_segment(const zbo_plan* plan, const u8* frame, const u32* dist
                 if (d >= 0xFFFFu) c->farWon++;
             }
         }
-        if (winner < 0) { ip += (size_t)(ZB_WARP / 2) * step; continue; }
+        if (winner < 0) { misses++; ip += (size_t)(ZB_WARP / 2) * step; continue; }
+        pair_iters(c, misses, 1);
+        misses = 0;
         {   size_t ms = probe, mm = probe - offset, mlen, fwd, back;
             if (wtype != 3)
                 while (ms > anchor && mm > lowLimit && frame[ms - 1] == frame[mm - 1]) { ms--; mm--; }
@@ -90,6 +116,7 @@ static void parse_segment(const zbo_plan* plan, const u8* frame, const u32* dist
             ip = ms + mlen; anchor = ip; searchStart = ip;
         }
     }
+    pair_iters(c, misses, 0);
 }
 
 int main(int argc, char** argv)
@@ -138,21 +165,37 @@ int main(int argc, char** argv)
          * waiting twice: 1 per step, 1 per far lane tried; per match and per tried false positive the first forward and
          * backward rounds, which went out together but waited twice in the sm_90a SASS (the compare of the current window
          * was scheduled before the loads of the candidate window and of the catch-up bytes), then the extra rounds of each;
-         * now: the same, but a hit's two windows per lane (lane 31's holding the catch-up) wait once, and the extra rounds
-         * start past 248 bytes forward and 8 bytes backward */
+         * once: the same, but a hit's two windows per lane (lane 31's holding the catch-up) wait once, and the extra rounds
+         * start past 248 bytes forward and 8 bytes backward;
+         * pairs: the same per iteration of two steps as per step before */
         double const rtOld = 2 * c.steps + c.fwdRounds + c.backRoundsTable + c.h2 + c.rep1Coop + c.tagFalse;
         double const rtTwice = c.steps + c.farTried + 2 * (M + c.tagFalse) + c.fwdExtra + c.backExtra;
-        double const rtNow = c.steps + c.farTried + (M + c.tagFalse) + c.fwdExtraWin + c.backExtraWin;
+        double const rtOnce = c.steps + c.farTried + (M + c.tagFalse) + c.fwdExtraWin + c.backExtraWin;
+        double const rtPairs = c.iters + c.farTried + (M + c.tagFalse) + c.fwdExtraWin + c.backExtraWin;
+        /* issue floor of config 2: 1 GiB in 16 KiB segments on the 132 SMs of an H100, 4 warp instructions per cycle per SM
+         * at 1980 MHz, the instructions per segment from the SASS counts above (tag false positives and far fetches left
+         * out of both) */
+        double const floorK = 65536.0 / (132.0 * 4.0 * 1980e6) * 1e3;
+        double const instStep = (c.steps - M) * SASS_STEP_MISS + M * SASS_STEP_HIT;
+        double const instPair = (c.iters - M) * SASS_PAIR_MISS + M * SASS_PAIR_HIT;
         printf("{\"input_bytes\": %zu, \"level\": %d, \"segments\": %.0f, \"per_segment\": {\"steps\": %.2f, \"matches\": %.2f, "
                "\"rep2\": %.2f, \"rep1\": %.2f, \"table\": %.2f, \"tried\": %.2f, \"tag_false\": %.3f, \"far_tried\": %.3f, "
                "\"far_out_of_reach\": %.3f, \"far_won\": %.3f, \"back_gt4\": %.2f, \"fwd_rounds\": %.2f, \"back_rounds\": %.2f, "
                "\"catchup_in_window\": %.2f, \"catchup_cooperative\": %.2f, \"fwd_past_window\": %.2f}, "
                "\"per_match\": {\"steps\": %.3f, \"fwd_rounds\": %.3f, \"back_rounds\": %.3f}, "
-               "\"round_trips_per_segment\": {\"two_per_step\": %.1f, \"hit_waits_twice\": %.1f, \"hit_waits_once\": %.1f}}\n",
+               "\"pairs_per_segment\": {\"iterations\": %.2f, \"win_first_half\": %.2f, \"win_second_half\": %.2f, "
+               "\"win_later_iteration\": %.2f, \"tries_per_iteration\": %.3f, \"iterations_per_match\": %.3f}, "
+               "\"round_trips_per_segment\": {\"two_per_step\": %.1f, \"hit_waits_twice\": %.1f, \"hit_waits_once\": %.1f, "
+               "\"pairs\": %.1f}, "
+               "\"issue_floor_ms\": {\"one_step_per_iteration\": %.2f, \"pairs\": %.2f}, \"instructions_per_match\": {\"one_step_per_iteration\": %.1f, "
+               "\"pairs\": %.1f}}\n",
                n, level, S, c.steps / S, M / S, c.h3 / S, c.h2 / S, c.h1 / S, c.tried / S, c.tagFalse / S, c.farTried / S,
                c.farLost / S, c.farWon / S, c.back4 / S, c.fwdRounds / S, c.backRounds / S,
                c.backInWin / S, c.backCoop / S, c.fwdExtraWin / S,
-               c.steps / M, c.fwdRounds / M, c.backRounds / M, rtOld / S, rtTwice / S, rtNow / S);
+               c.steps / M, c.fwdRounds / M, c.backRounds / M,
+               c.iters / S, c.winFirstHalf / S, c.winSecondHalf / S, c.winLater / S, (c.tried + c.h2 + c.h3) / c.iters, c.iters / M,
+               rtOld / S, rtTwice / S, rtOnce / S, rtPairs / S,
+               floorK * instStep / S, floorK * instPair / S, instStep / M, instPair / M);
     }
     free(src);
     return 0;

@@ -388,6 +388,27 @@ __device__ __forceinline__ u64 zb_hit_ld64(const ZbSeg& sg, u32 rel)
     return ((u64)__funnelshift_r(y, z, sh) << 32) | __funnelshift_r(x, y, sh);
 }
 
+/* the 4 bytes at rel and the 4 bytes at rel + 1: the two aligned words around rel hold these 5 bytes whatever rel's
+ * alignment (the second funnel shift clamps at 32: at rel % 4 == 3 the bytes at rel + 1 are the second word).  A window
+ * that straddles the dictionary / frame border is read byte by byte */
+template <bool DICT>
+__device__ __forceinline__ void zb_ld4x2(const ZbSeg& sg, u32 rel, u32& at, u32& at1)
+{
+    if (DICT && rel < sg.split && rel + 5u > sg.split) {
+        u64 v = 0;
+#pragma unroll
+        for (u32 i = 0; i < 5u; i++) v |= (u64)zb_seg_byte<true>(sg, rel + i) << (8u * i);
+        at = (u32)v; at1 = (u32)(v >> 8);
+        return;
+    }
+    const u8* const p = zb_seg_ptr<DICT>(sg, rel);
+    const u32* const w = (const u32*)((uintptr_t)p & ~(uintptr_t)3);
+    u32 const sh = ((u32)(uintptr_t)p & 3u) * 8u;
+    u32 const x = __ldg(w), y = __ldg(w + 1);
+    at = __funnelshift_r(x, y, sh);
+    at1 = __funnelshift_rc(x, y, sh + 8u);
+}
+
 template <bool DICT>
 __global__ void __launch_bounds__(32 * PARSE_WARPS, DICT ? (40 / PARSE_WARPS) : PARSE_MIN_CTAS)
 zb_parse_kernel(const u8* __restrict__ src, const ZbDictSlot* __restrict__ dicts, const ZbBlock* __restrict__ blocks, u32 nbBlocks, ZbParams prm, ZbStrides sd,
@@ -421,6 +442,7 @@ zb_parse_kernel(const u8* __restrict__ src, const ZbDictSlot* __restrict__ dicts
     }
     u32 const se = min(ss + ZB_PARSE_SEG, blockEnd);
     u32 const be = blockEnd;
+    int const last = min((int)se - 1, (int)be - 8);            /* the last position probed: p < se and p + 8 <= be */
 
     u32 ip = ss, anchor = ss;                                  /* the search restarts at the anchor: it is searchStart too */
     u32 rep1 = 0, rep2 = 0, nbSeq = 0;
@@ -428,42 +450,59 @@ zb_parse_kernel(const u8* __restrict__ src, const ZbDictSlot* __restrict__ dicts
 
     /* the 4 bytes at rel position x; x + 8 <= be */
     auto ld4 = [&](u32 x) { return DICT ? (u32)zb_seg_ld64x<DICT>(sg, x) : zb_ld32w2(sg.hi + x); };
-    while (ip < se && ip + 8u <= be) {
+    while ((int)ip <= last) {
+        /* two steps of the rule per iteration, one pair (p, p+1) per lane: lanes 0..15 hold the step at ip, lanes 16..31
+         * the step the rule takes next when the first finds nothing, at ip2 with its own acceleration.  Pairs never
+         * overlap (stepSize >= 2, checked at the launch), so position order is lane order, then p before p+1 */
         u32 const step = prm.stepSize + ((ip - anchor) >> 7);                /* kSearchStrength = 8 */
-        u32 const p = ip + (lane >> 1) * step + (lane & 1u);
-        bool const act = (p < se) && (p + 8u <= be);
+        u32 const ip2 = ip + 16u * step;
+        u32 const step2 = prm.stepSize + ((ip2 - anchor) >> 7);
+        u32 const next = ip2 + 16u * step2;                  /* where the search goes on when no position hits */
+        u32 const p = lane < 16u ? ip + lane * step : ip2 + (lane - 16u) * step2;
+        bool const act = (int)p <= last, act1 = (int)p < last;
         u32 const pp = act ? p : ip;                         /* a position every lane may load from (ip + 8 <= be) */
-        /* one round trip per step: the candidate row, the current window and both repcode windows are independent loads
-         * and all go out before the first is looked at.  dist[] only holds tag-verified candidates, so a step needs no
-         * random load: every window is contiguous across lanes.  A far distance (d16 == ZB_FAR) counts as a table
-         * candidate here; its 32-bit value is fetched only when its lane is tried, below */
-        u32 const d16 = act ? (u32)mydist[pp - bs] : 0u;
+        /* one round trip per iteration: the candidate pair, the current window and both repcode windows are independent
+         * loads and all go out before the first is looked at.  One window at p gives the 4 bytes at p and at p+1; one at
+         * p - rep1 gives both repcode-1 compares (read at 0 where only p+1 reaches the history: p + 1 == rep1).  dist[]
+         * only holds tag-verified candidates, so a step needs no random load: every window is contiguous across lanes.
+         * Whether a table candidate reaches the history is checked when its position is tried, below: a far distance
+         * (ZB_FAR) has its 32-bit value fetched only then.  pp + 1 < be: both entries lie in the block's row */
+        const u16* const dp = mydist + (pp - bs);
+        u32 const d0 = dp[0], d1 = dp[1];
+        u32 const r = pp - rep1;                             /* < pp: rep1 reaches the history from p (rep1 == 0: none) */
         bool const v3 = (lane == 0u) && (ip == anchor) && (rep2 != 0u);
-        bool const v2 = act && rep1 != 0u && p >= rep1;
-        u32 const cur = ld4(pp);
-        u32 const cur2 = ld4(v2 ? pp - rep1 : pp);
+        bool const v2 = act && r < pp;
+        bool const v21 = act1 && r + 1u <= pp;
+        u32 cur, cur1, rc, rc1;
+        zb_ld4x2<DICT>(sg, pp, cur, cur1);
+        zb_ld4x2<DICT>(sg, r < pp ? r : 0u, rc, rc1);
+        if (r >= pp) rc1 = rc;
         u32 cur3 = ~cur;
         if (ip == anchor && rep2 != 0u) cur3 = ld4(v3 ? pp - rep2 : pp);      /* warp-uniform condition */
-        bool const v1 = act && d16 != 0u && (d16 == ZB_FAR || p >= d16);
-        u32 const hit = (v3 && cur3 == cur) ? 3u : ((v2 && cur2 == cur) ? 2u : (v1 ? 1u : 0u));
-        u32 const hd = (d16 << 2) | hit;                     /* what the winner's lane hands out: one register through the tries */
-        u32 tent = __ballot_sync(ZB_FULL, hit != 0u);
-        /* lowest lane first.  A table hit (type 1) is only tag-verified by K1a: its bytes are checked while the match is
-         * extended; a false positive drops out and the next lane is tried — the result is "lowest lane whose hit is real",
-         * what the oracle computes.  So does a far candidate that reaches in front of the history (a lane whose repcodes
-         * had matched would not be a type-1 hit). */
+        u32 const hit = (v3 && cur3 == cur) ? 3u : ((v2 && rc == cur) ? 2u : ((act && d0 != 0u) ? 1u : 0u));
+        u32 const hit1 = (v21 && rc1 == cur1) ? 2u : ((act1 && d1 != 0u) ? 1u : 0u);
+        /* what a lane hands out when one of its positions is tried: type and distance.  A position that drops out clears
+         * its own; a lane tries p while hd holds a hit, then p+1 */
+        u32 hd = (d0 << 2) | hit, hd1 = (d1 << 2) | hit1;
+        u32 tent = __ballot_sync(ZB_FULL, (hit | hit1) != 0u);
+        /* lowest position first: the lowest lane with a hit, its p before its p+1.  A table hit (type 1) is only
+         * tag-verified by K1a: its bytes are checked while the match is extended; a false positive drops out and the next
+         * position is tried — the result is "lowest position whose hit is real", what the oracle computes over its two
+         * steps.  So does a table candidate that reaches in front of the history (a position whose repcodes had matched
+         * would not be a type-1 hit). */
         u32 probe = 0, wtype = 0, offset = 0, back = 0, fwdFrom4 = 0;
         bool found = false;
         while (tent) {
             u32 const winner = (u32)__ffs((int)tent) - 1u;
-            probe = __shfl_sync(ZB_FULL, p, winner);
-            u32 const w = __shfl_sync(ZB_FULL, hd, winner);
+            bool const odd = (hd & 3u) == 0u;                /* this lane's next position is p+1 */
+            probe = __shfl_sync(ZB_FULL, odd ? p + 1u : p, winner);
+            u32 const w = __shfl_sync(ZB_FULL, odd ? hd1 : hd, winner);
             wtype = w & 3u;
             offset = (wtype == 3u) ? rep2 : ((wtype == 2u) ? rep1 : w >> 2);
-            if (wtype == 1u && offset == ZB_FAR) {                                /* rare: one more round trip */
-                offset = myfar[probe - bs];
-                if (probe < offset) { tent &= tent - 1u; continue; }
-            }
+            /* a position that drops out clears its hit: its lane goes on to its p+1 or leaves the vote */
+            auto dropOut = [&]() { if (lane == winner) { if (odd) hd1 = 0u; else hd = 0u; } tent = __ballot_sync(ZB_FULL, ((hd | hd1) & 3u) != 0u); };
+            if (wtype == 1u && offset == ZB_FAR) offset = myfar[probe - bs];   /* rare: one more round trip */
+            if (probe < offset) { dropOut(); continue; }     /* a table candidate in front of the history (a repcode never is) */
             /* one round trip for the first forward round and the first backward round (zstd_fast.c:387-391) together, in
              * one pair of 8-byte windows per lane.  Lanes 0..30 count forward, 248 bytes: a table hit from the probe itself
              * (its first 4 bytes are not verified yet), a repcode hit from probe + 4.  Lane 31 reads the 8 bytes in front of
@@ -485,19 +524,20 @@ zb_parse_kernel(const u8* __restrict__ src, const ZbDictSlot* __restrict__ dicts
             u32 fwd;
             if (inc == 0u) fwd = 248u + zb_count_fwd<DICT>(sg, a + 248u, offset, be, lane);
             else { int const f = __ffs((int)inc) - 1; fwd = 8u * (u32)f + __shfl_sync(ZB_FULL, m, f); }
-            if (wtype == 1u && fwd < 4u) { tent &= tent - 1u; continue; }      /* tag collision */
+            if (wtype == 1u && fwd < 4u) { dropOut(); continue; }           /* tag collision */
             fwdFrom4 = (wtype == 1u) ? fwd - 4u : fwd;
             back = __shfl_sync(ZB_FULL, m, 31);
             if (!(stop >> 31)) back = 8u + zb_back_coop<DICT>(sg, probe - 8u, offset, anchor, lane);
             found = true;
             break;
         }
-        if (!found) { ip += 16u * step; continue; }
+        if (!found) { ip = next; continue; }
         u32 const ms = probe - back;
         u32 const mlen = back + 4u + fwdFrom4;
         if (wtype == 3u) { u32 const t = rep2; rep2 = rep1; rep1 = t; }
         else if (wtype == 1u) { rep2 = rep1; rep1 = offset; }
-        if (lane == 0) seqs[(size_t)b * sd.seq + k * (ZB_PARSE_SEG / 4u) + nbSeq] = zb_pack_raw(offset, mlen, ms - bs);   /* the address is rebuilt per match: it would not stay in a register */
+        {   u32 bb = b; asm("" : "+r"(bb));                /* the row's address is rebuilt per match: kept, it would spill */
+            if (lane == 0) seqs[(size_t)bb * sd.seq + k * (ZB_PARSE_SEG / 4u) + nbSeq] = zb_pack_raw(offset, mlen, ms - bs); }
         nbSeq++;
         ip = ms + mlen; anchor = ip;
     }
@@ -946,6 +986,7 @@ extern "C" cudaError_t zb_launch_match(const u8* d_src, const ZbDictSlot* d_dict
         if (dict) zb_parse_dfast_kernel<true><<<sgrid, 32 * PARSE_WARPS, 0, stream>>>(d_src, d_dicts, d_blocks, nbBlocks, *prm, sd, d_dist, d_far, d_dist2, d_far2, d_seqs, d_meta, d_segmeta);
         else      zb_parse_dfast_kernel<false><<<sgrid, 32 * PARSE_WARPS, 0, stream>>>(d_src, d_dicts, d_blocks, nbBlocks, *prm, sd, d_dist, d_far, d_dist2, d_far2, d_seqs, d_meta, d_segmeta);
     } else {
+        if (prm->stepSize < 2u) return cudaErrorInvalidValue;    /* zb_parse_kernel's pairs (p, p+1) must not overlap */
         e = zb_launch_walk(d_src, d_dicts, d_chunks, nbChunks, prm->mls, prm->tableN, prm->insStep, sd, slotFirstBlock, d_dist, d_far, 0, false, stream); if (e != cudaSuccess) return e;
         if (evMid) cudaEventRecord(evMid, stream);
         if (dict) zb_parse_kernel<true><<<sgrid, 32 * PARSE_WARPS, 0, stream>>>(d_src, d_dicts, d_blocks, nbBlocks, *prm, sd, d_dist, d_far, d_seqs, d_meta, d_segmeta);
