@@ -348,6 +348,34 @@ ZSTDB200_API size_t ZSTDB200_decompressFramesAsync(ZSTD_DCtx* dctx,
         const void* d_src, size_t srcSize, const size_t* srcOffsets, const size_t* srcSizes,
         size_t nbEntries, unsigned long long* d_dSizes, unsigned long long* d_result, void* stream);
 
+/* The same calls with one digested dictionary per entry (the decoder's counterpart of ZSTDB200_compressFrames_usingCDicts):
+ * a batch written against many dictionaries is read back in one launch sequence.  Everything stated above holds (slots,
+ * writes, per-entry results, return value, refusals, workspace, ordering, the staging ring, capture, launches); only where
+ * each entry's dictionary comes from differs.
+ * Entry i's bytes and result are what ZSTDB200_decompressDevice gives for it on a context whose sticky dictionary is ddicts[i]
+ * (ZSTD_DCtx_refDDict): a frame that names another dictionary ID gets dictionary_wrong (32), and fails alone.  A NULL entry,
+ * a NULL ddicts, or a DDict of size 0 means no dictionary for that entry.  ddicts is a host array read before the call
+ * returns; the same DDict may appear any number of times.  The DDicts must stay alive until the work ran.
+ * The context's sticky dictionary is not used and is left as it is; a pending ZSTD_DCtx_refPrefix still gets
+ * parameter_unsupported (40) and is forgotten.
+ * More refusals, decided before anything is enqueued (dSizes is then not written): parameter_unsupported (40) for a DDict
+ * resident on another device, as ZSTD_decompress_usingDDict gives it; under capture, stage_wrong (60) for any DDict not yet
+ * resident on the context's device.
+ * Dictionaries.  A DDict becomes resident on its first use: the call uploads every DDict it names that is not resident yet,
+ * then synchronises once with the context's own stream.  From then on a DDict costs a call one reference in the staging
+ * slot (8 bytes per entry); the kernels find each block's dictionary through it.  DDicts may be shared by contexts on one
+ * device and by threads.  ZSTDB200_getLastDStats fills launches (12, whatever the number of entries and dictionaries) and
+ * h2d_bytes, the dictionary bytes the call uploaded (0 when all were resident). */
+ZSTDB200_API size_t ZSTDB200_decompressFrames_usingDDicts(ZSTD_DCtx* dctx,
+        void* d_dst, size_t dstCapacity, const size_t* dstOffsets, const size_t* dstCapacities,
+        const void* d_src, size_t srcSize, const size_t* srcOffsets, const size_t* srcSizes,
+        size_t nbEntries, const ZSTD_DDict* const* ddicts, size_t* dSizes, void* stream);
+ZSTDB200_API size_t ZSTDB200_decompressFramesAsync_usingDDicts(ZSTD_DCtx* dctx,
+        void* d_dst, size_t dstCapacity, const size_t* dstOffsets, const size_t* dstCapacities,
+        const void* d_src, size_t srcSize, const size_t* srcOffsets, const size_t* srcSizes,
+        size_t nbEntries, const ZSTD_DDict* const* ddicts,
+        unsigned long long* d_dSizes, unsigned long long* d_result, void* stream);
+
 
 /* Compress one frame whose input and output already live in device memory (HBM).  The call returns when the frame is
  * complete (it synchronises to read the size).

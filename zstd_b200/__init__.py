@@ -156,6 +156,11 @@ def lib() -> ctypes.CDLL:
             L.ZSTDB200_decompressFrames.argtypes = [_vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp]
             L.ZSTDB200_decompressFramesAsync.restype = _sz
             L.ZSTDB200_decompressFramesAsync.argtypes = [_vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp]
+        if hasattr(L, "ZSTDB200_decompressFrames_usingDDicts"):                         # absent from older development builds
+            L.ZSTDB200_decompressFrames_usingDDicts.restype = _sz
+            L.ZSTDB200_decompressFrames_usingDDicts.argtypes = [_vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp]
+            L.ZSTDB200_decompressFramesAsync_usingDDicts.restype = _sz
+            L.ZSTDB200_decompressFramesAsync_usingDDicts.argtypes = [_vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp, _vp]
         L.ZSTDB200_getLastDStats.restype = None
         L.ZSTDB200_getLastDStats.argtypes = [_vp, ctypes.POINTER(DStats)]
     if hasattr(L, "ZSTD_createDDict"):                                                  # absent from older development builds
@@ -439,6 +444,15 @@ def _cdict_array(cdicts, n):
     return (_vp * n)(*[(cd._h if cd is not None else None) for cd in cdicts])
 
 
+def _ddict_array(ddicts, n):
+    """the host array of n DDict handles a per-entry-dictionary call reads (None: a NULL array)"""
+    if ddicts is None:
+        return None
+    if len(ddicts) != n:
+        raise ValueError(f"{len(ddicts)} dictionaries for {n} entries")
+    return (_vp * n)(*[(dd._h if dd is not None else None) for dd in ddicts])
+
+
 def _sequences(seqs):
     """an (n, 4) uint32 array (offset, litLength, matchLength, rep) from such an array or from (offset, litLength,
     matchLength) tuples"""
@@ -603,6 +617,38 @@ class ZSTD_DCtx:
         so, ss, do, dc = ((_sz * n)(*a) for a in (src_offsets, src_sizes, dst_offsets, dst_capacities))
         _check(lib().ZSTDB200_decompressFramesAsync(self._h, d_dst, dst_capacity, do, dc, d_src, src_size, so, ss, n,
                                                     d_d_sizes or None, d_result, stream))
+
+    def decompress_frames_using_ddicts(self, d_dst: int, dst_capacity: int, dst_offsets: Sequence[int],
+                                       dst_capacities: Sequence[int], d_src: int, src_size: int, src_offsets: Sequence[int],
+                                       src_sizes: Sequence[int], ddicts: Optional[Sequence[Optional["ZSTD_DDict"]]], stream: int = 0):
+        """ZSTDB200_decompressFrames_usingDDicts: decompress_frames with entry i decoded against ddicts[i] (None: no
+        dictionary; ddicts None: none for any entry) instead of the sticky dictionary.  Returns (result, [result per entry])."""
+        n = len(src_sizes)
+        if not (len(src_offsets) == len(dst_offsets) == len(dst_capacities) == n):
+            raise ValueError("src_offsets, src_sizes, dst_offsets and dst_capacities differ in length")
+        so, ss, do, dc = ((_sz * n)(*a) for a in (src_offsets, src_sizes, dst_offsets, dst_capacities))
+        dds = _ddict_array(ddicts, n)
+        sizes = (_sz * n)()
+        L = lib()
+        r = L.ZSTDB200_decompressFrames_usingDDicts(self._h, d_dst, dst_capacity, do, dc, d_src, src_size, so, ss, n, dds, sizes, stream)
+        if L.ZSTD_isError(r) and not any(L.ZSTD_isError(v) for v in sizes):
+            _check(r)                                       # refused: no entry holds the error
+        return r, list(sizes)
+
+    def decompress_frames_async_using_ddicts(self, d_dst: int, dst_capacity: int, dst_offsets: Sequence[int],
+                                             dst_capacities: Sequence[int], d_src: int, src_size: int, src_offsets: Sequence[int],
+                                             src_sizes: Sequence[int], ddicts: Optional[Sequence[Optional["ZSTD_DDict"]]],
+                                             d_result: int, d_d_sizes: int = 0, stream: int = 0) -> None:
+        """ZSTDB200_decompressFramesAsync_usingDDicts: decompress_frames_using_ddicts enqueued on `stream`, its results in
+        device memory as for decompress_frames_async.  The DDicts are kept alive until this context's next such call."""
+        n = len(src_sizes)
+        if not (len(src_offsets) == len(dst_offsets) == len(dst_capacities) == n):
+            raise ValueError("src_offsets, src_sizes, dst_offsets and dst_capacities differ in length")
+        so, ss, do, dc = ((_sz * n)(*a) for a in (src_offsets, src_sizes, dst_offsets, dst_capacities))
+        dds = _ddict_array(ddicts, n)
+        _check(lib().ZSTDB200_decompressFramesAsync_usingDDicts(self._h, d_dst, dst_capacity, do, dc, d_src, src_size, so, ss, n,
+                                                                dds, d_d_sizes or None, d_result, stream))
+        self._batch_ddicts = list(ddicts) if ddicts is not None else None     # the kernels read them after this returns
 
     def stats(self) -> DStats:
         s = DStats()

@@ -47,6 +47,8 @@
 #include <vector>
 #include <memory>
 #include <mutex>
+#include <atomic>
+#include <algorithm>
 #include <new>
 #include "../../include/zstd_b200.h"
 #include "zb_common.h"
@@ -80,6 +82,26 @@ typedef struct {
     u32 status;            /* 0 or the entry's error code: the first stage that fails it writes it, later stages skip it */
     u32 pad;
 } ZbdEntry;
+
+/* A resident DDict's descriptor, written on the device behind its bytes when it becomes resident (zbd_residentDicts): what the
+ * kernels need of a dictionary, found through one pointer. */
+typedef struct {
+    ZbdDictInfo di;
+    const u8* dict;        /* the whole dictionary on the device; its content is [dict + di.contentOff, + contentSize) */
+    u32 contentSize;
+    u32 pad;
+} ZbdDictRef;
+
+/* Where the kernels find a block's dictionary: one reference for the whole call (NULL: none), or, in batch calls with a
+ * dictionary per entry, an array of one reference per entry (a NULL reference: none), found through the frame's entry. */
+typedef struct {
+    const ZbdDictRef* one;
+    const ZbdDictRef* const* perEntry;
+} ZbdDicts;
+__device__ __forceinline__ const ZbdDictRef* zbd_dictOf(ZbdDicts ds, const u32* __restrict__ frameEntry, u32 frame)
+{
+    return ds.perEntry ? ds.perEntry[frameEntry[frame]] : ds.one;
+}
 
 /* d_res, the call's results in device memory.  [0, 5): the walk's error, blocks, frames, literal bytes, sequences.  A
  * stream-ordered call also uses [5, 7): the blocks and frames the kernels run (0 when the walk failed or the workspace holds
@@ -136,18 +158,19 @@ zbd_walk_kernel(const u8* __restrict__ src, u64 size, ZbdBlock* blocks, u32 capB
 /* ------------------------------------------------------------------------------------------------ D0 for batch calls
  * The entries' header chains are independent of each other, so one thread walks each entry: a count pass, a scan that gives
  * every entry its place in the call's arrays, and a fill pass that walks again and writes the descriptors there, shifted
- * into the call's coordinates.  zbd_walk is the same function as everywhere else. */
+ * into the call's coordinates.  zbd_walk is the same function as everywhere else, with the entry's dictionary. */
 #define ZBD_ENTRY_THREADS 128
 #define ZBD_ENTRY_SCAN    1024        /* the one CTA of the entry scan and of the verdict */
 __global__ void __launch_bounds__(ZBD_ENTRY_THREADS)
 zbd_entries_count_kernel(const u8* __restrict__ src, const ZbdSpan* __restrict__ spans, ZbdEntry* __restrict__ entries, u32 nbEntries,
-                         u32 dictEntropy, u32 dictID)
+                         ZbdDicts dicts)
 {
     u32 const e = blockIdx.x * ZBD_ENTRY_THREADS + threadIdx.x;
     if (e >= nbEntries) return;
     ZbdSpan const s = spans[e];
+    const ZbdDictRef* const r = dicts.perEntry ? dicts.perEntry[e] : dicts.one;
     u32 nb = 0, nf = 0; u64 lit = 0, seq = 0;
-    u32 const err = zbd_walk(src + s.srcOff, s.srcSize, NULL, 0, NULL, 0, &nb, &nf, &lit, &seq, dictEntropy != 0u, dictID);
+    u32 const err = zbd_walk(src + s.srcOff, s.srcSize, NULL, 0, NULL, 0, &nb, &nf, &lit, &seq, r && r->di.entropy, r ? r->di.dictID : 0u);
     ZbdEntry E; memset(&E, 0, sizeof(E));
     E.status = err;
     if (!err) { E.nb = nb; E.nf = nf; E.lit = lit; E.seq = seq; }
@@ -232,7 +255,7 @@ zbd_entries_scan_kernel(const ZbdSpan* __restrict__ spans, ZbdEntry* __restrict_
  * from the entry's coordinates to the call's; every frame records its entry in frameEntry. */
 __global__ void __launch_bounds__(ZBD_ENTRY_THREADS)
 zbd_entries_fill_kernel(const u8* __restrict__ src, const ZbdSpan* __restrict__ spans, const ZbdEntry* __restrict__ entries, u32 nbEntries,
-                        ZbdBlock* __restrict__ blocks, ZbdFrame* __restrict__ frames, u32* __restrict__ frameEntry, u32 dictEntropy, u32 dictID,
+                        ZbdBlock* __restrict__ blocks, ZbdFrame* __restrict__ frames, u32* __restrict__ frameEntry, ZbdDicts dicts,
                         u64 litCap, u64 seqCap)
 {
     u32 const e = blockIdx.x * ZBD_ENTRY_THREADS + threadIdx.x;
@@ -242,8 +265,9 @@ zbd_entries_fill_kernel(const u8* __restrict__ src, const ZbdSpan* __restrict__ 
     ZbdSpan const s = spans[e];
     ZbdBlock* const B = blocks + E.block;
     ZbdFrame* const F = frames + E.frame;
+    const ZbdDictRef* const r = dicts.perEntry ? dicts.perEntry[e] : dicts.one;
     u32 nb = 0, nf = 0; u64 lit = 0, seq = 0;
-    zbd_walk(src + s.srcOff, s.srcSize, B, E.nb, F, E.nf, &nb, &nf, &lit, &seq, dictEntropy != 0u, dictID);   /* the count pass's walk: it succeeds */
+    zbd_walk(src + s.srcOff, s.srcSize, B, E.nb, F, E.nf, &nb, &nf, &lit, &seq, r && r->di.entropy, r ? r->di.dictID : 0u);   /* the count pass's walk: it succeeds */
     u64 const litMax = s.dstCap + 16u * (u64)E.nb, seqMax = s.dstCap / 3u;
     for (u32 k = 0; k < E.nb; k++) {
         ZbdBlock& b = B[k];
@@ -268,9 +292,9 @@ struct ZbdLitWork {
 };
 
 template <bool PERSISTENT>
-__global__ void __launch_bounds__(32 * ZBD_WARPS)
+__global__ void __launch_bounds__(32 * ZBD_WARPS, 9)             /* 9 CTAs: up to 56 registers (without it ptxas cuts <false> to 48, and its streams decode slower) */
 zbd_literals_kernel(const u8* __restrict__ src, const ZbdBlock* __restrict__ blocks, u32 nbBlocks, u8* __restrict__ lits, ZbdBlockOut* __restrict__ bout,
-                    const u8* __restrict__ dict, ZbdDictInfo di, const u64* __restrict__ res, u64 litCap)
+                    ZbdDicts dicts, const u32* __restrict__ frameEntry, const u64* __restrict__ res, u64 litCap)
 {
     __shared__ ZbdLitWork work[ZBD_WARPS];
     u32 const lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
@@ -285,7 +309,8 @@ zbd_literals_kernel(const u8* __restrict__ src, const ZbdBlock* __restrict__ blo
     if (b.litType == 1u) { u8 const v = c[b.litHdr]; for (u32 i = lane; i < b.litRegen; i += 32u) out[i] = v; return; }
     if (lane == 0) {
         u32 nbSym = 0, log = 0, dn = 0;
-        const u8* const dp = zbd_hufDescription(&b, blocks, src, dict, &di, &dn);
+        const ZbdDictRef* const r = b.hufSrc == ZBD_DICT ? zbd_dictOf(dicts, frameEntry, b.frame) : NULL;    /* the walk names ZBD_DICT only with a dictionary */
+        const u8* const dp = zbd_hufDescription(&b, blocks, src, r ? r->dict : NULL, r ? &r->di : NULL, &dn);
         u32 const used = zbd_readHufWeights(wk.weights, &nbSym, &log, dp, dn, wk.fse, wk.norm, wk.next);
         if (used) zbd_hufStarts(wk.start, wk.weights, nbSym, log);
         wk.nbSym = nbSym; wk.log = log; wk.used = used;
@@ -332,7 +357,7 @@ struct ZbdSeqWork {
 template <bool PERSISTENT>
 __global__ void __launch_bounds__(32 * ZBD_WARPS)
 zbd_sequences_kernel(const u8* __restrict__ src, const ZbdBlock* __restrict__ blocks, u32 nbBlocks, u64* __restrict__ seqs, ZbdBlockOut* __restrict__ bout,
-                     const u8* __restrict__ dict, ZbdDictInfo di, const u64* __restrict__ res, u64 seqCap)
+                     ZbdDicts dicts, const u32* __restrict__ frameEntry, const u64* __restrict__ res, u64 seqCap)
 {
     __shared__ ZbdSeqWork work[ZBD_WARPS];
     u32 const lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
@@ -345,7 +370,11 @@ zbd_sequences_kernel(const u8* __restrict__ src, const ZbdBlock* __restrict__ bl
         return;
     }
     /* three lanes: one decoding table each, from the section that defined it */
-    if (lane < 3u) wk.log[lane] = zbd_seqTable(wk.table[lane], wk.norm[lane], wk.next[lane], lane, &b, blocks, src, dict, &di);
+    if (lane < 3u) {
+        bool const fromDict = b.fseSrc[0] == ZBD_DICT || b.fseSrc[1] == ZBD_DICT || b.fseSrc[2] == ZBD_DICT;
+        const ZbdDictRef* const r = fromDict ? zbd_dictOf(dicts, frameEntry, b.frame) : NULL;
+        wk.log[lane] = zbd_seqTable(wk.table[lane], wk.norm[lane], wk.next[lane], lane, &b, blocks, src, r ? r->dict : NULL, r ? &r->di : NULL);
+    }
     __syncwarp();
     if (lane == 0) {
         ZbdBlockOut& o = bout[bi];
@@ -383,7 +412,7 @@ zbd_sequences_kernel(const u8* __restrict__ src, const ZbdBlock* __restrict__ bl
 template <bool ENTRIES>
 __global__ void __launch_bounds__(SCAN_THREADS)
 zbd_scan_kernel(const ZbdBlock* __restrict__ blocks, u32 nbBlocks, const ZbdFrame* __restrict__ frames, u32 nbFrames, ZbdBlockOut* __restrict__ bout,
-                u64 dstCapacity, u64* __restrict__ res, ZbdDictInfo di, const u64* __restrict__ walk, u32* __restrict__ classList, u32 capF,
+                u64 dstCapacity, u64* __restrict__ res, ZbdDicts dicts, const u64* __restrict__ walk, u32* __restrict__ classList, u32 capF,
                 const ZbdSpan* __restrict__ spans, ZbdEntry* __restrict__ entries, const u32* __restrict__ frameEntry, u32 nbEntries)
 {
     __shared__ u64 warpSum[SCAN_THREADS / 32];
@@ -431,7 +460,10 @@ zbd_scan_kernel(const ZbdBlock* __restrict__ blocks, u32 nbBlocks, const ZbdFram
         ZbdFrame const fr = frames[f];
         u64 const fOff = fr.nbBlocks ? bout[fr.firstBlock].dstOff : 0;
         ZbdRep h; h.r[0] = 1u; h.r[1] = 4u; h.r[2] = 8u;            /* format: "Repeat Offsets" start values */
-        if (di.entropy) { h.r[0] = di.rep[0]; h.r[1] = di.rep[1]; h.r[2] = di.rep[2]; }      /* ... or the dictionary's */
+        if (const ZbdDictRef* const r = zbd_dictOf(dicts, frameEntry, f)) {                  /* ... or the dictionary's */
+            u32 const e = r->di.entropy, r0 = r->di.rep[0], r1 = r->di.rep[1], r2 = r->di.rep[2];
+            if (e) { h.r[0] = r0; h.r[1] = r1; h.r[2] = r2; }
+        }
         for (u32 k0 = 0; k0 < fr.nbBlocks; k0 += 32u) {
             u32 const k = k0 + lane;
             ZbdRep tr; tr.r[0] = tr.r[1] = tr.r[2] = 0;
@@ -498,10 +530,10 @@ zbd_scan_kernel(const ZbdBlock* __restrict__ blocks, u32 nbBlocks, const ZbdFram
  * which never looks below a frame's first match). */
 #define ZBD_TILE_LOG 6u
 template <bool PERSISTENT, bool ENTRIES>
-__global__ void __launch_bounds__(32 * ZBD_WARPS)
+__global__ void __launch_bounds__(32 * ZBD_WARPS, 8)             /* 8 CTAs: up to 64 registers (without it ptxas spills <false, false> down to 48) */
 zbd_place_kernel(const u8* __restrict__ src, const ZbdBlock* __restrict__ blocks, u32 nbBlocks, const u8* __restrict__ lits, u64* __restrict__ seqs,
                  u64* __restrict__ matchPos, u32* __restrict__ tileFirst, const ZbdBlockOut* __restrict__ bout, u8* __restrict__ dst,
-                 const u8* __restrict__ dictContent, u32 dictContentSize, u32* __restrict__ execErr, const u64* __restrict__ res,
+                 ZbdDicts dicts, u32* __restrict__ execErr, const u64* __restrict__ res,
                  const u32* __restrict__ frameEntry, ZbdEntry* __restrict__ entries)
 {
     u32 const lane = threadIdx.x & 31u;
@@ -528,6 +560,8 @@ zbd_place_kernel(const u8* __restrict__ src, const ZbdBlock* __restrict__ blocks
     u64* const mp = matchPos + b.seqPos;
     ZbdRep rep = o.start;
     u64 const inFrame = o.dstOff - o.frameOff;                       /* bytes of the frame in front of this block */
+    const ZbdDictRef* const dict = zbd_dictOf(dicts, frameEntry, b.frame);
+    u64 const reach = inFrame + (dict ? dict->contentSize : 0u);    /* offsets reach back over the frame so far and the dictionary's content */
     u32 op = 0, lp = 0, err = 0, failedAt = 0;
     if (ENTRIES && entryFirst && lane == 0) atomicMin(&tileFirst[o.dstOff >> ZBD_TILE_LOG], gFirst);
     if (!ENTRIES && o.dstOff == 0 && lane == 0) tileFirst[0] = gFirst;
@@ -542,7 +576,7 @@ zbd_place_kernel(const u8* __restrict__ src, const ZbdBlock* __restrict__ blocks
             u32 const off = zbd_rep_apply(&rep, ob, ll, false);
             if (lane == j) { myOff = off; myOp = op; myLp = lp; }
             op += ll;
-            if (!err && (off == 0u || (u64)off > inFrame + op + dictContentSize)) { err = ZBD_CORRUPT; failedAt = i0 + j; }
+            if (!err && (off == 0u || (u64)off > reach + op)) { err = ZBD_CORRUPT; failedAt = i0 + j; }
             op += ml; lp += ll;
         }
         if (err) break;
@@ -556,7 +590,7 @@ zbd_place_kernel(const u8* __restrict__ src, const ZbdBlock* __restrict__ blocks
             u64 const here = inFrame + mpos;                          /* its frame position */
             if ((u64)myOff > here) {                                 /* begins in the dictionary: those bytes now, the rest is a match of the same offset */
                 u32 const fromDict = (u32)((u64)myOff - here) < myML ? (u32)((u64)myOff - here) : myML;
-                const u8* const dp = dictContent + dictContentSize - ((u64)myOff - here);
+                const u8* const dp = dict->dict + dict->di.contentOff + dict->contentSize - ((u64)myOff - here);
                 for (u32 k = 0; k < fromDict; k++) out[mpos + k] = dp[k];
                 mpos += fromDict; myML -= fromDict;
             }
@@ -799,11 +833,15 @@ struct ZSTD_DDict_s {
     const u8* bytes;               /* the whole dictionary: that copy, or the caller's buffer */
     size_t size;
     ZbdDictInfo di;
-    mutable std::mutex lock;       /* guards the device state below */
+    mutable std::mutex lock;       /* guards the device state below; residentOn is also read without it */
     mutable int device;            /* -1 until the device buffer exists */
-    mutable bool resident;         /* uploaded since the digest */
-    mutable ZbDevBuf<u8> d_dict;
+    mutable std::atomic<int> residentOn;   /* the device the digest has been uploaded to, -1 until then; set once the upload completed */
+    mutable ZbDevBuf<u8> d_dict;   /* the bytes, then (at zbd_refOffset) the descriptor */
+    mutable ZbdDictRef ref;        /* the descriptor's host image, the source of its upload */
 };
+static size_t zbd_refOffset(size_t dictSize) { return (dictSize + 15) & ~(size_t)15; }
+/* the device descriptor of a DDict resident on the device in question */
+static const ZbdDictRef* zbd_ref(const ZSTD_DDict* dd) { return (const ZbdDictRef*)((const u8*)dd->d_dict + zbd_refOffset(dd->size)); }
 struct ZbdDDictFree { void operator()(ZSTD_DDict* dd) const { ZSTD_freeDDict(dd); } };
 typedef std::unique_ptr<ZSTD_DDict, ZbdDDictFree> ZbdDDictPtr;
 enum ZbdDictUses { ZBD_DICT_DONT_USE, ZBD_DICT_USE_ONCE, ZBD_DICT_USE_ALWAYS };    /* ZSTD_dictUses_e, zstd_decompress_internal.h */
@@ -840,6 +878,8 @@ struct ZSTD_DCtx_s {
      * d_verdict holds a synchronous call's result and sizes for its one read-back into h_verdict */
     ZbDevBuf<ZbdSpan> d_spans; ZbDevBuf<ZbdEntry> d_entries; ZbDevBuf<u32> d_frameEntry;   /* the entry of every frame */
     ZbHostBuf<ZbdSpan> stage[ZSTDB200_ASYNC_SLOTS]; bool stageBusy[ZSTDB200_ASYNC_SLOTS]; u32 stageNext; ZbEvents evStage;
+    /* calls with a DDict per entry: the entries' dictionary references, staged in the same slots as the spans */
+    ZbDevBuf<const ZbdDictRef*> d_refs; ZbHostBuf<const ZbdDictRef*> stageRefs[ZSTDB200_ASYNC_SLOTS];
     ZbDevBuf<unsigned long long> d_verdict; ZbHostBuf<unsigned long long> h_verdict;
 };
 
@@ -907,34 +947,38 @@ static ZbdDictInfo zbd_dictInfo(const ZSTD_DDict* dd)
     return di;
 }
 
+/* the kernels' dictionary for a call with one: dd's descriptor (dd resident on the context's device), or none */
+static ZbdDicts zbd_oneDict(const ZSTD_DDict* dd)
+{
+    ZbdDicts ds = { dd ? zbd_ref(dd) : NULL, NULL };
+    return ds;
+}
+
 /* D1 .. D4 over descriptors that are already on the device, with the resident dictionary dd (NULL: none); returns the
  * output size */
 static size_t zbd_run(ZSTD_DCtx* d, u8* d_dst, size_t dstCapacity, const u8* d_src, u32 nb, u32 nf, u64 seqCount, const ZSTD_DDict* dd,
                       cudaStream_t st)
 {
-    ZbdDictInfo const di = zbd_dictInfo(dd);
-    const u8* const d_dict = dd ? (const u8*)dd->d_dict : (const u8*)NULL;
+    ZbdDicts const ds = zbd_oneDict(dd);
     CK(cudaMemsetAsync(d->d_execErr, 0, sizeof(u32), st));
     CK(cudaEventRecord(d->ev[1], st));
     u32 const grid = (nb + ZBD_WARPS - 1u) / ZBD_WARPS;
-    zbd_literals_kernel<false><<<grid, 32 * ZBD_WARPS, 0, st>>>(d_src, d->d_blocks, nb, d->d_lits, d->d_bout, d_dict, di, NULL, 0);
+    zbd_literals_kernel<false><<<grid, 32 * ZBD_WARPS, 0, st>>>(d_src, d->d_blocks, nb, d->d_lits, d->d_bout, ds, NULL, NULL, 0);
     CK(cudaEventRecord(d->ev[2], st));
-    zbd_sequences_kernel<false><<<grid, 32 * ZBD_WARPS, 0, st>>>(d_src, d->d_blocks, nb, d->d_seqs, d->d_bout, d_dict, di, NULL, 0);
+    zbd_sequences_kernel<false><<<grid, 32 * ZBD_WARPS, 0, st>>>(d_src, d->d_blocks, nb, d->d_seqs, d->d_bout, ds, NULL, NULL, 0);
     CK(cudaEventRecord(d->ev[3], st));
-    zbd_scan_kernel<false><<<1, SCAN_THREADS, 0, st>>>(d->d_blocks, nb, d->d_frames, nf, d->d_bout, (u64)dstCapacity, d->d_res, di, NULL, NULL, 0, NULL, NULL, NULL, 0);
+    zbd_scan_kernel<false><<<1, SCAN_THREADS, 0, st>>>(d->d_blocks, nb, d->d_frames, nf, d->d_bout, (u64)dstCapacity, d->d_res, ds, NULL, NULL, 0, NULL, NULL, NULL, 0);
     CK(cudaMemcpyAsync(d->h_res, d->d_res, 2 * sizeof(u64), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));                                  /* nothing is written to dst before the sizes are known to fit */
     if (d->h_res[0]) return ZB_ERR((u32)d->h_res[0]);
     size_t const total = (size_t)d->h_res[1];
     CK(cudaEventRecord(d->ev[4], st));
-    u32 const dictContent = dd ? (u32)(dd->size - di.contentOff) : 0u;
-    const u8* const d_dictContent = dd ? d_dict + di.contentOff : (const u8*)NULL;
     TRY(zbd_reserve(d->d_tileFirst, (total >> ZBD_TILE_LOG) + 4));
     TRY(zbd_reserve(d->d_done, (size_t)seqCount + 4));
     CK(cudaMemsetAsync(d->d_tileFirst, 0xFF, ((total >> ZBD_TILE_LOG) + 4) * sizeof(u32), st));
     CK(cudaMemsetAsync(d->d_done, 0, (size_t)seqCount + 4, st));
     zbd_place_kernel<false, false><<<grid, 32 * ZBD_WARPS, 0, st>>>(d_src, d->d_blocks, nb, d->d_lits, d->d_seqs, d->d_matchPos, d->d_tileFirst, d->d_bout, d_dst,
-                                                             d_dictContent, dictContent, d->d_execErr, NULL, NULL, NULL);
+                                                             ds, d->d_execErr, NULL, NULL, NULL);
     CK(cudaEventRecord(d->ev[6], st));
     if (seqCount) {                                                  /* threads per frame by the matches a frame holds */
         u64 const perFrame = seqCount / (nf ? nf : 1u);
@@ -973,7 +1017,7 @@ static size_t zbd_ensure(ZSTD_DCtx* d, u32 nb, u32 nf, u64 litBytes, u64 seqCoun
  * bytes, or a prefix (rawContent) is raw content (zstd_ddict.c:95-107); a zstd-format one is parsed on the host. */
 static size_t zbd_digestDict(ZSTD_DDict* dd, const u8* dict, size_t size, bool rawContent)
 {
-    dd->bytes = dict; dd->size = dict ? size : 0; dd->resident = false;
+    dd->bytes = dict; dd->size = dict ? size : 0; dd->residentOn.store(-1);
     memset(&dd->di, 0, sizeof(dd->di));
     if (rawContent || dd->size == 0) return 0;
     u32 const e = zbd_parseDict(&dd->di, dict, size);
@@ -999,21 +1043,40 @@ static ZSTD_DDict* zbd_createDDict(const void* dict, size_t dictSize, bool byCop
     return dd;
 }
 
-/* Makes dd resident on `device`, the compressor's rule for a CDict (ZbRun::prepareDicts): the buffer is allocated on the first device that uses dd (one device
- * per DDict: another gets parameter_unsupported), the bytes are uploaded once per digest, and the upload has completed
- * before another context can use dd.  A resident DDict costs a call nothing: no copy, no synchronisation. */
-static size_t zbd_residentDict(const ZSTD_DDict* dd, int device, cudaStream_t st)
+/* Makes the DDicts dds[0 .. n) resident on `device`, the compressor's rule for a CDict (ZbRun::prepareDicts): a DDict's buffer is
+ * allocated on the first device that uses it (one device per DDict: another gets parameter_unsupported), its bytes and its
+ * descriptor are uploaded once per digest, and the upload has completed before another context can use it.  The uploads of
+ * all of them go out before one synchronisation.  Their locks are held until then, taken in address order, so that calls
+ * that name the same DDicts in other orders cannot deadlock; a DDict named twice counts once.  A resident DDict costs a call
+ * nothing: no copy, no synchronisation.  *uploaded (NULL: not wanted) grows by the bytes copied. */
+static size_t zbd_residentDicts(const ZSTD_DDict* const* dds, size_t n, int device, cudaStream_t st, size_t* uploaded)
 {
-    std::lock_guard<std::mutex> g(dd->lock);
-    if (dd->device >= 0 && dd->device != device) return ZB_ERR(ZB_error_parameter_unsupported);
-    if (dd->resident) return 0;
-    TRY(zbd_reserve(dd->d_dict, dd->size + 16));
-    dd->device = device;
-    CK(cudaMemcpyAsync(dd->d_dict, dd->bytes, dd->size, cudaMemcpyHostToDevice, st));
-    CK(cudaStreamSynchronize(st));                                    /* the source is pageable memory that may change after the call */
-    dd->resident = true;
+    std::vector<const ZSTD_DDict*> v(dds, dds + n);
+    std::sort(v.begin(), v.end());
+    v.erase(std::unique(v.begin(), v.end()), v.end());
+    std::vector<std::unique_lock<std::mutex>> locks;
+    locks.reserve(v.size());
+    for (const ZSTD_DDict* dd : v) locks.emplace_back(dd->lock);
+    std::vector<const ZSTD_DDict*> up;
+    for (const ZSTD_DDict* dd : v) {
+        if (dd->device >= 0 && dd->device != device) return ZB_ERR(ZB_error_parameter_unsupported);
+        if (dd->residentOn.load(std::memory_order_relaxed) != device) up.push_back(dd);
+    }
+    if (up.empty()) return 0;
+    for (const ZSTD_DDict* dd : up) {
+        size_t const at = zbd_refOffset(dd->size);
+        TRY(zbd_reserve(dd->d_dict, at + sizeof(ZbdDictRef)));
+        dd->device = device;
+        dd->ref.di = dd->di; dd->ref.dict = dd->d_dict; dd->ref.contentSize = (u32)(dd->size - dd->di.contentOff); dd->ref.pad = 0;
+        CK(cudaMemcpyAsync(dd->d_dict, dd->bytes, dd->size, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(dd->d_dict + at, &dd->ref, sizeof(ZbdDictRef), cudaMemcpyHostToDevice, st));
+        if (uploaded) *uploaded += dd->size + sizeof(ZbdDictRef);
+    }
+    CK(cudaStreamSynchronize(st));                                    /* the sources are pageable memory that may change after the call */
+    for (const ZSTD_DDict* dd : up) dd->residentOn.store(device, std::memory_order_release);
     return 0;
 }
+static size_t zbd_residentDict(const ZSTD_DDict* dd, int device, cudaStream_t st) { return zbd_residentDicts(&dd, 1, device, st, NULL); }
 
 /* dictionary bytes passed to a call, digested into the context's callDict */
 static size_t zbd_digestCallDict(ZSTD_DCtx* d, const void* dict, size_t dictSize)
@@ -1232,11 +1295,7 @@ __global__ void zbd_result_kernel(const u64* __restrict__ res, u32 capB, u32 cap
     *result = r;
 }
 
-static bool zbd_dictResident(const ZSTD_DDict* dd, int device)
-{
-    std::lock_guard<std::mutex> g(dd->lock);
-    return dd->resident && dd->device == device;
-}
+static bool zbd_dictResident(const ZSTD_DDict* dd, int device) { return dd->residentOn.load(std::memory_order_acquire) == device; }
 
 /* D0 .. D5 and the verdict enqueued on the caller's stream, with the context's sticky dictionary, under ZbOrder's rule; a DDict's
  * first upload on the device (on the context's stream, which synchronises) is refused under capture too */
@@ -1271,9 +1330,7 @@ static size_t zbd_decompressAsync(ZSTD_DCtx* d, void* dst, size_t dstCapacity, c
     }));
     if (dd) TRY(zbd_residentDict(dd, d->device, d->stream));           /* no copy once resident */
     ZbdDictInfo const di = zbd_dictInfo(dd);
-    const u8* const d_dict = dd ? (const u8*)dd->d_dict : (const u8*)NULL;
-    u32 const dictContent = dd ? (u32)(dd->size - di.contentOff) : 0u;
-    const u8* const d_dictContent = dd ? d_dict + di.contentOff : (const u8*)NULL;
+    ZbdDicts const ds = zbd_oneDict(dd);
     TRY(call.enter(st));
     const u8* const in = (const u8*)src;
     u64* const res = d->d_res;
@@ -1281,13 +1338,13 @@ static size_t zbd_decompressAsync(ZSTD_DCtx* d, void* dst, size_t dstCapacity, c
     auto grid = [&](int k, u32 most) { return d->grid[k] < most ? d->grid[k] : most; };
     CK(cudaMemsetAsync(d->d_execErr, 0, sizeof(u32), st));
     zbd_walk_kernel<<<1, ZBD_WALK_THREADS, 0, st>>>(in, (u64)srcSize, d->d_blocks, capB, d->d_frames, capF, res, di.entropy, di.dictID);
-    zbd_literals_kernel<true><<<grid(0, blockGrid), 32 * ZBD_WARPS, 0, st>>>(in, d->d_blocks, capB, d->d_lits, d->d_bout, d_dict, di, res, litCap);
-    zbd_sequences_kernel<true><<<grid(1, blockGrid), 32 * ZBD_WARPS, 0, st>>>(in, d->d_blocks, capB, d->d_seqs, d->d_bout, d_dict, di, res, seqCap);
-    zbd_scan_kernel<false><<<1, SCAN_THREADS, 0, st>>>(d->d_blocks, capB, d->d_frames, capF, d->d_bout, (u64)dstCapacity, res + ZBD_RES_SCAN, di, res,
+    zbd_literals_kernel<true><<<grid(0, blockGrid), 32 * ZBD_WARPS, 0, st>>>(in, d->d_blocks, capB, d->d_lits, d->d_bout, ds, NULL, res, litCap);
+    zbd_sequences_kernel<true><<<grid(1, blockGrid), 32 * ZBD_WARPS, 0, st>>>(in, d->d_blocks, capB, d->d_seqs, d->d_bout, ds, NULL, res, seqCap);
+    zbd_scan_kernel<false><<<1, SCAN_THREADS, 0, st>>>(d->d_blocks, capB, d->d_frames, capF, d->d_bout, (u64)dstCapacity, res + ZBD_RES_SCAN, ds, res,
                                                        d->d_class, capF, NULL, NULL, NULL, 0);
     zbd_clear_kernel<<<grid(3, (u32)(seqCap / 256u) + 1u), 256, 0, st>>>(res, d->d_tileFirst, d->d_done);
     zbd_place_kernel<true, false><<<grid(2, blockGrid), 32 * ZBD_WARPS, 0, st>>>(in, d->d_blocks, capB, d->d_lits, d->d_seqs, d->d_matchPos, d->d_tileFirst, d->d_bout,
-                                                                           (u8*)dst, d_dictContent, dictContent, d->d_execErr, res, NULL, NULL);
+                                                                           (u8*)dst, ds, d->d_execErr, res, NULL, NULL);
     zbd_matches_list_kernel<1024, false><<<grid(4, capF), 1024, 0, st>>>(d->d_blocks, d->d_frames, d->d_seqs, d->d_matchPos, d->d_tileFirst, (u8*)dst, d->d_done,
                                                             d->d_execErr, d->d_class, res, 0, NULL, NULL);
     zbd_matches_list_kernel<128, false><<<grid(5, capF), 128, 0, st>>>(d->d_blocks, d->d_frames, d->d_seqs, d->d_matchPos, d->d_tileFirst, (u8*)dst, d->d_done,
@@ -1331,9 +1388,23 @@ zbd_entries_result_kernel(const ZbdEntry* __restrict__ entries, u32 nbEntries, u
     if (threadIdx.x == 0) *result = firstBad != 0xFFFFFFFFu ? (unsigned long long)ZB_ERR(entries[firstBad].status) : total;
 }
 
-/* ownVerdict: the result and sizes go to the context's d_verdict (the synchronous call) instead of result / sizes */
+/* Entry i's dictionary reference for a batch call with a DDict per entry: *ref = dd's descriptor when dd is resident on
+ * `device`, NULL for no dictionary (dd NULL or empty).  Returns 0, 1 when dd is not resident yet, or parameter_unsupported
+ * when it is resident on another device.  No lock: residentOn is set once the upload has completed. */
+static size_t zbd_entryRef(const ZSTD_DDict* dd, int device, const ZbdDictRef** ref)
+{
+    *ref = NULL;
+    if (!dd || dd->size == 0) return 0;                               /* an empty dictionary is none */
+    int const on = dd->residentOn.load(std::memory_order_acquire);
+    if (on == device) { *ref = zbd_ref(dd); return 0; }
+    return on >= 0 ? ZB_ERR(ZB_error_parameter_unsupported) : 1;
+}
+
+/* ownVerdict: the result and sizes go to the context's d_verdict (the synchronous call) instead of result / sizes.
+ * perEntryDicts: entry i is decoded with ddicts[i] (ddicts NULL: no dictionary for any), not with the sticky dictionary */
 static size_t zbd_decompressFrames(ZSTD_DCtx* d, u8* dst, size_t dstCapacity, const size_t* dstOffsets, const size_t* dstCapacities,
                                    const u8* src, size_t srcSize, const size_t* srcOffsets, const size_t* srcSizes, size_t n,
+                                   bool perEntryDicts, const ZSTD_DDict* const* ddicts,
                                    unsigned long long* sizes, unsigned long long* result, bool ownVerdict, cudaStream_t st)
 {
     if (!d || (!result && !ownVerdict)) return ZB_ERR(ZB_error_GENERIC);
@@ -1351,7 +1422,7 @@ static size_t zbd_decompressFrames(ZSTD_DCtx* d, u8* dst, size_t dstCapacity, co
     TRY(call.begin(d->device, st));
     TRY(zbd_ctxInit(d));
     memset(&d->stats, 0, sizeof(d->stats));
-    const ZSTD_DDict* dd = zbd_getDDict(d);
+    const ZSTD_DDict* dd = perEntryDicts ? NULL : zbd_getDDict(d);    /* a call with a dictionary per entry leaves the sticky one as it is */
     if (dd && dd->size == 0) dd = NULL;                               /* an empty dictionary is none */
     if (dd && call.capturing && !zbd_dictResident(dd, d->device)) return ZB_ERR(ZB_error_stage_wrong);
     u64 const cap = zbd_asyncBlocks(srcSize, dstCapacity) + (u64)n;
@@ -1373,14 +1444,16 @@ static size_t zbd_decompressFrames(ZSTD_DCtx* d, u8* dst, size_t dstCapacity, co
         TRY(d->evStage.ensure(ZSTDB200_ASYNC_SLOTS, false));
         for (u32 s = 0; s < ZSTDB200_ASYNC_SLOTS; s++)               /* every slot, so that any can serve a capture */
             if (d->stage[s].cap < slots) { TRY(d->stage[s].ensure(slots, slots / 8 + 64)); d->stageBusy[s] = false; }
+        if (perEntryDicts) {
+            TRY(zbd_reserve(d->d_refs, slots));
+            for (u32 s = 0; s < ZSTDB200_ASYNC_SLOTS; s++)
+                if (d->stageRefs[s].cap < slots) { TRY(d->stageRefs[s].ensure(slots, slots / 8 + 64)); d->stageBusy[s] = false; }
+        }
         if (ownVerdict) { TRY(zbd_reserve(d->d_verdict, slots + 1)); TRY(d->h_verdict.ensure(slots + 1, slots / 8 + 64)); }
         return 0;
     }));
     if (dd) TRY(zbd_residentDict(dd, d->device, d->stream));           /* no copy once resident */
-    ZbdDictInfo const di = zbd_dictInfo(dd);
-    const u8* const d_dict = dd ? (const u8*)dd->d_dict : (const u8*)NULL;
-    u32 const dictContent = dd ? (u32)(dd->size - di.contentOff) : 0u;
-    const u8* const d_dictContent = dd ? d_dict + di.contentOff : (const u8*)NULL;
+    ZbdDicts ds = zbd_oneDict(dd);
     if (ownVerdict) { result = d->d_verdict; sizes = sizes ? d->d_verdict + 1 : NULL; }
     /* the spans, into the next slot of the ring; under capture the wait needs the relaxed mode (the event was recorded outside the graph) */
     u32 const slot = d->stageNext;
@@ -1395,23 +1468,41 @@ static size_t zbd_decompressFrames(ZSTD_DCtx* d, u8* dst, size_t dstCapacity, co
     }
     ZbdSpan* const h = d->stage[slot];
     for (size_t i = 0; i < n; i++) { h[i].srcOff = srcOffsets[i]; h[i].srcSize = srcSizes[i]; h[i].dstOff = dstOffsets[i]; h[i].dstCap = dstCapacities[i]; }
+    if (perEntryDicts) {
+        /* the entries' references, into the same slot.  A resident DDict costs one atomic read; the DDicts that are not resident
+         * yet are made resident together, with one synchronisation, then every reference is taken again. */
+        const ZbdDictRef** const hr = d->stageRefs[slot];
+        std::vector<const ZSTD_DDict*> cold;
+        for (size_t i = 0; i < n; i++) {
+            size_t const r = zbd_entryRef(ddicts ? ddicts[i] : NULL, d->device, &hr[i]);
+            if (zb_isErr(r)) return r;
+            if (r) cold.push_back(ddicts[i]);
+        }
+        if (!cold.empty()) {
+            if (call.capturing) return ZB_ERR(ZB_error_stage_wrong);
+            TRY(zbd_residentDicts(cold.data(), cold.size(), d->device, d->stream, &d->stats.h2d_bytes));
+            for (size_t i = 0; i < n; i++) if (zbd_entryRef(ddicts[i], d->device, &hr[i])) return ZB_ERR(ZB_error_GENERIC);
+        }
+        ds.perEntry = d->d_refs;
+    }
     TRY(call.enter(st));
     if (n) CK(cudaMemcpyAsync(d->d_spans, h, n * sizeof(ZbdSpan), cudaMemcpyHostToDevice, st));
+    if (n && perEntryDicts) CK(cudaMemcpyAsync(d->d_refs, d->stageRefs[slot], n * sizeof(const ZbdDictRef*), cudaMemcpyHostToDevice, st));
     if (!call.capturing) { CK(cudaEventRecord(d->evStage[slot], st)); d->stageBusy[slot] = true; }
     u64* const res = d->d_res;
     u32 const blockGrid = (capB + ZBD_WARPS - 1u) / ZBD_WARPS, entryGrid = (nbEntries + ZBD_ENTRY_THREADS - 1u) / ZBD_ENTRY_THREADS + (n == 0);
     auto grid = [&](int k, u32 most) { return d->grid[k] < most ? d->grid[k] : most; };
-    zbd_entries_count_kernel<<<entryGrid, ZBD_ENTRY_THREADS, 0, st>>>(src, d->d_spans, d->d_entries, nbEntries, di.entropy, di.dictID);
+    zbd_entries_count_kernel<<<entryGrid, ZBD_ENTRY_THREADS, 0, st>>>(src, d->d_spans, d->d_entries, nbEntries, ds);
     zbd_entries_scan_kernel<<<1, ZBD_ENTRY_SCAN, 0, st>>>(d->d_spans, d->d_entries, nbEntries, capB, capF, res);
     zbd_entries_fill_kernel<<<entryGrid, ZBD_ENTRY_THREADS, 0, st>>>(src, d->d_spans, d->d_entries, nbEntries, d->d_blocks, d->d_frames, d->d_frameEntry,
-                                                                     di.entropy, di.dictID, litCap, seqCap);
-    zbd_literals_kernel<true><<<grid(0, blockGrid), 32 * ZBD_WARPS, 0, st>>>(src, d->d_blocks, capB, d->d_lits, d->d_bout, d_dict, di, res, litCap);
-    zbd_sequences_kernel<true><<<grid(1, blockGrid), 32 * ZBD_WARPS, 0, st>>>(src, d->d_blocks, capB, d->d_seqs, d->d_bout, d_dict, di, res, seqCap);
-    zbd_scan_kernel<true><<<1, SCAN_THREADS, 0, st>>>(d->d_blocks, capB, d->d_frames, capF, d->d_bout, (u64)dstCapacity, res + ZBD_RES_SCAN, di, res,
+                                                                     ds, litCap, seqCap);
+    zbd_literals_kernel<true><<<grid(0, blockGrid), 32 * ZBD_WARPS, 0, st>>>(src, d->d_blocks, capB, d->d_lits, d->d_bout, ds, d->d_frameEntry, res, litCap);
+    zbd_sequences_kernel<true><<<grid(1, blockGrid), 32 * ZBD_WARPS, 0, st>>>(src, d->d_blocks, capB, d->d_seqs, d->d_bout, ds, d->d_frameEntry, res, seqCap);
+    zbd_scan_kernel<true><<<1, SCAN_THREADS, 0, st>>>(d->d_blocks, capB, d->d_frames, capF, d->d_bout, (u64)dstCapacity, res + ZBD_RES_SCAN, ds, res,
                                                       d->d_class, capF, d->d_spans, d->d_entries, d->d_frameEntry, nbEntries);
     zbd_clear_kernel<<<grid(3, (u32)(seqCap / 256u) + 1u), 256, 0, st>>>(res, d->d_tileFirst, d->d_done);
     zbd_place_kernel<true, true><<<grid(2, blockGrid), 32 * ZBD_WARPS, 0, st>>>(src, d->d_blocks, capB, d->d_lits, d->d_seqs, d->d_matchPos, d->d_tileFirst,
-                                                                              d->d_bout, dst, d_dictContent, dictContent, d->d_execErr, res, d->d_frameEntry,
+                                                                              d->d_bout, dst, ds, d->d_execErr, res, d->d_frameEntry,
                                                                               d->d_entries);
     zbd_matches_list_kernel<1024, true><<<grid(4, capF), 1024, 0, st>>>(d->d_blocks, d->d_frames, d->d_seqs, d->d_matchPos, d->d_tileFirst, dst, d->d_done,
                                                                         d->d_execErr, d->d_class, res, 0, d->d_frameEntry, d->d_entries);
@@ -1431,13 +1522,22 @@ extern "C" size_t ZSTDB200_decompressFramesAsync(ZSTD_DCtx* d, void* d_dst, size
                                                  size_t nbEntries, unsigned long long* d_dSizes, unsigned long long* d_result, void* stream)
 {
     return zbd_decompressFrames(d, (u8*)d_dst, dstCapacity, dstOffsets, dstCapacities, (const u8*)d_src, srcSize, srcOffsets, srcSizes, nbEntries,
-                                d_dSizes, d_result, false, (cudaStream_t)stream);
+                                false, NULL, d_dSizes, d_result, false, (cudaStream_t)stream);
+}
+extern "C" size_t ZSTDB200_decompressFramesAsync_usingDDicts(ZSTD_DCtx* d, void* d_dst, size_t dstCapacity, const size_t* dstOffsets,
+                                                             const size_t* dstCapacities, const void* d_src, size_t srcSize,
+                                                             const size_t* srcOffsets, const size_t* srcSizes, size_t nbEntries,
+                                                             const ZSTD_DDict* const* ddicts, unsigned long long* d_dSizes,
+                                                             unsigned long long* d_result, void* stream)
+{
+    return zbd_decompressFrames(d, (u8*)d_dst, dstCapacity, dstOffsets, dstCapacities, (const u8*)d_src, srcSize, srcOffsets, srcSizes, nbEntries,
+                                true, ddicts, d_dSizes, d_result, false, (cudaStream_t)stream);
 }
 
 /* the stream-ordered call on the caller's stream (NULL: the context's), then one read-back of the verdict and the sizes */
-extern "C" size_t ZSTDB200_decompressFrames(ZSTD_DCtx* d, void* d_dst, size_t dstCapacity, const size_t* dstOffsets, const size_t* dstCapacities,
-                                            const void* d_src, size_t srcSize, const size_t* srcOffsets, const size_t* srcSizes,
-                                            size_t nbEntries, size_t* dSizes, void* stream)
+static size_t zbd_decompressFramesSync(ZSTD_DCtx* d, void* d_dst, size_t dstCapacity, const size_t* dstOffsets, const size_t* dstCapacities,
+                                       const void* d_src, size_t srcSize, const size_t* srcOffsets, const size_t* srcSizes,
+                                       size_t nbEntries, bool perEntryDicts, const ZSTD_DDict* const* ddicts, size_t* dSizes, void* stream)
 {
     if (!d) return ZB_ERR(ZB_error_GENERIC);
     ZbDeviceGuard guard;
@@ -1445,12 +1545,27 @@ extern "C" size_t ZSTDB200_decompressFrames(ZSTD_DCtx* d, void* d_dst, size_t ds
     cudaStream_t const st = stream ? (cudaStream_t)stream : (cudaStream_t)d->stream;
     unsigned long long marker = 0;                                    /* non-NULL: the sizes are wanted */
     TRY(zbd_decompressFrames(d, (u8*)d_dst, dstCapacity, dstOffsets, dstCapacities, (const u8*)d_src, srcSize, srcOffsets, srcSizes, nbEntries,
-                             dSizes ? &marker : NULL, NULL, true, st));
+                             perEntryDicts, ddicts, dSizes ? &marker : NULL, NULL, true, st));
     size_t const words = 1 + (dSizes ? nbEntries : 0);
     CK(cudaMemcpyAsync(d->h_verdict, d->d_verdict, words * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     for (size_t i = 0; dSizes && i < nbEntries; i++) dSizes[i] = (size_t)d->h_verdict[1 + i];
     return (size_t)d->h_verdict[0];
+}
+extern "C" size_t ZSTDB200_decompressFrames(ZSTD_DCtx* d, void* d_dst, size_t dstCapacity, const size_t* dstOffsets, const size_t* dstCapacities,
+                                            const void* d_src, size_t srcSize, const size_t* srcOffsets, const size_t* srcSizes,
+                                            size_t nbEntries, size_t* dSizes, void* stream)
+{
+    return zbd_decompressFramesSync(d, d_dst, dstCapacity, dstOffsets, dstCapacities, d_src, srcSize, srcOffsets, srcSizes, nbEntries,
+                                    false, NULL, dSizes, stream);
+}
+extern "C" size_t ZSTDB200_decompressFrames_usingDDicts(ZSTD_DCtx* d, void* d_dst, size_t dstCapacity, const size_t* dstOffsets,
+                                                        const size_t* dstCapacities, const void* d_src, size_t srcSize,
+                                                        const size_t* srcOffsets, const size_t* srcSizes, size_t nbEntries,
+                                                        const ZSTD_DDict* const* ddicts, size_t* dSizes, void* stream)
+{
+    return zbd_decompressFramesSync(d, d_dst, dstCapacity, dstOffsets, dstCapacities, d_src, srcSize, srcOffsets, srcSizes, nbEntries,
+                                    true, ddicts, dSizes, stream);
 }
 
 /* ------------------------------------------------------------------------------------------------ one-shot calls */

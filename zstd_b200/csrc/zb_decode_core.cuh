@@ -504,7 +504,7 @@ ZBD_HD u32 zbd_rep_apply(ZbdRep* h, u32 offBase, u32 ll, bool symbolic)
     u32 const idx = offBase - 1u + (ll == 0u ? 1u : 0u);          /* 0, 1, 2, or 3 = "first offset minus one" */
     if (idx == 0u) return h->r[0];
     if (idx == 3u) off = (symbolic && ZBD_IS_SYM(h->r[0])) ? h->r[0] + 1u : h->r[0] - 1u;     /* symbolic: the low 28 bits count what is subtracted */
-    else off = h->r[idx];
+    else { off = h->r[1]; if (idx == 2u) off = h->r[2]; }              /* selected, not indexed: h stays in registers */
     if (idx != 1u) h->r[2] = h->r[1];
     h->r[1] = h->r[0]; h->r[0] = off;
     return off;
@@ -513,7 +513,8 @@ ZBD_HD u32 zbd_rep_apply(ZbdRep* h, u32 offBase, u32 ll, bool symbolic)
 ZBD_HD u32 zbd_rep_resolve(u32 v, const ZbdRep* start)
 {
     u32 const k = ZBD_IS_SYM(v);
-    return k ? start->r[k - 1u] - (v & 0x0FFFFFFFu) : v;
+    u32 const r = k == 1u ? start->r[0] : (k == 2u ? start->r[1] : start->r[2]);      /* selected, not indexed: the history stays in registers */
+    return k ? r - (v & 0x0FFFFFFFu) : v;
 }
 
 /* decoded sequence: offBase (28 bits) | litLength (18 bits) << 28 | matchLength (18 bits) << 46 */
