@@ -170,6 +170,25 @@ ZSTDB200_API size_t ZSTD_sequenceBound(size_t srcSize);                         
 ZSTDB200_API size_t ZSTD_mergeBlockDelimiters(ZSTD_Sequence* sequences, size_t seqsSize);   /* zstd_compress.c:3497, host code */
 ZSTDB200_API size_t ZSTD_compressSequences(ZSTD_CCtx* cctx, void* dst, size_t dstSize, const ZSTD_Sequence* inSeqs, size_t inSeqsSize,
                                            const void* src, size_t srcSize);
+/* lib/zstd.h:1594 — the parse of the frame ZSTD_compress2 writes for src on this context: the sticky level, the loaded
+ * dictionary or referenced CDict (whose level then applies) and the same blocks of min(128 KiB, window) bytes.  For every
+ * block of that frame, in order: its sequences, then a delimiter {offset 0, litLength = the block's trailing literals,
+ * matchLength 0, rep 0}.  A sequence's offset is the real distance (it may reach into the dictionary's content); rep is the
+ * repcode 1-3 the frame codes it with, 0 for a directly coded offset, with the reference's convention (a sequence without
+ * literals shifts the repcodes, zstd_compress.c:3411-3428).  The repcode history is {1,4,8} (or the dictionary's) at the
+ * frame's first block and unknown at every other, as for ZSTD_compressSequences, so rep is non-zero only where this frame
+ * really uses a repcode.  Feeding the output back to ZSTD_compressSequences with ZSTD_sf_explicitBlockDelimiters (or, after
+ * ZSTD_mergeBlockDelimiters, with ZSTD_sf_noBlockDelimiters) and the same level, dictionary and flags gives ZSTD_compress2's
+ * frame byte for byte.  Checksum, dictID and content-size flags do not change the output; nbWorkers is ignored as
+ * everywhere here.  An empty input gives 0 sequences; ZSTD_sequenceBound(srcSize) rows always suffice.
+ * Returns the number of sequences written, or an error code: dstSize_tooSmall (70) when they do not fit in outSeqsSize,
+ * dstBuffer_null (74) for a NULL outSeqs with a non-zero size, parameter_unsupported (40) with long-distance matching on,
+ * with a prefix pending (it stays pending) or for a level above 4 under ZSTDB200_setStrictLevels(1), GENERIC (1) without a
+ * device.  The GPU runs the match finder; only the input goes up and only the rows written come back.
+ * Two deliberate differences from the reference, which marks its version "for debugging only": a block below 7 bytes is
+ * one delimiter carrying its size (the reference fails there with sequenceProducer_failed), and on dstSize_tooSmall
+ * outSeqs is left untouched (the reference writes a prefix). */
+ZSTDB200_API size_t ZSTD_generateSequences(ZSTD_CCtx* cctx, ZSTD_Sequence* outSeqs, size_t outSeqsSize, const void* src, size_t srcSize);
 
 /* lib/zstd.h:236,242-246,114-120 ; lib/zstd_errors.h:106 */
 ZSTDB200_API size_t      ZSTD_compressBound(size_t srcSize);
@@ -443,6 +462,20 @@ ZSTDB200_API size_t ZSTDB200_CCtx_refPrefixDevice(ZSTD_CCtx* cctx, const void* d
 ZSTDB200_API size_t ZSTDB200_compressSequencesDevice(ZSTD_CCtx* cctx, void* d_dst, size_t dstCapacity,
                                                      const ZSTD_Sequence* d_seqs, size_t nbSeqs,
                                                      const void* d_src, size_t srcSize, void* stream);
+
+/* ZSTD_generateSequences with input and output in device memory: the parse of the GPU match finder, handed over without a
+ * round trip through the host.  d_outSeqs must be 4-byte aligned (parameter_outOfBound (42) otherwise); no row at or past
+ * outSeqsCapacity is written.  The Async form follows ZSTDB200_compressDeviceAsync's contract word for word (stream
+ * semantics with NULL = the legacy default stream, waves for inputs of 256 MiB or more, ordering with the context's other
+ * calls, no host wait once sized, the staging ring, the capture precondition and stage_wrong (60)): *d_result receives the
+ * number of rows or an error code (dstSize_tooSmall (70) when they do not fit), in stream order.  The other form is that
+ * call plus one read-back of the verdict; its NULL stream means the context's own streams, as for ZSTDB200_compressDevice.
+ * Both refuse as ZSTD_generateSequences does, before anything is enqueued.  ZSTDB200_getLastStats: match_ms is the match
+ * finder, stitch_ms the export, literals_ms and sequences_ms are 0. */
+ZSTDB200_API size_t ZSTDB200_generateSequencesDevice(ZSTD_CCtx* cctx, ZSTD_Sequence* d_outSeqs, size_t outSeqsCapacity,
+                                                     const void* d_src, size_t srcSize, void* stream);
+ZSTDB200_API size_t ZSTDB200_generateSequencesDeviceAsync(ZSTD_CCtx* cctx, ZSTD_Sequence* d_outSeqs, size_t outSeqsCapacity,
+                                                          const void* d_src, size_t srcSize, unsigned long long* d_result, void* stream);
 
 /* One frame compressed by several GPUs (the reference's counterpart: the jobs of ZSTDMT, zstdmt_compress.c:1168-1227 —
  * every job reads an overlap of the input in front of it, only the first writes the frame header, only the last the end

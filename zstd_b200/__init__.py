@@ -122,6 +122,12 @@ def lib() -> ctypes.CDLL:
     L.ZSTD_sequenceBound.argtypes = [_sz]
     L.ZSTD_mergeBlockDelimiters.restype = _sz
     L.ZSTD_mergeBlockDelimiters.argtypes = [_vp, _sz]
+    L.ZSTD_generateSequences.restype = _sz
+    L.ZSTD_generateSequences.argtypes = [_vp, _vp, _sz, _vp, _sz]
+    L.ZSTDB200_generateSequencesDevice.restype = _sz
+    L.ZSTDB200_generateSequencesDevice.argtypes = [_vp, _vp, _sz, _vp, _sz, _vp]
+    L.ZSTDB200_generateSequencesDeviceAsync.restype = _sz
+    L.ZSTDB200_generateSequencesDeviceAsync.argtypes = [_vp, _vp, _sz, _vp, _sz, _vp, _vp]
     L.ZSTDB200_compressFrames_usingCDict.restype = _sz
     L.ZSTDB200_compressFrames_usingCDict.argtypes = [_vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, ctypes.c_int, _vp]
     L.ZSTDB200_compressDeviceAsync.restype = _sz
@@ -428,6 +434,27 @@ class ZSTD_CCtx:
         """ZSTDB200_compressSequencesDevice: sequences (nb_seqs x 16 bytes), input and output in device memory (ints, e.g.
         torch.Tensor.data_ptr()).  Returns the compressed size."""
         return _check(lib().ZSTDB200_compressSequencesDevice(self._h, d_dst, dst_capacity, d_seqs, nb_seqs, d_src, src_size, stream))
+
+    def generate_sequences(self, src):
+        """ZSTD_generateSequences: the parse of the frame compress2 writes for src, as an (n, 4) uint32 array of
+        (offset, litLength, matchLength, rep), every block closed by a delimiter (0, trailing literals, 0, 0)."""
+        import numpy as np
+        p, n, keep = _buf(src)
+        cap = sequence_bound(n)
+        out = np.zeros((cap, 4), dtype=np.uint32)
+        r = _check(lib().ZSTD_generateSequences(self._h, out.ctypes.data, cap, p, n))
+        return out[:r].copy()
+
+    def generate_sequences_device(self, d_out: int, capacity: int, d_src: int, src_size: int, stream: int = 0) -> int:
+        """ZSTDB200_generateSequencesDevice: the same rows into device memory (d_out: capacity x 16 bytes, 4-byte aligned;
+        ints, e.g. torch.Tensor.data_ptr()).  Returns the number of rows."""
+        return _check(lib().ZSTDB200_generateSequencesDevice(self._h, d_out, capacity, d_src, src_size, stream))
+
+    def generate_sequences_device_async(self, d_out: int, capacity: int, d_src: int, src_size: int, d_result: int,
+                                        stream: int = 0) -> None:
+        """ZSTDB200_generateSequencesDeviceAsync: generate_sequences_device enqueued on `stream` (0 = the legacy default
+        stream); the number of rows, or an error code, lands in the 8 bytes at d_result in stream order."""
+        _check(lib().ZSTDB200_generateSequencesDeviceAsync(self._h, d_out, capacity, d_src, src_size, d_result, stream))
 
     def stats(self) -> Stats:
         s = Stats()

@@ -346,6 +346,9 @@ struct ZbCall {
      * the order of `stream`, which is then the caller's also when NULL (the legacy default stream) */
     unsigned long long* result = nullptr; unsigned long long* d_cSizes = nullptr;
     const ZSTD_CDict* const* cdicts = nullptr;                    /* a dictionary per frame in place of cdict (NULL entries: none, at `level`) */
+    /* ZSTD_generateSequences: each wave ends with the export of K1's stores as ZSTD_Sequence rows into dst instead of K2..K4;
+     * dstCapacity counts rows */
+    bool sequences = false;
 };
 
 static int g_strictLevels = 0;
@@ -560,11 +563,12 @@ static size_t zb_runLdm(ZSTD_CCtx* c, const ZbPlan& P, const u8* d_src, const u8
     return 0;
 }
 
-/* K1..K3 for blocks [b0, b1) = chunks [c0, c1), block b0 in the first of `rows`; d_dicts: the call's dictionary table, or NULL */
+/* K1..K3 for blocks [b0, b1) = chunks [c0, c1), block b0 in the first of `rows`; d_dicts: the call's dictionary table, or NULL;
+ * matchOnly: K1 alone */
 static size_t zb_runBlocks(ZSTD_CCtx* c, const ZbPlan& P, const u8* d_src, const ZbDictSlot* d_dicts, u32 b0, u32 b1, u32 c0, u32 c1,
-                           const ZbWorkRows& rows, cudaStream_t stream, bool timed, unsigned* launches)
+                           const ZbWorkRows& rows, cudaStream_t stream, bool timed, unsigned* launches, bool matchOnly)
 {
-    for (int phase = 0; phase < 3; phase++) {
+    for (int phase = 0; phase < (matchOnly ? 1 : 3); phase++) {
         for (size_t g = 0; g < P.groups.size(); g++) {
             ZbGroup const& G = P.groups[g];
             u32 const lo = G.b0 > b0 ? G.b0 : b0, hi = G.b1 < b1 ? G.b1 : b1;
@@ -729,7 +733,7 @@ static ZbWaves zb_wavePlan(const ZSTD_CCtx* c, const ZbPlan& P, const ZbCall& a)
     size_t bound = 0;
     if (!a.deviceMemory) for (size_t f = 0; f < a.nbFrames; f++) {
         if (a.frameOffsets[f] + a.frameSizes[f] > W.inEnd) W.inEnd = a.frameOffsets[f] + a.frameSizes[f];
-        bound += ZSTD_compressBound(a.frameSizes[f]) + 32;
+        bound += a.sequences ? ZSTD_sequenceBound(a.frameSizes[f]) : ZSTD_compressBound(a.frameSizes[f]) + 32;
     }
     W.outCap = a.deviceMemory ? a.dstCapacity : (a.dstCapacity < bound ? a.dstCapacity : bound);
     return W;
@@ -838,7 +842,7 @@ struct ZbRun {
         /* wave streams are created on first use: every stream beyond the hardware queue count (8 by default) shares a
          * queue with another one, and a download queued behind another wave's kernels stalls the whole pipeline */
         if (!W.single) for (u32 s = 0; s < W.slots; s++) TRY(c->waveStream[s].ensure());
-        if (!a.deviceMemory) { TRY(c->d_in.ensure(W.inEnd + 16)); TRY(c->d_out.ensure(W.outCap + 16)); TRY(c->waveStream[ZB_WAVE_SLOTS_MAX].ensure()); }
+        if (!a.deviceMemory) { TRY(c->d_in.ensure(W.inEnd + 16)); TRY(c->d_out.ensure(W.outCap * (a.sequences ? sizeof(ZSTD_Sequence) : 1) + 16)); TRY(c->waveStream[ZB_WAVE_SLOTS_MAX].ensure()); }
         if (!P.ldm.empty()) TRY(zb_ldmBuffers(c, P));
         TRY(c->d_dicts.ensure(P.dicts.size())); TRY(c->d_imageChunks.ensure(P.cdicts.empty() ? 0 : P.slots.size()));   /* at most an image per entry */
         size_t const stageBytes = a.result ? zb_stageBytes(P) : 0;
@@ -897,11 +901,15 @@ struct ZbRun {
                 st = c->waveStream[w % W.slots];
                 CK(cudaStreamWaitEvent(st, c->evH2D[w], 0));
             }
-            err = zb_runBlocks(c, P, d_in, d_dicts, b0, b1, W.wc[w], W.wc[w + 1], rows, st, W.single && !async, &launches);
+            err = zb_runBlocks(c, P, d_in, d_dicts, b0, b1, W.wc[w], W.wc[w + 1], rows, st, W.single && !async, &launches, a.sequences);
             if (err) break;
             if (w > 0) CK(cudaStreamWaitEvent(st, c->evStitch[w - 1], 0));
-            CK(zb_launch_stitch(d_in, c->d_blocks + b0, b1 - b0, c->d_frames, &rows,
-                                c->d_outOffsets + b0, w > 0 ? c->d_totals + (w - 1) : NULL, c->d_totals + w, d_out, W.outCap, st));
+            if (a.sequences)                                      /* the rows are placed as the stitch places bytes, wave after wave */
+                CK(zb_launch_seqexport(c->d_blocks + b0, b1 - b0, d_dicts, &rows, c->d_outOffsets + b0, w > 0 ? c->d_totals + (w - 1) : NULL,
+                                       c->d_totals + w, d_out, W.outCap, st));
+            else
+                CK(zb_launch_stitch(d_in, c->d_blocks + b0, b1 - b0, c->d_frames, &rows,
+                                    c->d_outOffsets + b0, w > 0 ? c->d_totals + (w - 1) : NULL, c->d_totals + w, d_out, W.outCap, st));
             launches += 2;
             if (!W.single) CK(cudaEventRecord(c->evStitch[w], st));
             /* the wave's size goes to the host behind the event the next wave's stitch waits for: a store into mapped
@@ -963,9 +971,12 @@ struct ZbRun {
             cudaEventElapsedTime(&ms, c->ev[EV_K0], c->ev[EV_KEND]); c->stats.kernel_ms = ms;
             cudaEventElapsedTime(&ms, c->ev[EV_K0], c->ev[EV_K1]); c->stats.match_ms = ms;
             if (P.groups.size() == 1) { cudaEventElapsedTime(&ms, c->ev[EV_K0], c->ev[EV_MID]); c->stats.cand_ms = ms; cudaEventElapsedTime(&ms, c->ev[EV_MID], c->ev[EV_K1]); c->stats.parse_ms = ms; }
-            cudaEventElapsedTime(&ms, c->ev[EV_K1], c->ev[EV_K2]); c->stats.literals_ms = ms;
-            cudaEventElapsedTime(&ms, c->ev[EV_K2], c->ev[EV_K3]); c->stats.sequences_ms = ms;
-            cudaEventElapsedTime(&ms, c->ev[EV_K3], c->ev[EV_KEND]); c->stats.stitch_ms = ms;
+            if (a.sequences) { cudaEventElapsedTime(&ms, c->ev[EV_K1], c->ev[EV_KEND]); c->stats.stitch_ms = ms; }   /* K1, then the export */
+            else {
+                cudaEventElapsedTime(&ms, c->ev[EV_K1], c->ev[EV_K2]); c->stats.literals_ms = ms;
+                cudaEventElapsedTime(&ms, c->ev[EV_K2], c->ev[EV_K3]); c->stats.sequences_ms = ms;
+                cudaEventElapsedTime(&ms, c->ev[EV_K3], c->ev[EV_KEND]); c->stats.stitch_ms = ms;
+            }
         } else { cudaEventElapsedTime(&ms, c->ev[EV_START], c->ev[EV_END]); c->stats.kernel_ms = ms; }
         c->stats.total_ms = c->stats.kernel_ms;
         c->stats.launches = launches; c->stats.nbBlocks = (u32)P.blocks.size();
@@ -979,6 +990,15 @@ struct ZbRun {
         const u8* const src = (const u8*)a.src; u8* const dst = (u8*)a.dst;
         cudaStream_t const last = c->waveStream[(W.nbWaves - 1u) % W.slots];   /* ordered behind every earlier wave's stitch */
         if (!err) { CK(zb_launch_call_result(c->d_frames, (u32)a.nbFrames, c->d_outOffsets, c->d_totals + W.nbWaves - 1, a.dstCapacity, d_sizes, d_result, last)); launches++; }
+        if (a.sequences) {                                        /* one download of exactly the rows written, once the verdict is known */
+            CK(cudaEventRecord(c->ev[EV_END], last));
+            size_t const n = endSync(last, false);
+            if (zb_isErr(n)) return n;
+            if (n) CK(cudaMemcpyAsync(dst, d_out, n * sizeof(ZSTD_Sequence), cudaMemcpyDeviceToHost, last));
+            CK(cudaStreamSynchronize(last));
+            c->stats.d2h_bytes = n * sizeof(ZSTD_Sequence);
+            return n;
+        }
         std::vector<u64> xxh;
         if (a.checksum && !err) {
             xxh.resize(a.nbFrames);
@@ -1031,7 +1051,7 @@ static size_t zb_compress(ZSTD_CCtx* c, const ZbCall& a)
     if (P.unsupported) return ZB_ERR(ZB_error_parameter_unsupported);
     TRY(zb_checkDicts(c, P, a.nbFrames, call.capturing));
     ZbRun r{c, a, P, zb_wavePlan(c, P, a), (async || (a.deviceMemory && a.stream)) ? a.stream : c->stream};
-    r.timeline = !r.W.single && !async && getenv("ZSTDB200_TIMELINE") != NULL;
+    r.timeline = !r.W.single && !async && !a.sequences && getenv("ZSTDB200_TIMELINE") != NULL;
     TRY(call.size([&] { return r.sizeBuffers(); }));
     TRY(r.enqueue(call));
     return a.deviceMemory ? r.finishOrdered(call) : r.finishHost();
@@ -1562,6 +1582,43 @@ extern "C" size_t ZSTD_compressSequences(ZSTD_CCtx* c, void* dst, size_t dstCapa
                                          const void* src, size_t srcSize)                       /* zstd_compress.c:6858 */
 {
     return zb_compressSeqs(c, dst, dstCapacity, seqs, n, src, srcSize, false, NULL);
+}
+
+/* ZSTD_generateSequences (lib/zstd.h:1594) and its device forms: the parse of the frame ZSTD_compress2 writes for src on this
+ * context (sticky level, dictionary or CDict, block boundaries), run through the executor with the export as every wave's
+ * tail.  d_result: a stream-ordered call's verdict (NULL: synchronous). */
+static size_t zb_generateSeqs(ZSTD_CCtx* c, ZSTD_Sequence* out, size_t outCapacity, const void* src, size_t srcSize, bool deviceMemory,
+                              cudaStream_t stream, unsigned long long* d_result)
+{
+    if (outCapacity && !out) return ZB_ERR(ZB_error_dstBuffer_null);
+    if (deviceMemory && ((uintptr_t)out & 3u)) return ZB_ERR(ZB_error_parameter_outOfBound);    /* ZSTD_Sequence's alignment */
+    if (c->advLdm || c->advPrefix) return ZB_ERR(ZB_error_parameter_unsupported);   /* not exported yet; the prefix stays pending */
+    const ZSTD_CDict* const cd = c->advRefCDict ? c->advRefCDict : c->advLocalDict.get();
+    size_t const off = 0;
+    ZbCall a = { out, outCapacity, src, &off, &srcSize, 1, cd, c->advRefCDict ? c->advRefCDict->level : c->advLevel, NULL, deviceMemory,
+                 stream, false, false };                          /* the frame header's flags do not change the parse */
+    a.result = d_result; a.sequences = true;
+    return zb_compress(c, a);
+}
+
+extern "C" size_t ZSTD_generateSequences(ZSTD_CCtx* c, ZSTD_Sequence* outSeqs, size_t outSeqsSize, const void* src, size_t srcSize)
+{
+    if (!c) return ZB_ERR(ZB_error_GENERIC);
+    return zb_generateSeqs(c, outSeqs, outSeqsSize, src, srcSize, false, NULL, NULL);
+}
+
+extern "C" size_t ZSTDB200_generateSequencesDevice(ZSTD_CCtx* c, ZSTD_Sequence* d_outSeqs, size_t outSeqsCapacity, const void* d_src,
+                                                   size_t srcSize, void* stream)
+{
+    if (!c) return ZB_ERR(ZB_error_GENERIC);
+    return zb_generateSeqs(c, d_outSeqs, outSeqsCapacity, d_src, srcSize, true, (cudaStream_t)stream, NULL);
+}
+
+extern "C" size_t ZSTDB200_generateSequencesDeviceAsync(ZSTD_CCtx* c, ZSTD_Sequence* d_outSeqs, size_t outSeqsCapacity, const void* d_src,
+                                                        size_t srcSize, unsigned long long* d_result, void* stream)
+{
+    if (!c || !d_result) return ZB_ERR(ZB_error_GENERIC);
+    return zb_generateSeqs(c, d_outSeqs, outSeqsCapacity, d_src, srcSize, true, (cudaStream_t)stream, d_result);
 }
 
 extern "C" size_t ZSTDB200_compressSequencesDevice(ZSTD_CCtx* c, void* d_dst, size_t dstCapacity, const ZSTD_Sequence* d_seqs, size_t n,

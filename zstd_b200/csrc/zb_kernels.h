@@ -97,6 +97,13 @@ cudaError_t zb_launch_stitch(const u8* d_src, const ZbBlock* d_blocks, u32 nbBlo
                              u64* d_outOffsets, const u64* d_base, u64* d_total,
                              u8* d_dst, u64 dstCapacity, cudaStream_t stream);
 cudaError_t zb_launch_checksums(const u8* d_src, const ZbFrame* d_frames, u32 nbFrames, const u64* d_outOffsets, u8* d_dst, u64 dstCapacity, cudaStream_t stream);
+/* The tail of a ZSTD_generateSequences wave in place of K2..K4 (zb_seqexport.cu): K1c's stores of the wave's blocks, from the
+ * seqs and meta rows, as ZSTD_Sequence rows at d_out (4-byte aligned): each block's sequences with real offsets and the
+ * repcode the block codes them with (history: d_dicts[dictSlot].codeRep at a frame's first block, {1,4,8} without a
+ * table, unknown elsewhere), then its delimiter {0, trailing literals, 0, 0}.  d_offsets gets nbBlocks + 1 row indices,
+ * starting at *d_base (NULL = 0); *d_total the running count after this wave.  No row at or past `capacity` is written. */
+cudaError_t zb_launch_seqexport(const ZbBlock* d_blocks, u32 nbBlocks, const ZbDictSlot* d_dicts, const ZbWorkRows* rows,
+                                u64* d_offsets, const u64* d_base, u64* d_total, void* d_out, u64 capacity, cudaStream_t stream);
 /* the last kernel of a call: d_cSizes[f] (d_cSizes may be NULL) and *d_result = *d_total, or dstSize_tooSmall
  * when *d_total > dstCapacity; d_total NULL (no frames): 0 */
 cudaError_t zb_launch_call_result(const ZbFrame* d_frames, u32 nbFrames, const u64* d_outOffsets, const u64* d_total,
