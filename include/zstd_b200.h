@@ -219,6 +219,15 @@ ZSTDB200_API size_t     ZSTD_decompress_usingDict(ZSTD_DCtx* dctx, void* dst, si
 /* lib/zstd.h:195-227 — header readers (host code).  ZSTD_CONTENTSIZE_UNKNOWN = (0ULL - 1), ZSTD_CONTENTSIZE_ERROR = (0ULL - 2). */
 ZSTDB200_API unsigned long long ZSTD_getFrameContentSize(const void* src, size_t srcSize);
 ZSTDB200_API size_t     ZSTD_findFrameCompressedSize(const void* src, size_t srcSize);
+/* lib/zstd.h:1437-1473 — what the frames in src[0, srcSize) decompress to, read from frame and block headers alone; both
+ * return what the reference returns for every input.  Skippable frames count 0.  Windows up to 2^31 are read, although
+ * the decoder refuses windows above 2^27; legacy (pre-v0.8) frames are not supported and give ZSTD_CONTENTSIZE_ERROR.
+ * ZSTD_findDecompressedSize: the frames' content sizes summed; ZSTD_CONTENTSIZE_UNKNOWN at the first frame that states
+ * none; ZSTD_CONTENTSIZE_ERROR for a bad frame header or block-header chain, bytes behind the last frame, or a sum past
+ * 2^64.  ZSTD_decompressBound: the same sum, with a frame that states no content size counted as its number of blocks
+ * times min(window, 128 KiB); ZSTD_CONTENTSIZE_ERROR for invalid input. */
+ZSTDB200_API unsigned long long ZSTD_findDecompressedSize(const void* src, size_t srcSize);
+ZSTDB200_API unsigned long long ZSTD_decompressBound(const void* src, size_t srcSize);
 /* lib/zstd.h:1120 — the dictionary ID a frame names (host code): 0 when it names none, for a skippable frame, and when the
  * header can not be read (too short, not a frame). */
 ZSTDB200_API unsigned   ZSTD_getDictID_fromFrame(const void* src, size_t srcSize);
@@ -394,6 +403,45 @@ ZSTDB200_API size_t ZSTDB200_decompressFramesAsync_usingDDicts(ZSTD_DCtx* dctx,
         const void* d_src, size_t srcSize, const size_t* srcOffsets, const size_t* srcSizes,
         size_t nbEntries, const ZSTD_DDict* const* ddicts,
         unsigned long long* d_dSizes, unsigned long long* d_result, void* stream);
+
+/* ZSTDB200_decompressFramesAsync with the batch's index in device memory, for a GPU reader that finds its pages' offsets and
+ * sizes in a kernel: no copy to the host and no synchronisation stand between that kernel and the decode.  The contract of
+ * ZSTDB200_decompressFramesAsync holds word for word (slots, writes, per-entry results, return value, the sticky dictionary,
+ * ordering, "no host wait once sized"), but for these points.
+ * Arrays.  d_dstOffsets, d_dstCapacities, d_srcOffsets and d_srcSizes are device (or managed) arrays of nbEntries values,
+ * 8-byte aligned; otherwise the call returns parameter_outOfBound (42) before enqueuing anything.  The call's kernels read
+ * them in stream order, so a kernel that writes them may be queued on `stream` just before the call; they must stay valid
+ * until the work ran.  No descriptor crosses PCIe and the staging ring is not used.
+ * Checks in stream order.  The checks the host form makes in its host loop (source ranges inside [0, srcSize), slots inside
+ * [0, dstCapacity), ascending and disjoint) are made on the device.  A violation makes the whole call's verdict
+ * parameter_outOfBound (42) in *d_result; nothing is then written to d_dst or d_dSizes.  Decided on the host, before
+ * enqueuing: ZSTD_error_GENERIC (1) without a device, with d_result NULL or an array NULL while nbEntries > 0;
+ * parameter_unsupported (40) for a pending prefix; stage_wrong (60) under capture on a context not sized; memory_allocation (64).
+ * Workspace.  The sum of the slots is not known on the host, so literals and sequences are sized from dstCapacity; blocks and
+ * frames as for the host form (B + nbEntries).  An entry's admission depends only on the block and frame bounds, so for the
+ * same values the bytes and results equal ZSTDB200_decompressFramesAsync's, workSpace_tooSmall (66) and dstSize_tooSmall (70)
+ * included.
+ * CUDA graphs.  A replay reads the arrays at replay time: one graph decodes whatever batch of at most nbEntries entries the
+ * arrays describe then.  Pad a smaller batch with empty entries (an entry of 0 bytes gives 0).
+ * ZSTDB200_getLastDStats fills launches: 13, the host form's 12 and the kernel that checks and packs the arrays.
+ * Per-entry DDicts and a synchronous form are not offered. */
+ZSTDB200_API size_t ZSTDB200_decompressFramesAsync_deviceOffsets(ZSTD_DCtx* dctx,
+        void* d_dst, size_t dstCapacity, const unsigned long long* d_dstOffsets, const unsigned long long* d_dstCapacities,
+        const void* d_src, size_t srcSize, const unsigned long long* d_srcOffsets, const unsigned long long* d_srcSizes,
+        size_t nbEntries, unsigned long long* d_dSizes, unsigned long long* d_result, void* stream);
+
+/* Each entry's decompressed size on the device, to size the slots of a batch without reading headers on the host:
+ * d_contentSizes[i] = ZSTD_findDecompressedSize(d_src + d_srcOffsets[i], d_srcSizes[i]) and d_bounds[i] =
+ * ZSTD_decompressBound(...) of the same range.  Either output may be NULL, not both (ZSTD_error_GENERIC).  An entry whose
+ * range lies outside [0, srcSize) gets ZSTD_CONTENTSIZE_ERROR in both; no byte outside the input is read.
+ * One kernel, one thread per entry, following the entry's frame and block headers (one dependent load per block: a 1 GiB
+ * entry of 128 KiB blocks is a chain of 8192).  The call uses none of the context's buffers (the context names the device),
+ * enqueues on `stream` (NULL: the legacy default stream) without joining the context's call order, and may be captured at
+ * any time.  Every array is 8-byte aligned, otherwise parameter_outOfBound (42) before enqueuing.  Returns 0 once enqueued;
+ * ZSTD_error_GENERIC without a device or with an input array NULL while nbEntries > 0. */
+ZSTDB200_API size_t ZSTDB200_findDecompressedSizesAsync(ZSTD_DCtx* dctx, const void* d_src, size_t srcSize,
+        const unsigned long long* d_srcOffsets, const unsigned long long* d_srcSizes, size_t nbEntries,
+        unsigned long long* d_contentSizes, unsigned long long* d_bounds, void* stream);
 
 
 /* Compress one frame whose input and output already live in device memory (HBM).  The call returns when the frame is

@@ -167,6 +167,15 @@ def lib() -> ctypes.CDLL:
             L.ZSTDB200_decompressFrames_usingDDicts.argtypes = [_vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp]
             L.ZSTDB200_decompressFramesAsync_usingDDicts.restype = _sz
             L.ZSTDB200_decompressFramesAsync_usingDDicts.argtypes = [_vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp, _vp]
+        if hasattr(L, "ZSTD_findDecompressedSize"):                                     # absent from older development builds
+            L.ZSTD_findDecompressedSize.restype = ctypes.c_ulonglong
+            L.ZSTD_findDecompressedSize.argtypes = [_vp, _sz]
+            L.ZSTD_decompressBound.restype = ctypes.c_ulonglong
+            L.ZSTD_decompressBound.argtypes = [_vp, _sz]
+            L.ZSTDB200_findDecompressedSizesAsync.restype = _sz
+            L.ZSTDB200_findDecompressedSizesAsync.argtypes = [_vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp]
+            L.ZSTDB200_decompressFramesAsync_deviceOffsets.restype = _sz
+            L.ZSTDB200_decompressFramesAsync_deviceOffsets.argtypes = [_vp, _vp, _sz, _vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp, _vp, _vp]
         L.ZSTDB200_getLastDStats.restype = None
         L.ZSTDB200_getLastDStats.argtypes = [_vp, ctypes.POINTER(DStats)]
     if hasattr(L, "ZSTD_createDDict"):                                                  # absent from older development builds
@@ -677,6 +686,24 @@ class ZSTD_DCtx:
                                                                 dds, d_d_sizes or None, d_result, stream))
         self._batch_ddicts = list(ddicts) if ddicts is not None else None     # the kernels read them after this returns
 
+    def decompress_frames_async_device_offsets(self, d_dst: int, dst_capacity: int, d_dst_offsets: int, d_dst_capacities: int,
+                                               d_src: int, src_size: int, d_src_offsets: int, d_src_sizes: int, nb_entries: int,
+                                               d_result: int, d_d_sizes: int = 0, stream: int = 0) -> None:
+        """ZSTDB200_decompressFramesAsync_deviceOffsets: decompress_frames_async with the four arrays in device memory (one
+        u64 per entry each, 8-byte aligned, e.g. int64 tensors' data_ptr()), read by the call's kernels in stream order.  An
+        array out of bounds gives parameter_outOfBound (42) in *d_result, and nothing is written to d_dst or d_d_sizes."""
+        _check(lib().ZSTDB200_decompressFramesAsync_deviceOffsets(self._h, d_dst, dst_capacity, d_dst_offsets or None,
+                                                                  d_dst_capacities or None, d_src, src_size, d_src_offsets or None,
+                                                                  d_src_sizes or None, nb_entries, d_d_sizes or None, d_result, stream))
+
+    def find_decompressed_sizes_async(self, d_src: int, src_size: int, d_src_offsets: int, d_src_sizes: int, nb_entries: int,
+                                      d_content_sizes: int = 0, d_bounds: int = 0, stream: int = 0) -> None:
+        """ZSTDB200_findDecompressedSizesAsync: for entry i = d_src[src_offsets[i], + src_sizes[i]) (device arrays of one u64
+        per entry), ZSTD_findDecompressedSize of it to d_content_sizes[i] and ZSTD_decompressBound to d_bounds[i] (0 = not
+        wanted), in stream order.  A range outside [0, src_size) gets ZSTD_CONTENTSIZE_ERROR (2**64 - 2)."""
+        _check(lib().ZSTDB200_findDecompressedSizesAsync(self._h, d_src, src_size, d_src_offsets or None, d_src_sizes or None,
+                                                         nb_entries, d_content_sizes or None, d_bounds or None, stream))
+
     def stats(self) -> DStats:
         s = DStats()
         lib().ZSTDB200_getLastDStats(self._h, ctypes.byref(s))
@@ -690,6 +717,20 @@ def ZSTD_decompress(frames, max_size: Optional[int] = None) -> bytes:
         return d.decompress(frames, max_size)
     finally:
         d.close()
+
+
+def ZSTD_findDecompressedSize(frames) -> int:
+    """lib/zstd.h:1437 — the content sizes of the frames in a host buffer summed (skippable frames count 0);
+    ZSTD_CONTENTSIZE_UNKNOWN (2**64 - 1) when a frame states none, ZSTD_CONTENTSIZE_ERROR (2**64 - 2) for invalid input."""
+    p, n, keep = _buf(frames)
+    return lib().ZSTD_findDecompressedSize(p, n)
+
+
+def ZSTD_decompressBound(frames) -> int:
+    """lib/zstd.h:1460 — an upper bound of what the frames in a host buffer decompress to, from their headers;
+    ZSTD_CONTENTSIZE_ERROR (2**64 - 2) for invalid input."""
+    p, n, keep = _buf(frames)
+    return lib().ZSTD_decompressBound(p, n)
 
 
 def ZSTD_compress(src, level: int = 3) -> bytes:

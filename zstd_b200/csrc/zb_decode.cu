@@ -105,8 +105,10 @@ __device__ __forceinline__ const ZbdDictRef* zbd_dictOf(ZbdDicts ds, const u32* 
 
 /* d_res, the call's results in device memory.  [0, 5): the walk's error, blocks, frames, literal bytes, sequences.  A
  * stream-ordered call also uses [5, 7): the blocks and frames the kernels run (0 when the walk failed or the workspace holds
- * fewer), [10, 12): D3's error and output size, [12, 15): the frames of each D5 width.  [9]: D4 / D5's error (u32). */
+ * fewer), [10, 12): D3's error and output size, [12, 15): the frames of each D5 width.  [9]: D4 / D5's error (u32).  [7]: a
+ * batch call with a device-resident index, 1 when the index check refused it. */
 #define ZBD_RES_RUN      5
+#define ZBD_RES_REFUSED  7
 #define ZBD_RES_EXEC     9
 #define ZBD_RES_SCAN     10
 #define ZBD_RES_CLASS    12
@@ -160,7 +162,46 @@ zbd_walk_kernel(const u8* __restrict__ src, u64 size, ZbdBlock* blocks, u32 capB
  * every entry its place in the call's arrays, and a fill pass that walks again and writes the descriptors there, shifted
  * into the call's coordinates.  zbd_walk is the same function as everywhere else, with the entry's dictionary. */
 #define ZBD_ENTRY_THREADS 128
-#define ZBD_ENTRY_SCAN    1024        /* the one CTA of the entry scan and of the verdict */
+#define ZBD_ENTRY_SCAN    1024        /* the one CTA of the entry scan, of the index check and of the verdict */
+
+/* Batch calls with a device-resident index (ZSTDB200_decompressFramesAsync_deviceOffsets): the checks the host form makes in
+ * its host loop, made here in stream order, and the arrays packed into the spans the count, scan and fill passes read.  One
+ * CTA, because one entry out of bounds refuses the whole call: then every span is written empty, so that nothing is walked or
+ * placed, and *refused = 1 tells the verdict. */
+__global__ void __launch_bounds__(ZBD_ENTRY_SCAN)
+zbd_entries_pack_kernel(const u64* __restrict__ srcOffsets, const u64* __restrict__ srcSizes, const u64* __restrict__ dstOffsets,
+                        const u64* __restrict__ dstCapacities, u32 nbEntries, u64 srcSize, u64 dstCapacity, ZbdSpan* __restrict__ spans,
+                        u64* __restrict__ refused)
+{
+    bool bad = false;
+    for (u32 e = threadIdx.x; e < nbEntries; e += ZBD_ENTRY_SCAN) {  /* source ranges inside the input; slots inside the output, ascending and disjoint */
+        u64 const so = srcOffsets[e], ss = srcSizes[e], dof = dstOffsets[e], dc = dstCapacities[e];
+        bad |= so > srcSize || ss > srcSize - so || dof > dstCapacity || dc > dstCapacity - dof;
+        if (e + 1u < nbEntries) bad |= dof + dc > dstOffsets[e + 1u];
+    }
+    bad = __syncthreads_or(bad);
+    for (u32 e = threadIdx.x; e < nbEntries; e += ZBD_ENTRY_SCAN) {
+        ZbdSpan s = { 0, 0, 0, 0 };
+        if (!bad) { s.srcOff = srcOffsets[e]; s.srcSize = srcSizes[e]; s.dstOff = dstOffsets[e]; s.dstCap = dstCapacities[e]; }
+        spans[e] = s;
+    }
+    if (threadIdx.x == 0) *refused = bad;
+}
+
+/* ZSTDB200_findDecompressedSizesAsync: one thread per entry, the host functions' header hop on the entry's range; a range
+ * outside the input reads nothing and gets ZBD_CONTENTSIZE_ERROR */
+#define ZBD_SIZES_THREADS 128
+__global__ void __launch_bounds__(ZBD_SIZES_THREADS)
+zbd_sizes_kernel(const u8* __restrict__ src, u64 srcSize, const u64* __restrict__ srcOffsets, const u64* __restrict__ srcSizes, u64 nbEntries,
+                 u64* __restrict__ contentSizes, u64* __restrict__ bounds)
+{
+    u64 const e = (u64)blockIdx.x * ZBD_SIZES_THREADS + threadIdx.x;
+    if (e >= nbEntries) return;
+    u64 const o = srcOffsets[e], n = srcSizes[e];
+    bool const inside = o <= srcSize && n <= srcSize - o;
+    if (contentSizes) contentSizes[e] = inside ? zbd_findDecompressedSize(src + o, n) : ZBD_CONTENTSIZE_ERROR;
+    if (bounds) bounds[e] = inside ? zbd_decompressBound(src + o, n) : ZBD_CONTENTSIZE_ERROR;
+}
 __global__ void __launch_bounds__(ZBD_ENTRY_THREADS)
 zbd_entries_count_kernel(const u8* __restrict__ src, const ZbdSpan* __restrict__ spans, ZbdEntry* __restrict__ entries, u32 nbEntries,
                          ZbdDicts dicts)
@@ -1367,12 +1408,15 @@ extern "C" size_t ZSTDB200_decompressDeviceAsync(ZSTD_DCtx* d, void* d_dst, size
 /* ------------------------------------------------------------------------------------------------ batch calls
  * ZSTDB200_decompressFrames[Async] (include/zstd_b200.h states the contract): the stream-ordered pipeline above with D0 walked
  * entry by entry and D3 .. D5 in their per-entry mode, then this verdict.  One CTA: every entry's size or error code to
- * sizes (NULL: none), and to *result the sum of the sizes, or the error code of the lowest-index entry that failed. */
+ * sizes (NULL: none), and to *result the sum of the sizes, or the error code of the lowest-index entry that failed.  A call
+ * whose device-resident index was refused (refused non-NULL and set) gets parameter_outOfBound, and sizes is not written. */
 __global__ void __launch_bounds__(ZBD_ENTRY_SCAN)
-zbd_entries_result_kernel(const ZbdEntry* __restrict__ entries, u32 nbEntries, unsigned long long* sizes, unsigned long long* result)
+zbd_entries_result_kernel(const ZbdEntry* __restrict__ entries, u32 nbEntries, unsigned long long* sizes, unsigned long long* result,
+                          const u64* __restrict__ refused)
 {
     __shared__ u32 firstBad;
     __shared__ unsigned long long total;
+    if (refused && *refused) { if (threadIdx.x == 0) *result = ZB_ERR(ZB_error_parameter_outOfBound); return; }
     if (threadIdx.x == 0) { firstBad = 0xFFFFFFFFu; total = 0; }
     __syncthreads();
     u64 sum = 0;
@@ -1401,9 +1445,11 @@ static size_t zbd_entryRef(const ZSTD_DDict* dd, int device, const ZbdDictRef** 
 }
 
 /* ownVerdict: the result and sizes go to the context's d_verdict (the synchronous call) instead of result / sizes.
- * perEntryDicts: entry i is decoded with ddicts[i] (ddicts NULL: no dictionary for any), not with the sticky dictionary */
+ * perEntryDicts: entry i is decoded with ddicts[i] (ddicts NULL: no dictionary for any), not with the sticky dictionary.
+ * deviceIndex: the four arrays are device memory; zbd_entries_pack_kernel checks them and writes the spans in stream order,
+ * instead of the host loop and the staging ring (not with perEntryDicts) */
 static size_t zbd_decompressFrames(ZSTD_DCtx* d, u8* dst, size_t dstCapacity, const size_t* dstOffsets, const size_t* dstCapacities,
-                                   const u8* src, size_t srcSize, const size_t* srcOffsets, const size_t* srcSizes, size_t n,
+                                   const u8* src, size_t srcSize, const size_t* srcOffsets, const size_t* srcSizes, size_t n, bool deviceIndex,
                                    bool perEntryDicts, const ZSTD_DDict* const* ddicts,
                                    unsigned long long* sizes, unsigned long long* result, bool ownVerdict, cudaStream_t st)
 {
@@ -1411,7 +1457,12 @@ static size_t zbd_decompressFrames(ZSTD_DCtx* d, u8* dst, size_t dstCapacity, co
     if (n && (!dstOffsets || !dstCapacities || !srcOffsets || !srcSizes)) return ZB_ERR(ZB_error_GENERIC);
     if (d->dictUses == ZBD_DICT_USE_ONCE) { zbd_clearDict(d); return ZB_ERR(ZB_error_parameter_unsupported); }   /* a prefix is forgotten */
     u64 sumCap = 0;
-    for (size_t i = 0; i < n; i++) {            /* source ranges inside the input; slots inside the output, ascending and disjoint */
+    if (deviceIndex) {                          /* the slots' sum is not known here; they lie inside the output */
+        if (((uintptr_t)dstOffsets | (uintptr_t)dstCapacities | (uintptr_t)srcOffsets | (uintptr_t)srcSizes) & 7u)
+            return ZB_ERR(ZB_error_parameter_outOfBound);
+        sumCap = dstCapacity;
+    }
+    for (size_t i = 0; !deviceIndex && i < n; i++) {    /* source ranges inside the input; slots inside the output, ascending and disjoint */
         if (srcOffsets[i] > srcSize || srcSizes[i] > srcSize - srcOffsets[i]) return ZB_ERR(ZB_error_parameter_outOfBound);
         if (dstOffsets[i] > dstCapacity || dstCapacities[i] > dstCapacity - dstOffsets[i]) return ZB_ERR(ZB_error_parameter_outOfBound);
         if (i + 1 < n && dstOffsets[i] + dstCapacities[i] > dstOffsets[i + 1]) return ZB_ERR(ZB_error_parameter_outOfBound);
@@ -1441,9 +1492,11 @@ static size_t zbd_decompressFrames(ZSTD_DCtx* d, u8* dst, size_t dstCapacity, co
         TRY(zbd_reserve(d->d_done, seqCap + 4));
         TRY(zbd_reserve(d->d_tileFirst, (dstCapacity >> ZBD_TILE_LOG) + 4));
         TRY(zbd_reserve(d->d_spans, slots)); TRY(zbd_reserve(d->d_entries, slots));
-        TRY(d->evStage.ensure(ZSTDB200_ASYNC_SLOTS, false));
-        for (u32 s = 0; s < ZSTDB200_ASYNC_SLOTS; s++)               /* every slot, so that any can serve a capture */
-            if (d->stage[s].cap < slots) { TRY(d->stage[s].ensure(slots, slots / 8 + 64)); d->stageBusy[s] = false; }
+        if (!deviceIndex) {
+            TRY(d->evStage.ensure(ZSTDB200_ASYNC_SLOTS, false));
+            for (u32 s = 0; s < ZSTDB200_ASYNC_SLOTS; s++)           /* every slot, so that any can serve a capture */
+                if (d->stage[s].cap < slots) { TRY(d->stage[s].ensure(slots, slots / 8 + 64)); d->stageBusy[s] = false; }
+        }
         if (perEntryDicts) {
             TRY(zbd_reserve(d->d_refs, slots));
             for (u32 s = 0; s < ZSTDB200_ASYNC_SLOTS; s++)
@@ -1456,18 +1509,21 @@ static size_t zbd_decompressFrames(ZSTD_DCtx* d, u8* dst, size_t dstCapacity, co
     ZbdDicts ds = zbd_oneDict(dd);
     if (ownVerdict) { result = d->d_verdict; sizes = sizes ? d->d_verdict + 1 : NULL; }
     /* the spans, into the next slot of the ring; under capture the wait needs the relaxed mode (the event was recorded outside the graph) */
-    u32 const slot = d->stageNext;
-    d->stageNext = (slot + 1u) % ZSTDB200_ASYNC_SLOTS;
-    if (d->stageBusy[slot]) {
-        cudaStreamCaptureMode m = cudaStreamCaptureModeRelaxed;
-        CK(cudaThreadExchangeStreamCaptureMode(&m));
-        cudaError_t const e = cudaEventSynchronize(d->evStage[slot]);
-        cudaThreadExchangeStreamCaptureMode(&m);
-        CK(e);
-        d->stageBusy[slot] = false;
+    u32 slot = 0;
+    if (!deviceIndex) {
+        slot = d->stageNext;
+        d->stageNext = (slot + 1u) % ZSTDB200_ASYNC_SLOTS;
+        if (d->stageBusy[slot]) {
+            cudaStreamCaptureMode m = cudaStreamCaptureModeRelaxed;
+            CK(cudaThreadExchangeStreamCaptureMode(&m));
+            cudaError_t const e = cudaEventSynchronize(d->evStage[slot]);
+            cudaThreadExchangeStreamCaptureMode(&m);
+            CK(e);
+            d->stageBusy[slot] = false;
+        }
+        ZbdSpan* const h = d->stage[slot];
+        for (size_t i = 0; i < n; i++) { h[i].srcOff = srcOffsets[i]; h[i].srcSize = srcSizes[i]; h[i].dstOff = dstOffsets[i]; h[i].dstCap = dstCapacities[i]; }
     }
-    ZbdSpan* const h = d->stage[slot];
-    for (size_t i = 0; i < n; i++) { h[i].srcOff = srcOffsets[i]; h[i].srcSize = srcSizes[i]; h[i].dstOff = dstOffsets[i]; h[i].dstCap = dstCapacities[i]; }
     if (perEntryDicts) {
         /* the entries' references, into the same slot.  A resident DDict costs one atomic read; the DDicts that are not resident
          * yet are made resident together, with one synchronisation, then every reference is taken again. */
@@ -1486,10 +1542,15 @@ static size_t zbd_decompressFrames(ZSTD_DCtx* d, u8* dst, size_t dstCapacity, co
         ds.perEntry = d->d_refs;
     }
     TRY(call.enter(st));
-    if (n) CK(cudaMemcpyAsync(d->d_spans, h, n * sizeof(ZbdSpan), cudaMemcpyHostToDevice, st));
-    if (n && perEntryDicts) CK(cudaMemcpyAsync(d->d_refs, d->stageRefs[slot], n * sizeof(const ZbdDictRef*), cudaMemcpyHostToDevice, st));
-    if (!call.capturing) { CK(cudaEventRecord(d->evStage[slot], st)); d->stageBusy[slot] = true; }
     u64* const res = d->d_res;
+    if (deviceIndex)
+        zbd_entries_pack_kernel<<<1, ZBD_ENTRY_SCAN, 0, st>>>((const u64*)srcOffsets, (const u64*)srcSizes, (const u64*)dstOffsets, (const u64*)dstCapacities,
+                                                              nbEntries, (u64)srcSize, (u64)dstCapacity, d->d_spans, res + ZBD_RES_REFUSED);
+    else {
+        if (n) CK(cudaMemcpyAsync(d->d_spans, d->stage[slot], n * sizeof(ZbdSpan), cudaMemcpyHostToDevice, st));
+        if (n && perEntryDicts) CK(cudaMemcpyAsync(d->d_refs, d->stageRefs[slot], n * sizeof(const ZbdDictRef*), cudaMemcpyHostToDevice, st));
+        if (!call.capturing) { CK(cudaEventRecord(d->evStage[slot], st)); d->stageBusy[slot] = true; }
+    }
     u32 const blockGrid = (capB + ZBD_WARPS - 1u) / ZBD_WARPS, entryGrid = (nbEntries + ZBD_ENTRY_THREADS - 1u) / ZBD_ENTRY_THREADS + (n == 0);
     auto grid = [&](int k, u32 most) { return d->grid[k] < most ? d->grid[k] : most; };
     zbd_entries_count_kernel<<<entryGrid, ZBD_ENTRY_THREADS, 0, st>>>(src, d->d_spans, d->d_entries, nbEntries, ds);
@@ -1510,10 +1571,10 @@ static size_t zbd_decompressFrames(ZSTD_DCtx* d, u8* dst, size_t dstCapacity, co
                                                                       d->d_execErr, d->d_class + capF, res, 1, d->d_frameEntry, d->d_entries);
     zbd_matches_list_kernel<32, true><<<grid(6, capF), 32, 0, st>>>(d->d_blocks, d->d_frames, d->d_seqs, d->d_matchPos, d->d_tileFirst, dst, d->d_done,
                                                                     d->d_execErr, d->d_class + 2 * (size_t)capF, res, 2, d->d_frameEntry, d->d_entries);
-    zbd_entries_result_kernel<<<1, ZBD_ENTRY_SCAN, 0, st>>>(d->d_entries, nbEntries, sizes, result);
+    zbd_entries_result_kernel<<<1, ZBD_ENTRY_SCAN, 0, st>>>(d->d_entries, nbEntries, sizes, result, deviceIndex ? res + ZBD_RES_REFUSED : NULL);
     CK(cudaGetLastError());
     TRY(call.leave(st));
-    d->stats.launches = 12;
+    d->stats.launches = deviceIndex ? 13 : 12;
     return 0;
 }
 
@@ -1522,7 +1583,7 @@ extern "C" size_t ZSTDB200_decompressFramesAsync(ZSTD_DCtx* d, void* d_dst, size
                                                  size_t nbEntries, unsigned long long* d_dSizes, unsigned long long* d_result, void* stream)
 {
     return zbd_decompressFrames(d, (u8*)d_dst, dstCapacity, dstOffsets, dstCapacities, (const u8*)d_src, srcSize, srcOffsets, srcSizes, nbEntries,
-                                false, NULL, d_dSizes, d_result, false, (cudaStream_t)stream);
+                                false, false, NULL, d_dSizes, d_result, false, (cudaStream_t)stream);
 }
 extern "C" size_t ZSTDB200_decompressFramesAsync_usingDDicts(ZSTD_DCtx* d, void* d_dst, size_t dstCapacity, const size_t* dstOffsets,
                                                              const size_t* dstCapacities, const void* d_src, size_t srcSize,
@@ -1531,7 +1592,44 @@ extern "C" size_t ZSTDB200_decompressFramesAsync_usingDDicts(ZSTD_DCtx* d, void*
                                                              unsigned long long* d_result, void* stream)
 {
     return zbd_decompressFrames(d, (u8*)d_dst, dstCapacity, dstOffsets, dstCapacities, (const u8*)d_src, srcSize, srcOffsets, srcSizes, nbEntries,
-                                true, ddicts, d_dSizes, d_result, false, (cudaStream_t)stream);
+                                false, true, ddicts, d_dSizes, d_result, false, (cudaStream_t)stream);
+}
+extern "C" size_t ZSTDB200_decompressFramesAsync_deviceOffsets(ZSTD_DCtx* d, void* d_dst, size_t dstCapacity, const unsigned long long* d_dstOffsets,
+                                                               const unsigned long long* d_dstCapacities, const void* d_src, size_t srcSize,
+                                                               const unsigned long long* d_srcOffsets, const unsigned long long* d_srcSizes,
+                                                               size_t nbEntries, unsigned long long* d_dSizes, unsigned long long* d_result, void* stream)
+{
+    static_assert(sizeof(size_t) == sizeof(unsigned long long), "the index arrays are read as size_t");
+    return zbd_decompressFrames(d, (u8*)d_dst, dstCapacity, (const size_t*)d_dstOffsets, (const size_t*)d_dstCapacities, (const u8*)d_src, srcSize,
+                                (const size_t*)d_srcOffsets, (const size_t*)d_srcSizes, nbEntries, true, false, NULL, d_dSizes, d_result, false,
+                                (cudaStream_t)stream);
+}
+
+/* One kernel on the caller's stream; no buffer of the context is used, so the call may be captured at any time and does not
+ * take part in the context's call order.  The device is chosen as zbd_ctxInit chooses it, without creating anything. */
+extern "C" size_t ZSTDB200_findDecompressedSizesAsync(ZSTD_DCtx* d, const void* d_src, size_t srcSize, const unsigned long long* d_srcOffsets,
+                                                      const unsigned long long* d_srcSizes, size_t nbEntries,
+                                                      unsigned long long* d_contentSizes, unsigned long long* d_bounds, void* stream)
+{
+    if (!d || (!d_contentSizes && !d_bounds)) return ZB_ERR(ZB_error_GENERIC);
+    if (nbEntries && (!d_srcOffsets || !d_srcSizes)) return ZB_ERR(ZB_error_GENERIC);
+    if (((uintptr_t)d_srcOffsets | (uintptr_t)d_srcSizes | (uintptr_t)d_contentSizes | (uintptr_t)d_bounds) & 7u)
+        return ZB_ERR(ZB_error_parameter_outOfBound);
+    ZbDeviceGuard guard;
+    int dev = d->device;
+    if (dev < 0) {
+        int n = 0;
+        if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) { cudaGetLastError(); return ZB_ERR(ZB_error_GENERIC); }
+        dev = d->bindDevice < 0 ? 0 : d->bindDevice;
+    }
+    CK(cudaSetDevice(dev));
+    if (nbEntries == 0) return 0;
+    u64 const grid = (nbEntries + ZBD_SIZES_THREADS - 1u) / ZBD_SIZES_THREADS;
+    if (grid > 0x7FFFFFFFull) return ZB_ERR(ZB_error_parameter_outOfBound);
+    zbd_sizes_kernel<<<(u32)grid, ZBD_SIZES_THREADS, 0, (cudaStream_t)stream>>>((const u8*)d_src, (u64)srcSize, (const u64*)d_srcOffsets,
+                                                                                (const u64*)d_srcSizes, (u64)nbEntries, (u64*)d_contentSizes, (u64*)d_bounds);
+    CK(cudaGetLastError());
+    return 0;
 }
 
 /* the stream-ordered call on the caller's stream (NULL: the context's), then one read-back of the verdict and the sizes */
@@ -1545,7 +1643,7 @@ static size_t zbd_decompressFramesSync(ZSTD_DCtx* d, void* d_dst, size_t dstCapa
     cudaStream_t const st = stream ? (cudaStream_t)stream : (cudaStream_t)d->stream;
     unsigned long long marker = 0;                                    /* non-NULL: the sizes are wanted */
     TRY(zbd_decompressFrames(d, (u8*)d_dst, dstCapacity, dstOffsets, dstCapacities, (const u8*)d_src, srcSize, srcOffsets, srcSizes, nbEntries,
-                             perEntryDicts, ddicts, dSizes ? &marker : NULL, NULL, true, st));
+                             false, perEntryDicts, ddicts, dSizes ? &marker : NULL, NULL, true, st));
     size_t const words = 1 + (dSizes ? nbEntries : 0);
     CK(cudaMemcpyAsync(d->h_verdict, d->d_verdict, words * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
@@ -1622,24 +1720,13 @@ extern "C" unsigned long long ZSTD_getFrameContentSize(const void* src, size_t s
 }
 extern "C" size_t ZSTD_findFrameCompressedSize(const void* src, size_t srcSize)
 {
-    const u8* const in = (const u8*)src;
-    ZbdFrameHeader h;
-    u32 const e = zbd_readFrameHeader(&h, in, srcSize);
-    if (e) return ZB_ERR(e);
-    if (h.skippable) return (8u + h.contentSize > srcSize) ? ZB_ERR(ZB_error_srcSize_wrong) : (size_t)(8u + h.contentSize);
-    size_t p = h.headerSize;
-    while (true) {
-        if (p + 3 > srcSize) return ZB_ERR(ZB_error_srcSize_wrong);
-        u32 const bh = zbd_le(in + p, 3);
-        u32 const type = (bh >> 1) & 3u, bsz = bh >> 3;
-        if (type == 3u) return ZB_ERR(ZBD_CORRUPT);
-        p += 3u + (type == ZB_BT_RLE ? 1u : bsz);
-        if (p > srcSize) return ZB_ERR(ZB_error_srcSize_wrong);
-        if (bh & 1u) break;
-    }
-    if (h.hasChecksum) { p += 4; if (p > srcSize) return ZB_ERR(ZB_error_srcSize_wrong); }
-    return p;
+    ZbdFrameSizeInfo fi;
+    u32 const e = zbd_frameSizeInfo(&fi, (const u8*)src, srcSize);
+    return e ? ZB_ERR(e) : (size_t)fi.cSize;
 }
+/* lib/zstd.h:1437, :1460 */
+extern "C" unsigned long long ZSTD_findDecompressedSize(const void* src, size_t srcSize) { return zbd_findDecompressedSize((const u8*)src, srcSize); }
+extern "C" unsigned long long ZSTD_decompressBound(const void* src, size_t srcSize) { return zbd_decompressBound((const u8*)src, srcSize); }
 
 /* ------------------------------------------------------------------------------------------------ streaming (lib/zstd.h:880-924)
  * The GPU decodes whole frames, so the stream front end collects compressed bytes until a frame is complete

@@ -160,6 +160,82 @@ ZBD_HDN u32 zbd_readFrameHeader(ZbdFrameHeader* h, const u8* src, u64 size)
     return ZBD_OK;
 }
 
+/* ---- one frame's sizes from its frame and block headers alone (the reference's ZSTD_findFrameSizeInfo,
+ * zstd_decompress.c:732-790): nothing behind a block header is read, no block size is checked against the window, and
+ * windows up to 2^31 are read although the decoder refuses those above 2^27. ---- */
+#define ZBD_CONTENTSIZE_ERROR 0xFFFFFFFFFFFFFFFEull
+typedef struct {
+    u64 cSize;             /* bytes of the frame incl. header and checksum */
+    u64 contentSize;       /* the header's content size (ZBD_CONTENTSIZE_UNKNOWN if absent), 0 for a skippable frame,
+                              ZBD_CONTENTSIZE_ERROR when the header cannot be read */
+    u64 bound;             /* the content size if stated, else nbBlocks x min(window, 128 KiB); 0 for a skippable frame */
+} ZbdFrameSizeInfo;
+/* returns 0 or the error code of ZSTD_findFrameCompressedSize: those of zbd_readFrameHeader, 20 for a reserved block type,
+ * 72 (srcSize_wrong) for a frame cut short.  A skippable frame that states 0xFFFFFFF8 bytes or more gets contentSize and
+ * bound ZBD_CONTENTSIZE_ERROR: the reference's 32-bit frame size wraps there and its size readers refuse the frame. */
+ZBD_HDN u32 zbd_frameSizeInfo(ZbdFrameSizeInfo* fi, const u8* src, u64 size)
+{
+    fi->cSize = 0; fi->contentSize = ZBD_CONTENTSIZE_ERROR; fi->bound = 0;
+    ZbdFrameHeader h;
+    u32 const e = zbd_readFrameHeader(&h, src, size);
+    if (e) return e;
+    if (h.skippable) {
+        bool const wraps = h.contentSize > 0xFFFFFFF7ull;
+        fi->contentSize = fi->bound = wraps ? ZBD_CONTENTSIZE_ERROR : 0u;
+        if (8u + h.contentSize > size) return 72u;
+        fi->cSize = 8u + h.contentSize;
+        return ZBD_OK;
+    }
+    fi->contentSize = h.contentSize;
+    u64 p = h.headerSize, nbBlocks = 0;
+    while (true) {
+        if (p + 3u > size) return 72u;
+        u32 const bh = zbd_le(src + p, 3);
+        u32 const type = (bh >> 1) & 3u;
+        if (type == 3u) return ZBD_CORRUPT;
+        p += 3u + (type == ZB_BT_RLE ? 1u : (bh >> 3));
+        if (p > size) return 72u;
+        nbBlocks++;
+        if (bh & 1u) break;
+    }
+    if (h.hasChecksum) { p += 4u; if (p > size) return 72u; }
+    u64 const blockMax = h.windowSize < ZB_BLOCK_MAX ? h.windowSize : ZB_BLOCK_MAX;
+    fi->cSize = p;
+    fi->bound = h.contentSize != ZBD_CONTENTSIZE_UNKNOWN ? h.contentSize : nbBlocks * blockMax;
+    return ZBD_OK;
+}
+
+/* the reference's ZSTD_findDecompressedSize (zstd_decompress.c:641-678): the content sizes of the frames in src[0, size)
+ * summed, skippable frames 0; ZBD_CONTENTSIZE_UNKNOWN at the first frame that states none; ZBD_CONTENTSIZE_ERROR for a bad
+ * header or block-header chain, trailing bytes, or a sum past 2^64 */
+ZBD_HDN u64 zbd_findDecompressedSize(const u8* src, u64 size)
+{
+    u64 total = 0;
+    while (size >= 5u) {
+        ZbdFrameSizeInfo fi;
+        u32 const e = zbd_frameSizeInfo(&fi, src, size);
+        if (fi.contentSize >= ZBD_CONTENTSIZE_ERROR) return fi.contentSize;      /* the header decides before the blocks do */
+        if (total + fi.contentSize < total) return ZBD_CONTENTSIZE_ERROR;
+        total += fi.contentSize;
+        if (e) return ZBD_CONTENTSIZE_ERROR;
+        src += fi.cSize; size -= fi.cSize;
+    }
+    return size ? ZBD_CONTENTSIZE_ERROR : total;
+}
+
+/* the reference's ZSTD_decompressBound (zstd_decompress.c:805-834): the frames' bounds summed (modulo 2^64, as there) */
+ZBD_HDN u64 zbd_decompressBound(const u8* src, u64 size)
+{
+    u64 bound = 0;
+    while (size > 0) {
+        ZbdFrameSizeInfo fi;
+        if (zbd_frameSizeInfo(&fi, src, size) || fi.bound == ZBD_CONTENTSIZE_ERROR) return ZBD_CONTENTSIZE_ERROR;
+        src += fi.cSize; size -= fi.cSize;
+        bound += fi.bound;
+    }
+    return bound;
+}
+
 /* ---- one block as the walker describes it to the kernels ---- */
 typedef struct {
     u64 srcOff;            /* first byte of the block's content (behind its 3-byte header) in the compressed input */
