@@ -1338,6 +1338,56 @@ __global__ void zbd_result_kernel(const u64* __restrict__ res, u32 capB, u32 cap
 
 static bool zbd_dictResident(const ZSTD_DDict* dd, int device) { return dd->residentOn.load(std::memory_order_acquire) == device; }
 
+/* A stream-ordered call's workspace: blocks and frames (capB, capF), literal bytes and sequences (litCap, seqCap: D1 / D2
+ * decode a block whose literals or sequences lie past them into the spare area behind, which nothing reads), and the output
+ * bytes the tile index covers (outMax).  Batch calls (batch) also need d_frameEntry. */
+struct ZbdCaps { u32 capB, capF; u64 litCap, seqCap, outMax; };
+static size_t zbd_reserveWork(ZSTD_DCtx* d, const ZbdCaps& w, bool batch)
+{
+    TRY(zbd_reserve(d->d_blocks, w.capB));
+    TRY(d->d_bout.ensure((size_t)w.capB + 1, w.capB / 8 + 64));
+    TRY(zbd_reserve(d->d_frames, w.capF));
+    if (batch) TRY(zbd_reserve(d->d_frameEntry, w.capF));
+    TRY(zbd_reserve(d->d_class, 3 * (size_t)w.capF));
+    TRY(zbd_reserve(d->d_lits, w.litCap + ZB_BLOCK_MAX + 32));
+    TRY(zbd_reserve(d->d_seqs, w.seqCap + ZBD_NBSEQ_MAX + 1));
+    TRY(zbd_reserve(d->d_matchPos, w.seqCap + 1));
+    TRY(zbd_reserve(d->d_done, w.seqCap + 4));
+    TRY(zbd_reserve(d->d_tileFirst, (w.outMax >> ZBD_TILE_LOG) + 4));
+    return 0;
+}
+
+/* D1 .. D5 of a stream-ordered call on st, behind its walk: literals, sequences, scan, clear, place and the three D5 widths,
+ * ZBD_ENQUEUE_LAUNCHES kernels, persistent grids that read their counts from the walk's words in d_res and write nothing once
+ * the walk or D3 has failed.  Batch calls (ENTRIES) run over the nbEntries entries in d_spans / d_entries / d_frameEntry.
+ * Launch errors are the caller's to collect (cudaGetLastError). */
+#define ZBD_ENQUEUE_LAUNCHES 8
+template <bool ENTRIES>
+static void zbd_enqueue(ZSTD_DCtx* d, const u8* src, u8* dst, size_t dstCapacity, const ZbdCaps& w, ZbdDicts ds, u32 nbEntries,
+                          cudaStream_t st)
+{
+    u64* const res = d->d_res;
+    u32* const frameEntry = ENTRIES ? (u32*)d->d_frameEntry : NULL;
+    ZbdEntry* const entries = ENTRIES ? (ZbdEntry*)d->d_entries : NULL;
+    const ZbdSpan* const spans = ENTRIES ? (const ZbdSpan*)d->d_spans : NULL;
+    u32 const blockGrid = (w.capB + ZBD_WARPS - 1u) / ZBD_WARPS;
+    auto grid = [&](int k, u32 most) { return d->grid[k] < most ? d->grid[k] : most; };
+    zbd_literals_kernel<true><<<grid(0, blockGrid), 32 * ZBD_WARPS, 0, st>>>(src, d->d_blocks, w.capB, d->d_lits, d->d_bout, ds, frameEntry, res, w.litCap);
+    zbd_sequences_kernel<true><<<grid(1, blockGrid), 32 * ZBD_WARPS, 0, st>>>(src, d->d_blocks, w.capB, d->d_seqs, d->d_bout, ds, frameEntry, res, w.seqCap);
+    zbd_scan_kernel<ENTRIES><<<1, SCAN_THREADS, 0, st>>>(d->d_blocks, w.capB, d->d_frames, w.capF, d->d_bout, (u64)dstCapacity, res + ZBD_RES_SCAN, ds, res,
+                                                         d->d_class, w.capF, spans, entries, frameEntry, nbEntries);
+    zbd_clear_kernel<<<grid(3, (u32)(w.seqCap / 256u) + 1u), 256, 0, st>>>(res, d->d_tileFirst, d->d_done);
+    zbd_place_kernel<true, ENTRIES><<<grid(2, blockGrid), 32 * ZBD_WARPS, 0, st>>>(src, d->d_blocks, w.capB, d->d_lits, d->d_seqs, d->d_matchPos, d->d_tileFirst,
+                                                                                   d->d_bout, dst, ds, d->d_execErr, res, frameEntry, entries);
+    u32* const list = d->d_class;
+    zbd_matches_list_kernel<1024, ENTRIES><<<grid(4, w.capF), 1024, 0, st>>>(d->d_blocks, d->d_frames, d->d_seqs, d->d_matchPos, d->d_tileFirst, dst,
+                                                                             d->d_done, d->d_execErr, list, res, 0, frameEntry, entries);
+    zbd_matches_list_kernel<128, ENTRIES><<<grid(5, w.capF), 128, 0, st>>>(d->d_blocks, d->d_frames, d->d_seqs, d->d_matchPos, d->d_tileFirst, dst,
+                                                                           d->d_done, d->d_execErr, list + w.capF, res, 1, frameEntry, entries);
+    zbd_matches_list_kernel<32, ENTRIES><<<grid(6, w.capF), 32, 0, st>>>(d->d_blocks, d->d_frames, d->d_seqs, d->d_matchPos, d->d_tileFirst, dst,
+                                                                         d->d_done, d->d_execErr, list + 2 * (size_t)w.capF, res, 2, frameEntry, entries);
+}
+
 /* D0 .. D5 and the verdict enqueued on the caller's stream, with the context's sticky dictionary, under ZbOrder's rule; a DDict's
  * first upload on the device (on the context's stream, which synchronises) is refused under capture too */
 static size_t zbd_decompressAsync(ZSTD_DCtx* d, void* dst, size_t dstCapacity, const void* src, size_t srcSize,
@@ -1355,47 +1405,19 @@ static size_t zbd_decompressAsync(ZSTD_DCtx* d, void* dst, size_t dstCapacity, c
     if (dd && call.capturing && !zbd_dictResident(dd, d->device)) return ZB_ERR(ZB_error_stage_wrong);
     u64 const cap = zbd_asyncBlocks(srcSize, dstCapacity);
     if (cap > 0x7FFFFFFFull) return ZB_ERR(ZB_error_memory_allocation);
-    u32 const capB = (u32)cap, capF = (u32)cap;
-    u64 const litCap = (u64)dstCapacity + 16u * cap, seqCap = (u64)dstCapacity / 3u;
-    TRY(call.size([&]() -> size_t {
-        TRY(zbd_reserve(d->d_blocks, capB));
-        TRY(d->d_bout.ensure((size_t)capB + 1, capB / 8 + 64));
-        TRY(zbd_reserve(d->d_frames, capF));
-        TRY(zbd_reserve(d->d_class, 3 * (size_t)capF));
-        TRY(zbd_reserve(d->d_lits, litCap + ZB_BLOCK_MAX + 32));
-        TRY(zbd_reserve(d->d_seqs, seqCap + ZBD_NBSEQ_MAX + 1));
-        TRY(zbd_reserve(d->d_matchPos, seqCap + 1));
-        TRY(zbd_reserve(d->d_done, seqCap + 4));
-        TRY(zbd_reserve(d->d_tileFirst, (dstCapacity >> ZBD_TILE_LOG) + 4));
-        return 0;
-    }));
+    ZbdCaps const w = { (u32)cap, (u32)cap, (u64)dstCapacity + 16u * cap, (u64)dstCapacity / 3u, (u64)dstCapacity };
+    TRY(call.size([&]() { return zbd_reserveWork(d, w, false); }));
     if (dd) TRY(zbd_residentDict(dd, d->device, d->stream));           /* no copy once resident */
     ZbdDictInfo const di = zbd_dictInfo(dd);
-    ZbdDicts const ds = zbd_oneDict(dd);
     TRY(call.enter(st));
     const u8* const in = (const u8*)src;
-    u64* const res = d->d_res;
-    u32 const blockGrid = (capB + ZBD_WARPS - 1u) / ZBD_WARPS;
-    auto grid = [&](int k, u32 most) { return d->grid[k] < most ? d->grid[k] : most; };
     CK(cudaMemsetAsync(d->d_execErr, 0, sizeof(u32), st));
-    zbd_walk_kernel<<<1, ZBD_WALK_THREADS, 0, st>>>(in, (u64)srcSize, d->d_blocks, capB, d->d_frames, capF, res, di.entropy, di.dictID);
-    zbd_literals_kernel<true><<<grid(0, blockGrid), 32 * ZBD_WARPS, 0, st>>>(in, d->d_blocks, capB, d->d_lits, d->d_bout, ds, NULL, res, litCap);
-    zbd_sequences_kernel<true><<<grid(1, blockGrid), 32 * ZBD_WARPS, 0, st>>>(in, d->d_blocks, capB, d->d_seqs, d->d_bout, ds, NULL, res, seqCap);
-    zbd_scan_kernel<false><<<1, SCAN_THREADS, 0, st>>>(d->d_blocks, capB, d->d_frames, capF, d->d_bout, (u64)dstCapacity, res + ZBD_RES_SCAN, ds, res,
-                                                       d->d_class, capF, NULL, NULL, NULL, 0);
-    zbd_clear_kernel<<<grid(3, (u32)(seqCap / 256u) + 1u), 256, 0, st>>>(res, d->d_tileFirst, d->d_done);
-    zbd_place_kernel<true, false><<<grid(2, blockGrid), 32 * ZBD_WARPS, 0, st>>>(in, d->d_blocks, capB, d->d_lits, d->d_seqs, d->d_matchPos, d->d_tileFirst, d->d_bout,
-                                                                           (u8*)dst, ds, d->d_execErr, res, NULL, NULL);
-    zbd_matches_list_kernel<1024, false><<<grid(4, capF), 1024, 0, st>>>(d->d_blocks, d->d_frames, d->d_seqs, d->d_matchPos, d->d_tileFirst, (u8*)dst, d->d_done,
-                                                            d->d_execErr, d->d_class, res, 0, NULL, NULL);
-    zbd_matches_list_kernel<128, false><<<grid(5, capF), 128, 0, st>>>(d->d_blocks, d->d_frames, d->d_seqs, d->d_matchPos, d->d_tileFirst, (u8*)dst, d->d_done,
-                                                          d->d_execErr, d->d_class + capF, res, 1, NULL, NULL);
-    zbd_matches_list_kernel<32, false><<<grid(6, capF), 32, 0, st>>>(d->d_blocks, d->d_frames, d->d_seqs, d->d_matchPos, d->d_tileFirst, (u8*)dst, d->d_done,
-                                                        d->d_execErr, d->d_class + 2 * (size_t)capF, res, 2, NULL, NULL);
-    zbd_result_kernel<<<1, 1, 0, st>>>(res, capB, capF, result);
+    zbd_walk_kernel<<<1, ZBD_WALK_THREADS, 0, st>>>(in, (u64)srcSize, d->d_blocks, w.capB, d->d_frames, w.capF, d->d_res, di.entropy, di.dictID);
+    zbd_enqueue<false>(d, in, (u8*)dst, dstCapacity, w, zbd_oneDict(dd), 0, st);
+    zbd_result_kernel<<<1, 1, 0, st>>>(d->d_res, w.capB, w.capF, result);
     CK(cudaGetLastError());
     TRY(call.leave(st));
-    d->stats.launches = 10;
+    d->stats.launches = ZBD_ENQUEUE_LAUNCHES + 2;                     /* and the walk and the verdict */
     return 0;
 }
 
@@ -1479,18 +1501,10 @@ static size_t zbd_decompressFrames(ZSTD_DCtx* d, u8* dst, size_t dstCapacity, co
     u64 const cap = zbd_asyncBlocks(srcSize, dstCapacity) + (u64)n;
     if (cap > 0x7FFFFFFFull) return ZB_ERR(ZB_error_memory_allocation);
     u32 const capB = (u32)cap, capF = (u32)cap, nbEntries = (u32)n;
-    u64 const litCap = sumCap + 32u * cap, seqCap = sumCap / 3u;      /* the entries' shares (zbd_entries_scan_kernel) fit */
+    ZbdCaps const w = { capB, capF, sumCap + 32u * cap, sumCap / 3u, (u64)dstCapacity };   /* the entries' shares (zbd_entries_scan_kernel) fit */
     size_t const slots = n ? n : 1;
     TRY(call.size([&]() -> size_t {
-        TRY(zbd_reserve(d->d_blocks, capB));
-        TRY(d->d_bout.ensure((size_t)capB + 1, capB / 8 + 64));
-        TRY(zbd_reserve(d->d_frames, capF)); TRY(zbd_reserve(d->d_frameEntry, capF));
-        TRY(zbd_reserve(d->d_class, 3 * (size_t)capF));
-        TRY(zbd_reserve(d->d_lits, litCap + ZB_BLOCK_MAX + 32));
-        TRY(zbd_reserve(d->d_seqs, seqCap + ZBD_NBSEQ_MAX + 1));
-        TRY(zbd_reserve(d->d_matchPos, seqCap + 1));
-        TRY(zbd_reserve(d->d_done, seqCap + 4));
-        TRY(zbd_reserve(d->d_tileFirst, (dstCapacity >> ZBD_TILE_LOG) + 4));
+        TRY(zbd_reserveWork(d, w, true));
         TRY(zbd_reserve(d->d_spans, slots)); TRY(zbd_reserve(d->d_entries, slots));
         if (!deviceIndex) {
             TRY(d->evStage.ensure(ZSTDB200_ASYNC_SLOTS, false));
@@ -1551,30 +1565,16 @@ static size_t zbd_decompressFrames(ZSTD_DCtx* d, u8* dst, size_t dstCapacity, co
         if (n && perEntryDicts) CK(cudaMemcpyAsync(d->d_refs, d->stageRefs[slot], n * sizeof(const ZbdDictRef*), cudaMemcpyHostToDevice, st));
         if (!call.capturing) { CK(cudaEventRecord(d->evStage[slot], st)); d->stageBusy[slot] = true; }
     }
-    u32 const blockGrid = (capB + ZBD_WARPS - 1u) / ZBD_WARPS, entryGrid = (nbEntries + ZBD_ENTRY_THREADS - 1u) / ZBD_ENTRY_THREADS + (n == 0);
-    auto grid = [&](int k, u32 most) { return d->grid[k] < most ? d->grid[k] : most; };
+    u32 const entryGrid = (nbEntries + ZBD_ENTRY_THREADS - 1u) / ZBD_ENTRY_THREADS + (n == 0);
     zbd_entries_count_kernel<<<entryGrid, ZBD_ENTRY_THREADS, 0, st>>>(src, d->d_spans, d->d_entries, nbEntries, ds);
     zbd_entries_scan_kernel<<<1, ZBD_ENTRY_SCAN, 0, st>>>(d->d_spans, d->d_entries, nbEntries, capB, capF, res);
     zbd_entries_fill_kernel<<<entryGrid, ZBD_ENTRY_THREADS, 0, st>>>(src, d->d_spans, d->d_entries, nbEntries, d->d_blocks, d->d_frames, d->d_frameEntry,
-                                                                     ds, litCap, seqCap);
-    zbd_literals_kernel<true><<<grid(0, blockGrid), 32 * ZBD_WARPS, 0, st>>>(src, d->d_blocks, capB, d->d_lits, d->d_bout, ds, d->d_frameEntry, res, litCap);
-    zbd_sequences_kernel<true><<<grid(1, blockGrid), 32 * ZBD_WARPS, 0, st>>>(src, d->d_blocks, capB, d->d_seqs, d->d_bout, ds, d->d_frameEntry, res, seqCap);
-    zbd_scan_kernel<true><<<1, SCAN_THREADS, 0, st>>>(d->d_blocks, capB, d->d_frames, capF, d->d_bout, (u64)dstCapacity, res + ZBD_RES_SCAN, ds, res,
-                                                      d->d_class, capF, d->d_spans, d->d_entries, d->d_frameEntry, nbEntries);
-    zbd_clear_kernel<<<grid(3, (u32)(seqCap / 256u) + 1u), 256, 0, st>>>(res, d->d_tileFirst, d->d_done);
-    zbd_place_kernel<true, true><<<grid(2, blockGrid), 32 * ZBD_WARPS, 0, st>>>(src, d->d_blocks, capB, d->d_lits, d->d_seqs, d->d_matchPos, d->d_tileFirst,
-                                                                              d->d_bout, dst, ds, d->d_execErr, res, d->d_frameEntry,
-                                                                              d->d_entries);
-    zbd_matches_list_kernel<1024, true><<<grid(4, capF), 1024, 0, st>>>(d->d_blocks, d->d_frames, d->d_seqs, d->d_matchPos, d->d_tileFirst, dst, d->d_done,
-                                                                        d->d_execErr, d->d_class, res, 0, d->d_frameEntry, d->d_entries);
-    zbd_matches_list_kernel<128, true><<<grid(5, capF), 128, 0, st>>>(d->d_blocks, d->d_frames, d->d_seqs, d->d_matchPos, d->d_tileFirst, dst, d->d_done,
-                                                                      d->d_execErr, d->d_class + capF, res, 1, d->d_frameEntry, d->d_entries);
-    zbd_matches_list_kernel<32, true><<<grid(6, capF), 32, 0, st>>>(d->d_blocks, d->d_frames, d->d_seqs, d->d_matchPos, d->d_tileFirst, dst, d->d_done,
-                                                                    d->d_execErr, d->d_class + 2 * (size_t)capF, res, 2, d->d_frameEntry, d->d_entries);
+                                                                     ds, w.litCap, w.seqCap);
+    zbd_enqueue<true>(d, src, dst, dstCapacity, w, ds, nbEntries, st);
     zbd_entries_result_kernel<<<1, ZBD_ENTRY_SCAN, 0, st>>>(d->d_entries, nbEntries, sizes, result, deviceIndex ? res + ZBD_RES_REFUSED : NULL);
     CK(cudaGetLastError());
     TRY(call.leave(st));
-    d->stats.launches = deviceIndex ? 13 : 12;
+    d->stats.launches = ZBD_ENQUEUE_LAUNCHES + (deviceIndex ? 5 : 4);   /* and count, scan, fill, the verdict, the index check */
     return 0;
 }
 
